@@ -1,4 +1,4 @@
-"""arroyo_b200: B200-native (sm_100a) window-assign / keyed-aggregate / windowed-join operators behind
+"""arroyo_b200: H100-native (sm_90a) window-assign / keyed-aggregate / windowed-join operators behind
 Arroyo's ArrowOperator surface.  The compute lives in libarroyo_b200.so (hand-written CUDA behind a C ABI,
 include/arroyo_b200.h); this package is the Python host-side mirror of the reference's operator interface
 (arroyo-operator/src/operator.rs:1143-1257, context.rs) used by the tests and the benchmark.

@@ -1,5 +1,5 @@
-"""Builds libarroyo_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the
-repo snapshot to the GPU box)."""
+"""Builds libarroyo_b200.so in-tree with nvcc for sm_90a (H100): no JIT cache, the library sits beside the package
+and is loaded from the source tree."""
 import os
 import shutil
 import subprocess
@@ -9,6 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libarroyo_b200.so")
 SOURCES = ["abi.cu", "window_agg.cu", "shuffle.cu", "join.cu", "session.cu", "updating_agg.cu", "ttl_join.cu"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
 HEADERS = ["common.cuh", "dict.cuh", "bdict.cuh", "ingest_two_pass.cuh", "scan.cuh", "planner.h", "arrow_io.h", "op.h", os.path.join("..", "..", "include", "arroyo_b200.h")]
 
 
@@ -34,7 +35,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB
     objs = []
     flags = [
-        "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+        *GENCODE, "-O3", "-std=c++17", "-lineinfo",
         "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr",
     ]
     if verbose:
@@ -61,7 +62,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if failed:
         raise RuntimeError("nvcc compilation failed")
     tmp = LIB + ".tmp"  # link beside the target, then rename: a reader never sees a half-written library
-    cmd = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", tmp, *objs, "-lcudart"]
+    cmd = [nvcc_path(), *GENCODE, "-shared", "-o", tmp, *objs, "-lcudart"]
     subprocess.check_call(cmd)
     os.replace(tmp, LIB)
     return LIB

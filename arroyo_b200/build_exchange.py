@@ -31,7 +31,7 @@ def build(force: bool = False):
     if not force and os.path.exists(LIB) and all(os.path.getmtime(LIB) >= os.path.getmtime(d) for d in deps):
         return LIB
     tmp = LIB + ".tmp"
-    cmd = [main_build.nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    cmd = [main_build.nvcc_path(), *main_build.GENCODE, "-O3", "-std=c++17", "-lineinfo",
            "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr", "-I" + inc, "-shared", "-o", tmp, SRC,
            "-L" + HERE, "-l:" + os.path.basename(main_lib), "-L" + os.path.dirname(lib), "-l:" + os.path.basename(lib),
            "-Xlinker", "-rpath=$ORIGIN", "-Xlinker", "-rpath=" + os.path.dirname(lib), "-lcudart"]

@@ -149,8 +149,8 @@ static __device__ __forceinline__ uint32_t dict_lookup_or_insert(const DictView&
 }
 
 // slot count: 3.5 x ids => load factor 0.25 at the expected key count (0.29 when every id is used).
-// Measured (profiles/r01_probe2.txt): the random 16-byte probe runs at 92 G/s at load 0.25 vs 72 G/s at
-// 0.5 -- shorter chains mean fewer divergent replays per warp.  ARROYO_B200_DICT_QUARTER_SLOTS_PER_ID
+// The random 16-byte probe is faster at load 0.25 than at 0.5: shorter chains mean fewer divergent replays per
+// warp.  ARROYO_B200_DICT_QUARTER_SLOTS_PER_ID
 // (default 14 = 3.5 slots per id) trades chain length against L2 footprint for experiments.
 inline uint64_t dict_slots_for(uint64_t ids) {
   static const uint64_t q = [] {

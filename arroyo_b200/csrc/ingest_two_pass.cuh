@@ -2,10 +2,9 @@
 // (Included by window_agg.cu inside its anonymous namespace, after IngestParams / slow_row.)
 //
 // Why: the direct kernel (ingest_kernel) pays one scattered 16-byte probe and one scattered RED per accumulator for
-// every row, and a scattered access costs ~2 SM-cycles per *lane* in the LSU wherever its line lives (probe + 2 REDs
-// = 6.7 cycles per row, 43 G rows/s; profiles/r01_*).
-// What is cheap on this chip is shared memory: a random LDS.128 costs 8.5 SM-cycles per WARP instruction and a 32-bit
-// shared-memory atomic 3.5 (profiles/r02_probe5_primitives.txt) -- twenty times less per row than the global path.
+// every row, and a scattered global access costs SM-cycles per *lane* in the LSU wherever its line lives.
+// What is cheap is shared memory: a random shared load or 32-bit shared-memory atomic costs a few SM-cycles per WARP
+// instruction (tools/probe5.cu measures both) -- far less per row than the global path.
 // So rows are first brought together by key range, then aggregated in shared memory:
 //
 //   pass 1  part_kernel   every block takes tiles of 4096 rows: window-assign (pane = ts / slide), late / guard tests,
@@ -115,7 +114,7 @@ __device__ __noinline__ void off_path_row(const IngestParams& p, long long key, 
 // pass 1
 // ---------------------------------------------------------------------------------------------------------------
 // Shared-memory atomics rank the tile: ATOMS.ADD with return costs ~3.5 SM-cycles per warp instruction on spread
-// addresses (0.11 per lane; MATCH.ANY, the atomic-free alternative, costs 62: profiles/r02_probe5_primitives.txt).
+// addresses; MATCH.ANY, the atomic-free alternative, costs many times more (tools/probe5.cu).
 template <int NV, int SIG>
 __global__ void __launch_bounds__(P1_THREADS, P1_BLOCKS_PER_SM) part_kernel(const __grid_constant__ IngestParams p,
                                                                             const __grid_constant__ TwoPassParams tp) {
@@ -361,11 +360,11 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 // 8-byte load (the eight tags of its home group), a SIMD compare, and -- for the slot whose tag matches -- one 8-byte
 // load to confirm the key and one 2-byte load for the index: straight-line, ~25 instructions.  (With a probe loop every
 // warp has some lane that needs another round -- it was three quarters of the kernel's instructions -- and comparing
-// eight full keys costs four 16-byte loads and sixteen compares per row: profiles/r02_two_pass_c .. _f.)  At a
+// eight full keys costs four 16-byte loads and sixteen compares per row.)  At a
 // quarter load a group overflows once in ten thousand keys; those and first sightings take the slow path.
-// The bucket's accumulators live once in shared memory and take shared-memory atomics (ATOMS.ADD.32: ~3.5 SM-cycles
+// The bucket's accumulators live once in shared memory and take shared-memory atomics (ATOMS.ADD.32: a few SM-cycles
 // per warp instruction on spread addresses, duplicates inside a warp included).  The shared-memory data pipe is what
-// bounds this kernel (72 % busy in profiles/r02_two_pass_h), so a row costs two atomics, not three: the 64-bit wrapping
+// bounds this kernel, so a row costs two atomics, not three: the 64-bit wrapping
 // SUM's low word takes every row's low half (the returned old value tells whether it wrapped); that carry -- minus one
 // for a negative row, whose high word is all ones -- rides in the high 16 bits of the key's row-count word, which is
 // flushed before either half can reach 2^15.  Only values that are not sign-extended 32-bit numbers add their high

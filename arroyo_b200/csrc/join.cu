@@ -1,4 +1,4 @@
-// Instant (windowed) join on sm_100a.
+// Instant (windowed) join on sm_90a (H100).
 //
 // Replaces InstantJoin (arroyo-worker/src/arrow/instant_join.rs:109-172 process_side, :241-283
 // process_batch_index / handle_watermark) and the DataFusion HashJoinExec it runs once per window instant
@@ -245,7 +245,7 @@ class InstantJoinOp final : public OpBase {
   int device_;
   cudaStream_t stream_ = nullptr;
   bool own_stream_ = false;
-  int num_sms_ = 148;
+  int num_sms_ = 132;  // set from the device at creation
   int join_type_;
   Side side_[2];
   int64_t last_wm_ = INT64_MIN;

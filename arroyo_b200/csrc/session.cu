@@ -1,4 +1,4 @@
-// Session window aggregate on sm_100a.
+// Session window aggregate on sm_90a (H100).
 //
 // Replaces SessionAggregatingWindowFunc (arroyo-worker/src/arrow/session_aggregating_window.rs:60-279 operator,
 // :397-523 ActiveSession, :533-691 KeyComputingHolder, :850-895 process_batch) and the arrow-rs / DataFusion work
@@ -610,7 +610,7 @@ class SessionOp final : public OpBase {
   int device_;
   cudaStream_t stream_ = nullptr;
   bool own_stream_ = false;
-  int num_sms_ = 148;
+  int num_sms_ = 132;  // set from the device at creation
   bool keyed_;
   int key_col_, ts_col_;
   int64_t gap_;

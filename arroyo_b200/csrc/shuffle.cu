@@ -1,4 +1,4 @@
-// Key-hash shuffle partitioner on sm_100a: the device half of the Shuffle edge.
+// Key-hash shuffle partitioner on sm_90a (H100): the device half of the Shuffle edge.
 //
 // Replaces ArrowCollector::collect -> repartition (arroyo-operator/src/context.rs:506-541) and
 // server_for_hash_array (arroyo-operator/src/lib.rs:30-41): hash the routing key, dest =
@@ -169,15 +169,17 @@ int32_t arroyo_b200_ts_minmax(int32_t device, uint64_t stream, uint64_t ts_dev, 
     AB_CUDA(cudaSetDevice(device));
     static thread_local long long* d_out = nullptr;
     static thread_local int d_dev = -1;
+    static thread_local int d_sms = 0;
     if (!d_out || d_dev != device) {
       AB_CUDA(cudaMalloc(&d_out, 2 * sizeof(long long)));
+      AB_CUDA(cudaDeviceGetAttribute(&d_sms, cudaDevAttrMultiProcessorCount, device));
       d_dev = device;
     }
     cudaStream_t st = (cudaStream_t)stream;
     const long long init[2] = {LLONG_MAX, LLONG_MIN};
     AB_CUDA(cudaMemcpyAsync(d_out, init, sizeof init, cudaMemcpyHostToDevice, st));
     if (n_rows > 0) {
-      int grid = (int)std::min<int64_t>((n_rows + 255) / 256, 148 * 8);
+      int grid = (int)std::min<int64_t>((n_rows + 255) / 256, (int64_t)d_sms * 8);
       minmax_kernel<<<grid, 256, 0, st>>>((const long long*)ts_dev, n_rows, d_out);
       AB_CUDA(cudaGetLastError());
     }

@@ -1,4 +1,4 @@
-// Non-windowed join with expiration on sm_100a: the GPU side of `JoinWithExpiration`
+// Non-windowed join with expiration on sm_90a (H100): the GPU side of `JoinWithExpiration`
 // (arroyo-worker/src/arrow/join_with_expiration.rs:42-130), SURVEY.md 8(f) rank 3.  Inner joins of append-only inputs.
 //
 // The reference keeps each side's rows in a key-time table (`KeyTimeView`, arroyo-state/src/tables/
@@ -170,7 +170,7 @@ class TtlJoinOp final : public OpBase {
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
   bool own_stream_ = false;
-  int num_sms_ = 148;
+  int num_sms_ = 132;  // set from the device at creation
   TSide side_[2];
   DevBuf cnt_, off_, total_, sums_, pair_new_, pair_old_, out_ts_;
   std::vector<DevBuf> out_cols_;

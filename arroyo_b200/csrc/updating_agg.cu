@@ -1,4 +1,4 @@
-// Updating (non-windowed) keyed aggregate on sm_100a: the GPU side of `IncrementalAggregatingFunc`
+// Updating (non-windowed) keyed aggregate on sm_90a (H100): the GPU side of `IncrementalAggregatingFunc`
 // (arroyo-worker/src/arrow/incremental_aggregator.rs), SURVEY.md 8(f) rank 2.
 //
 // The reference keeps one accumulator object per key and aggregate, updates them ONE ROW AT A TIME through dyn
@@ -215,7 +215,7 @@ class UpdatingAggOp final : public OpBase {
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
   bool own_stream_ = false;
-  int num_sms_ = 148;
+  int num_sms_ = 132;  // set from the device at creation
   bool keyed_ = false;
   int key_col_ = 0, ts_col_ = 0;
   int n_vals_ = 0, val_cols_[4];

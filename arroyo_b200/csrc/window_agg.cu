@@ -1,4 +1,4 @@
-// Tumbling / sliding window keyed aggregate on sm_100a.
+// Tumbling / sliding window keyed aggregate on sm_90a (H100).
 //
 // Replaces, behind the ArrowOperator surface:
 //   TumblingAggregatingWindowFunc  arroyo-worker/src/arrow/tumbling_aggregating_window.rs:250-392
@@ -437,7 +437,7 @@ __global__ void __launch_bounds__(THREADS, AB_INGEST_MIN_BLOCKS) ingest_kernel(c
 
     // One row per lane per iteration: a warp instruction covers 256 contiguous bytes per column, and
     // with several resident blocks per SM there are well over a thousand independent probe chains in
-    // flight per SM (profiles/r01_probe2.txt: occupancy beats rows-per-thread for the scattered part).
+    // flight per SM (occupancy, not rows per thread, is what keeps the scattered part busy).
     // The next row's columns are requested before the current row is processed, so the streaming loads
     // overlap the dependent probe -> RED chain.  The trip count is uniform so that the warp votes below
     // stay convergent in tail tiles.
@@ -884,7 +884,7 @@ class WindowAggOp final : public OpBase {
   int device_;
   cudaStream_t stream_ = nullptr;
   bool own_stream_ = false;
-  int num_sms_ = 148;
+  int num_sms_ = 132;  // set from the device at creation
 
   // dictionary (bdict.cuh): n_buckets_ buckets of BD_KS slots; ids = BD_ID_BASE + bucket * BD_CAPB + index
   uint64_t id_cap_ = 0;
@@ -1567,8 +1567,8 @@ void WindowAggOp::upload_ring() {
 }
 
 // Host->device copies of the input columns are submitted in groups with cudaMemcpyBatchAsync: a 64 Ki-row batch is
-// three 512 KiB copies, and one cudaMemcpyAsync per copy tops out at 39 GB/s on this box's Gen5 x16 link where
-// groups of 48 reach 55 GB/s (profiles/r01_pcie_probe2.txt) -- and cost a tenth of the host time.
+// three 512 KiB copies, and one cudaMemcpyAsync per copy leaves a PCIe Gen5 x16 link well short of what grouped
+// submissions reach -- and costs far more host time per copy.
 void WindowAggOp::queue_copy(void* dst, const void* src, size_t bytes) {
   if (bytes == 0) return;
   copy_dst_.push_back(dst);
@@ -1698,8 +1698,8 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
     }
   }
   // ARROYO_B200_FLAG_ZERO_COPY: pinned (page-locked, device-mapped) Arrow buffers are read in place by the
-  // ingest kernel over PCIe: no staging memory.  Measured slower than DMA staging on this pool's hosts
-  // (0.96 vs 1.22 G rows/s end to end: SM loads over PCIe ~23 GB/s vs copy engine ~29 GB/s), hence opt-in.
+  // ingest kernel over PCIe: no staging memory.  SM loads over PCIe move less than the copy engines do, so this
+  // is slower than DMA staging end to end, hence opt-in.
   if (n > 0 && (cfg.flags & ARROYO_B200_FLAG_ZERO_COPY)) {
     bool pinned = true;
     const uint64_t* devp[ARROYO_B200_MAX_COLS] = {nullptr};

@@ -888,7 +888,6 @@ def bench(args, torch, dist, rank, world, local, all_cpus=None):
 
     if rank == 0:
         peak, peak_kind = B.measured_peak()
-        traffic = B.ncu_traffic()
         ingest_gbs = 24.0 * d["ingest_rows_timed"] / (d["ingest_ms"] * 1e-3) / 1e9 if d["ingest_ms"] else None
         out = {"metric": "rows/sec sliding-window SUM (1M keys)", "value": world * K * rows / (ms * 1e-3),
                "unit": "rows/s", "n_gpus": world, "steps": K, "warmup": W, "warmup_requested": args.warmup,
@@ -908,13 +907,11 @@ def bench(args, torch, dist, rank, world, local, all_cpus=None):
                         "local stage closes panes 2 rounds behind (LaggedCombiner)" if res["pipelined"] else
                         "synchronous: watermark exchange, local close, shuffle, owner stage in sequence"),
                "rows_out_per_step": res["rows_out"] / max(K, 1), "gpu_launches": res["launches"],
-               "roofline": {"bound": "hbm", "kernel": (traffic or {}).get("kernel", "ingest"),
+               "roofline": {"bound": "hbm", "kernel": "ingest",
                             "achieved": round(ingest_gbs, 1) if ingest_gbs else None, "peak": peak,
                             "peak_kind": peak_kind, "unit": "GB/s",
                             "frac": round(ingest_gbs / peak, 4) if ingest_gbs else None,
-                            "traffic": (round(traffic["dram_bytes_per_row"] * d["ingest_rows_timed"] /
-                                              max(d["ingest_launches"], 1))
-                                        if traffic and traffic.get("dram_bytes_per_row") else None),
+                            "traffic": None,
                             "algorithmic_bytes_per_launch": 24.0 * d["ingest_rows_timed"] / max(d["ingest_launches"], 1),
                             "note": "rank 0's raw-row ingest kernel"},
                "host_ms_per_step": res["host_ms_per_step"], "owner_stage_kernel_ms_per_step": res["owner_ms"],

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- rows/sec of the sliding-window SUM/AVG hot path (BASELINE.json config 3) on N B200s.
+"""bench.py -- rows/sec of the sliding-window SUM/AVG hot path (BASELINE.json config 3) on N H100s.
 
 Workload (`config.workload`): hop(1 s slide, 10 s width) SUM(value), AVG(value), COUNT(*) GROUP BY key,
 1 048 576 distinct i64 keys (uniform), Arrow-shaped batches of 65 536 rows [key i64, value i64,
@@ -15,7 +15,7 @@ one 10-s window (<= 1 Mi rows x 6 columns).
             arroyo_b200_op_process_batch, emitted windows out as host Arrow batches
   roofline  the ingest (window-assign + partial aggregate: part_kernel + agg_kernel per launch): 24 algorithmic
             bytes per input row / the CUDA-event time of the step's ingest launches, against the measured HBM
-            copy bandwidth (MEASURED_PEAKS.json); `traffic` = DRAM bytes from the committed ncu capture
+            copy bandwidth (MEASURED_PEAKS.json) or, without it, the H100 SXM data sheet's 3.35 TB/s
   verified  the windows of a second, identical pass over the panes the CPU baseline consumed equal the C
             oracle's, checksum by checksum (rows out, sum COUNT, wrapping sum SUM bit-exact; sum AVG 1e-6);
             a mismatch makes the script exit non-zero
@@ -28,6 +28,13 @@ pre-aggregates it per pane, hash-partitions the partial rows on the device, exch
 library's own round: csrc/exchange.cu) and the owner of a key merges and emits (weak scaling: per-GPU
 input fixed; arroyo_b200/multi_gpu.py).  `--workload join | session`: BASELINE configs[3] / configs[4]
 (bench_workloads.py).
+
+--dump-outputs DIR (N = 1, sliding): after the timed steps, the windows the last timed step emitted (the device batches a
+caller of handle_watermark_device_poll receives), rows ordered by (window start, key), written as float64 .npy files:
+key_hi / key_lo (the i64 key's signed high and unsigned low 32 bits, so that it survives float64 exactly), sum, avg,
+count per row, and window.npy = [start, end, _timestamp] per window in ns after the stream's first pane.  Above
+DUMP_MAX_ROWS rows a fixed seeded sample of the ordered rows is written.  Inputs are generated from fixed seeds, so two
+builds run with the same arguments can be compared file by file.
 """
 import os as _os
 
@@ -56,6 +63,7 @@ T0 = 1_700_000_000 * S
 BATCH_ROWS = 65_536
 WIDTH, SLIDE, WM_DELAY = 10 * S, 1 * S, 1 * S
 KEY_MULT = 0x9E3779B97F4A7C15  # odd => bijection on u64: keys are scattered over the i64 range
+DUMP_MAX_ROWS = 64_000_000 // 40  # --dump-outputs: five float64 columns per row stay under 64 MB
 
 
 def parse():
@@ -91,17 +99,15 @@ def parse():
                     help="measurement knob: the one-pass ingest kernel (probe + REDs per row) instead of the two-pass ingest")
     ap.add_argument("--local-chunk-log2", type=int, default=24,
                     help="N>1, partials: rows per ingest launch of the local stage = 2^n (one pane per launch: the two-pass "
-                         "ingest pays its per-launch table builds once; 2^23 measured 0.73 vs 0.53 ms per step, "
-                         "profiles/r02_partials_n1_c2*.json)")
+                         "ingest pays its per-launch table builds once)")
     ap.add_argument("--python-exchange", action="store_true",
                     help="N>1, partials: the shuffle round through torch.distributed (device partitioner + all_gather + "
                          "all_to_all_single from Python) instead of the library's own round (csrc/exchange.cu: partition + "
-                         "control all-gather + grouped ncclSend / ncclRecv in one C call): 56.7 vs 61.9 G rows/s at N = 2 "
-                         "(profiles/r02_bench_n2*.json)")
+                         "control all-gather + grouped ncclSend / ncclRecv in one C call)")
     ap.add_argument("--native-exchange", action="store_true",
                     help="N>1, partials: the library's own round (see --python-exchange).  It is the default up to 4 GPUs, "
-                         "where it was measured; above that the default is the torch.distributed round, the one that has "
-                         "run on eight GPUs (round 1) -- the library's round is selected with this flag")
+                         "above that the default is the torch.distributed round -- the library's round is selected "
+                         "with this flag")
     ap.add_argument("--sync-plan", action="store_true",
                     help="N>1, partials: run the local stage, the shuffle and the owner stage in sequence on one host "
                          "thread instead of as a two-stage pipeline")
@@ -118,8 +124,12 @@ def parse():
                          "the same second, i.e. what an owner behind that many senders receives")
     ap.add_argument("--shuffle", default="partials", choices=["partials", "rows"],
                     help="N>1: what crosses the all-to-all (per-pane partial aggregates, or raw rows)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="N = 1, sliding: write the windows the last timed step emitted to DIR/*.npy (module docstring)")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if args.dump_outputs and (world > 1 or args.workload != "sliding" or args.impl != "ours"):
+        ap.error("--dump-outputs covers the N = 1 sliding workload of --impl ours")
     args.native_exchange = (not args.python_exchange) and (world <= 4 or args.native_exchange)
     return args
 
@@ -265,18 +275,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
-
-
-def ncu_traffic():
-    """dram bytes per ingest launch from the committed ncu capture (profiles/), or None."""
-    p = os.path.join(ROOT, "profiles", "ingest_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+    return 3350.0, "data sheet (H100 SXM HBM3)"
 
 
 def op_flags(args):
@@ -474,8 +473,9 @@ def build_batch_lists(torch, panes, rows_per_pane):
 
 def bind_to_gpu_numa_node(local):
     """Pins this process to the CPUs NVML reports as local to GPU `local`, before any pinned host memory is
-    allocated (first touch then places it on the GPU's NUMA node).  On this pool's two-socket hosts a process that
-    lands on the other socket moves host<->device data at about 20 GB/s instead of 55.  Returns a description."""
+    allocated (first touch then places it on the GPU's NUMA node).  On a two-socket host a process that lands on the
+    other socket moves host<->device data across the socket link, well below the GPU's own host link.  Returns a
+    description."""
     try:
         import pynvml
         pynvml.nvmlInit()
@@ -492,10 +492,14 @@ def bind_to_gpu_numa_node(local):
         return f"unchanged ({type(e).__name__}: {e})"
 
 
-def device_resident(args, torch, native, ffi, local, panes, W, K, rows, collect=False, sampler=None):
+def device_resident(args, torch, native, ffi, local, panes, W, K, rows, collect=False, sampler=None, last=None):
     """W warm-up + K timed steps over `panes` (already in HBM); CUDA events on the operator's stream.
     Returns (ms, stats delta, rows emitted, clocks, per-window checksums if `collect`).  With `collect` every emitted
-    window is reduced to checksums on the device (torch kernels inside the loop): that pass verifies, it is not timed."""
+    window is reduced to checksums on the device (torch kernels inside the loop): that pass verifies, it is not timed.
+    A list passed as `last` receives the windows whose emission the last timed step began, as (n_rows, [column
+    tensors]) copied on the device when they arrive (the library's pointers are valid only until its next call).  The
+    last warm-up step's windows are copied the same way and dropped, so that the timed copy finds its kernels loaded and
+    its memory in torch's cache."""
     import pyarrow as pa
     device = torch.device("cuda", local)
     plans = build_batch_lists(torch, panes, rows)
@@ -509,6 +513,7 @@ def device_resident(args, torch, native, ffi, local, panes, W, K, rows, collect=
     sums = {}
 
     outstanding = False
+    begun_in = None  # the step whose watermark began the outstanding emission
 
     def gather():
         # the windows of the outstanding emission (arroyo_b200_op_handle_watermark_device_poll)
@@ -519,6 +524,10 @@ def device_resident(args, torch, native, ffi, local, panes, W, K, rows, collect=
         emitted = op.handle_watermark_device_poll()
         for n, _ in emitted:
             rows_out += n
+        if last is not None and K > 0 and begun_in in (W - 1, W + K - 1):
+            from arroyo_b200.multi_gpu import _Ptr
+            last.extend((n, [torch.as_tensor(_Ptr(c, n), device=device).clone() for c in cols])
+                        for n, cols in emitted if n)
         if collect:
             for ws, we, n, cnt, sm, av in window_checksums(torch, device, emitted):
                 sums[ws] = (we, n, cnt, sm, av)
@@ -527,20 +536,20 @@ def device_resident(args, torch, native, ffi, local, panes, W, K, rows, collect=
         # handle_watermark as the begin / poll pair: the emission is enqueued, the next batches are handed over and
         # submitted behind it, and only then are the emitted windows' row counts read -- the device never idles while
         # the host goes round (with `--sync-emit`: the blocking call, one round trip more per step)
-        nonlocal rows_out, outstanding
+        nonlocal rows_out, outstanding, begun_in
         for cols, nrows, wm in plans[p]:
             op.process_device_batches(cols, nrows, 3)
             if wm is None:
                 continue
             if args.sync_emit:
-                outstanding = True
+                outstanding, begun_in = True, p
                 op.handle_watermark_device_begin(wm)
                 gather()
                 continue
             op.submit()
             gather()
             op.handle_watermark_device_begin(wm)
-            outstanding = True
+            outstanding, begun_in = True, p
 
     if sampler is None:
         sampler = ClockSampler(local)
@@ -551,6 +560,8 @@ def device_resident(args, torch, native, ffi, local, panes, W, K, rows, collect=
     gather()
     op.flush()
     torch.cuda.synchronize()
+    if last is not None:
+        last.clear()
     st0 = op.stats()
     rows_out = 0
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -570,6 +581,28 @@ def device_resident(args, torch, native, ffi, local, panes, W, K, rows, collect=
     del plans
     torch.cuda.empty_cache()
     return ms, {k: st1[k] - st0[k] for k in st1}, rows_out, clocks, sums
+
+
+def dump_outputs(torch, out_dir, windows):
+    """Writes `windows` (device_resident's `last`: columns key, window.start, window.end, sum, avg, count,
+    _timestamp) as float64 .npy files, rows ordered by (window start, key) (module docstring)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    cols = [torch.cat([c[i] for _, c in windows]) if windows else torch.empty(0, dtype=torch.int64) for i in range(7)]
+    key, ws = cols[0], cols[1]
+    order = torch.argsort(key, stable=True)
+    order = order[torch.argsort(ws[order], stable=True)].cpu().numpy()
+    if order.size > DUMP_MAX_ROWS:
+        pick = np.sort(np.random.default_rng(42).choice(order.size, DUMP_MAX_ROWS, replace=False))
+        order = order[pick]
+    host = [c.cpu().numpy()[order] for c in cols]
+    key = host[0]
+    arrays = {"key_hi": (key >> 32).astype(np.float64), "key_lo": (key & 0xFFFFFFFF).astype(np.float64),
+              "sum": host[3].astype(np.float64), "avg": host[4].view(np.float64), "count": host[5].astype(np.float64),
+              "window": np.array(sorted([int(c[i][0]) - T0 for i in (1, 2, 6)] for _, c in windows),
+                                 dtype=np.float64).reshape(-1, 3)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a))
 
 
 def run_ours(args):
@@ -610,25 +643,24 @@ def run_ours(args):
     assert rows % BATCH_ROWS == 0
     gen_pane = make_generator(torch, device, rows, args.keys, args.dist, 42 + rank, args.keyspace)
     panes = [gen_pane(p) for p in range(W + K)]
-    ms, d, rows_out, clocks, _ = device_resident(args, torch, native, ffi, local, panes, W, K, rows)
+    last = [] if args.dump_outputs else None
+    ms, d, rows_out, clocks, _ = device_resident(args, torch, native, ffi, local, panes, W, K, rows, last=last)
     del panes
+    if args.dump_outputs:
+        dump_outputs(torch, args.dump_outputs, last)
+        del last
 
     value = K * rows / (ms * 1e-3)
     peak, peak_kind = measured_peak()
     ingest_gbs = 24.0 * d["ingest_rows_timed"] / (d["ingest_ms"] * 1e-3) / 1e9 if d["ingest_ms"] else None
     emit_share = d["emit_ms"] / ms if ms else None
     step_bytes = 24.0 * rows + 72.0 * args.keys + 48.0 * (rows_out / max(K, 1))
-    traffic = ncu_traffic()
     alg_per_launch = 24.0 * d["ingest_rows_timed"] / max(d["ingest_launches"], 1)
-    roof = {"bound": "hbm", "kernel": (traffic or {}).get("kernel", "ingest"),
+    roof = {"bound": "hbm", "kernel": "ingest = part_kernel + agg_kernel",
             "achieved": round(ingest_gbs, 1) if ingest_gbs else None,
             "peak": peak, "peak_kind": peak_kind, "unit": "GB/s",
             "frac": round(ingest_gbs / peak, 4) if ingest_gbs else None,
-            # DRAM bytes of the ncu capture scaled to this run's launch size (the capture's own launch is recorded
-            # beside it), so `traffic` and `algorithmic_bytes_per_launch` describe the same launch
-            "traffic": (round(traffic["dram_bytes_per_row"] * d["ingest_rows_timed"] / max(d["ingest_launches"], 1))
-                        if traffic and traffic.get("dram_bytes_per_row") else None),
-            "traffic_source": (traffic or {}).get("source"),
+            "traffic": None,
             "algorithmic_bytes_per_launch": alg_per_launch,
             "ingest_ms_per_step": d["ingest_ms"] / K, "emit_ms_per_step": d["emit_ms"] / K,
             "ingest_share_of_step": round(d["ingest_ms"] / ms, 3), "emit_share_of_step": round(emit_share, 3),

@@ -1,5 +1,5 @@
 /*
- * arroyo_b200.h -- C ABI of libarroyo_b200.so: B200-native (sm_100a) window-assign /
+ * arroyo_b200.h -- C ABI of libarroyo_b200.so: H100-native (sm_90a) window-assign /
  * keyed-aggregate / windowed-join operators behind Arroyo's ArrowOperator surface.
  *
  * This is the drop-in boundary (SURVEY.md 8(b)).  Every entry point cites the reference

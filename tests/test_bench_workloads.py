@@ -1,8 +1,7 @@
 """Host-side pieces of `bench.py --workload join | session` (bench_workloads.py) that need no GPU: the column checksum
 both sides of the verification use, the identity Shuffle edge of a one-subtask job, and the CPU baselines (the C
-restatements of the join / session operators on key-partitioned subtasks) at toy sizes.  The GPU plans themselves run on
-the GPU box (`python bench.py --workload join`, `--workload session`, N = 1 and N = 2: profiles/r02_bench_join_*.json,
-r02_bench_session_*.json)."""
+restatements of the join / session operators on key-partitioned subtasks) at toy sizes.  The GPU plans themselves run
+through `python bench.py --workload join` and `--workload session` on a GPU."""
 import os
 import sys
 

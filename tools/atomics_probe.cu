@@ -1,7 +1,7 @@
-// Micro-probe (not product code): how fast can B200 do the scatter part of a keyed aggregate?
+// Micro-probe (not product code): how fast can an H100 do the scatter part of a keyed aggregate?
 // Measures, for R random rows into K keys: (a) 1/2/3 x RED.64 into dense L2-resident arrays,
 // (b) the same preceded by a 16-byte dictionary probe, (c) u32 vs u64 counters, (d) AoS vs SoA.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/atomics_probe tools/atomics_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/atomics_probe tools/atomics_probe.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
@@ -61,7 +61,7 @@ template <int MODE>
 float run(const char* name, const long long* k, const long long* v, const long long* t, long long n, unsigned long long K,
           unsigned long long* acc, const ulonglong2* dict, uint32_t dmask, unsigned long long* sink, int reps) {
   cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-  int grid = 148 * 8;
+  int grid = 132 * 8;
   for (int w = 0; w < 2; ++w) probe<MODE><<<grid, 256>>>(k, v, t, n, K, acc, dict, dmask, sink);
   CK(cudaDeviceSynchronize());
   CK(cudaEventRecord(e0));

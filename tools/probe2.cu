@@ -1,4 +1,4 @@
-// Micro-probe 2 (not product code): what limits the random 16-byte dictionary probe on B200, and which
+// Micro-probe 2 (not product code): what limits the random 16-byte dictionary probe on an H100, and which
 // issue pattern gets the most probes in flight?  Variants: rows per thread (MLP), ldcg vs ldg(nc) vs
 // cp.async-to-shared, threads per block.
 #include <cuda_runtime.h>
@@ -54,7 +54,7 @@ void run(const char* name, int threads, const long long* k, const long long* v, 
   size_t smem = LOAD == 2 ? (size_t)threads * RPT * 16 : 0;
   if (smem > 48 * 1024) CK(cudaFuncSetAttribute(probe<RPT, LOAD, RED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int occ = 0; CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, probe<RPT, LOAD, RED>, threads, smem));
-  int grid = 148 * (occ > 0 ? occ : 1);
+  int grid = 132 * (occ > 0 ? occ : 1);
   for (int w = 0; w < 2; ++w) probe<RPT, LOAD, RED><<<grid, threads, smem>>>(k, v, n, d, dm, acc, K, sink);
   CK(cudaDeviceSynchronize());
   CK(cudaEventRecord(e0));

@@ -186,9 +186,9 @@ int main() {
     printf("---- dict %.2f slots/id (%.0f MB), ids in %s order ----\n", spi, cap * 16.0 / 1e6, order ? "slot" : "arrival");
     {
       CK(cudaMemset(acc, 0, K * 16)); CK(cudaMemset(n_defer, 0, 4));
-      direct_kernel<<<148 * 8, 256>>>(k, v, t, n, slots, cap, acc, acc + K, wm); CK(cudaDeviceSynchronize()); check("direct");
+      direct_kernel<<<132 * 8, 256>>>(k, v, t, n, slots, cap, acc, acc + K, wm); CK(cudaDeviceSynchronize()); check("direct");
       CK(cudaEventRecord(e0));
-      for (int r = 0; r < 5; ++r) direct_kernel<<<148 * 8, 256>>>(k, v, t, n, slots, cap, acc, acc + K, wm);
+      for (int r = 0; r < 5; ++r) direct_kernel<<<132 * 8, 256>>>(k, v, t, n, slots, cap, acc, acc + K, wm);
       CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1)); float ms; CK(cudaEventElapsedTime(&ms, e0, e1)); ms /= 5;
       printf("direct probe + 2 RED                                         %7.3f ms  %7.2f Grows/s\n", ms, n / ms / 1e6);
     }
@@ -204,7 +204,7 @@ int main() {
       CK(cudaFuncSetAttribute(aggregate_kernel<BT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemB));
       CK(cudaFuncSetAttribute(partition_kernel<RPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemA));
       int occB = 0; CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occB, aggregate_kernel<BT>, BT, smemB));
-      const int gridA = (int)std::min<long long>((n_sub + A_THREADS * RPT - 1) / (A_THREADS * RPT), 148 * 2);
+      const int gridA = (int)std::min<long long>((n_sub + A_THREADS * RPT - 1) / (A_THREADS * RPT), 132 * 2);
       auto pass = [&]() {
         for (long long off = 0; off < n; off += n_sub) {
           partition_kernel<RPT><<<gridA, A_THREADS, smemA>>>(k + off, v + off, t + off, n_sub, cap, log_spb, P, region, RC, cursor, n_defer, wm, slide_inv, slide);

@@ -101,7 +101,7 @@ int main() {
   for (long long i = 0; i < n; ++i) { st = mix64(st + i); hk[i] = keys[st % K]; hv[i] = (long long)((st >> 20) % 100000000); want_sum += (unsigned long long)hv[i]; }
   CK(cudaMemcpy(k, hk.data(), n * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(v, hv.data(), n * 8, cudaMemcpyHostToDevice));
   cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-  const int grid = 148 * 8;
+  const int grid = 132 * 8;
   auto timeit = [&](const char* name, auto launch, auto reset) {
     reset(); launch(); CK(cudaDeviceSynchronize()); CK(cudaGetLastError());
     float best = 1e9f;

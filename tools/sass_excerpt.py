@@ -17,7 +17,7 @@ PAT = re.compile(r"UBLKCP|SYNCS|ATOMS|ATOMG|\bRED\.|LDS\.128|STS\.128|STG\.E\.12
 
 def main():
     sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
-    print("# cuobjdump -sass arroyo_b200/libarroyo_b200.so (sm_100a): opcode counts and first occurrences per kernel")
+    print("# cuobjdump -sass arroyo_b200/libarroyo_b200.so (sm_90a): opcode counts and first occurrences per kernel")
     for kernel in ("agg_kernelILi1", "agg_kernelILi0", "part_kernelILi1ELi1", "part_kernelILi0ELi0"):
         inside, ops, first = False, Counter(), {}
         for line in sass.splitlines():
