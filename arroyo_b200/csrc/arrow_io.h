@@ -71,6 +71,23 @@ inline std::vector<InColumn> import_batch(const ArrowArray* a, const ArrowSchema
   return cols;
 }
 
+// The aggregating operators compute sum / avg / min / max of Int64 columns grouped by an Int64, UInt64 or
+// timestamp[ns] key (INTEGRATION.md §1).  Any other input type is refused, so the plan stays on the stock operator
+// instead of being aggregated with signed-integer arithmetic over the wrong bits.  key_col < 0: unkeyed.
+inline void require_aggregate_input_types(const std::vector<InColumn>& cols, int key_col, const int* val_cols,
+                                          int n_vals) {
+  if (key_col >= 0) {
+    const std::string& f = cols[key_col].format;
+    if (f != "l" && f != "L" && f.compare(0, 4, "tsn:") != 0)
+      throw Error(ARROYO_B200_UNSUPPORTED, "group-by key of type '" + f + "' (supported: l, L, tsn:)");
+  }
+  for (int v = 0; v < n_vals; ++v) {
+    const std::string& f = cols[val_cols[v]].format;
+    if (f != "l")
+      throw Error(ARROYO_B200_UNSUPPORTED, "aggregate input of type '" + f + "' (only Int64 'l' is supported)");
+  }
+}
+
 // ---- export -------------------------------------------------------------------------------
 struct OutColumn {
   std::string name;

@@ -1012,10 +1012,8 @@ void SessionOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arrow
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
+  require_aggregate_input_types(cols, keyed_ ? key_col_ : -1, val_cols_, n_vals_);
   if (keyed_) key_format_ = cols[key_col_].format;
-  for (int g = 0; g < n_aggs_; ++g)
-    if (agg_kind_[g] == ARROYO_B200_AGG_MIN_I64 || agg_kind_[g] == ARROYO_B200_AGG_MAX_I64)
-      agg_format_[g] = cols[cfg.aggs[g].input_col].format;
   release_inputs(false);
   st_.rows_in += (uint64_t)n;
   if (n == 0) {

@@ -30,7 +30,7 @@ namespace ab {
 namespace {
 
 constexpr int U_MAX_ACC = ARROYO_B200_MAX_AGGS + 1;
-enum : int { U_ROWS = 0, U_SUM = 1, U_MIN = 3, U_MAX = 4 };
+enum : int { U_ROWS = 0, U_SUM = 1, U_SUM_F64 = 2, U_MIN = 3, U_MAX = 4 };
 
 struct UState {
   unsigned long long* cur;   // [n_acc][id_cap]; cur[0] = rows
@@ -77,6 +77,7 @@ __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__
       unsigned long long* dst = p.st.cur + (unsigned long long)a * p.st.id_cap + id;
       switch (p.st.acc_kind[a]) {
         case U_SUM: atomicAdd(dst, (unsigned long long)v); break;
+        case U_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), (double)v); break;
         case U_MIN: atomicMin(reinterpret_cast<long long*>(dst), v); break;
         case U_MAX: atomicMax(reinterpret_cast<long long*>(dst), v); break;
       }
@@ -103,7 +104,7 @@ struct UFlush {
 
 __device__ __forceinline__ unsigned long long finalise(int kind, unsigned long long acc, unsigned long long rows) {
   if (kind == ARROYO_B200_AGG_COUNT_STAR) return rows;
-  if (kind == ARROYO_B200_AGG_AVG_I64) return (unsigned long long)__double_as_longlong((double)(long long)acc / (double)rows);
+  if (kind == ARROYO_B200_AGG_AVG_I64) return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)acc) / (double)rows);
   return acc;
 }
 
@@ -279,7 +280,9 @@ UpdatingAggOp::UpdatingAggOp(const ArroyoB200OpConfig& c) {
     int ak;
     switch (kind) {
       case ARROYO_B200_AGG_SUM_I64: ak = U_SUM; agg_format_.push_back("l"); break;
-      case ARROYO_B200_AGG_AVG_I64: ak = U_SUM; agg_format_.push_back("g"); break;  // exact integer sum, divided at output
+      // AVG sums the inputs as f64, like the reference's accumulator (each value cast to f64, then added): an
+      // integer sum would wrap and average to garbage once the values pass 2^63 in total
+      case ARROYO_B200_AGG_AVG_I64: ak = U_SUM_F64; agg_format_.push_back("g"); break;
       case ARROYO_B200_AGG_MIN_I64: ak = U_MIN; agg_format_.push_back("l"); break;
       case ARROYO_B200_AGG_MAX_I64: ak = U_MAX; agg_format_.push_back("l"); break;
       default: throw Error(ARROYO_B200_UNSUPPORTED, "unsupported aggregate kind");
@@ -438,10 +441,8 @@ void UpdatingAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const A
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
+  require_aggregate_input_types(cols, keyed_ ? key_col_ : -1, val_cols_, n_vals_);
   if (keyed_) key_format_ = cols[key_col_].format;
-  for (int g = 0; g < n_aggs_; ++g)
-    if (agg_kind_[g] == ARROYO_B200_AGG_MIN_I64 || agg_kind_[g] == ARROYO_B200_AGG_MAX_I64)
-      agg_format_[g] = cols[cfg.aggs[g].input_col].format;
   st_.rows_in += (uint64_t)n;
   if (n == 0) {
     if (batch->release) batch->release(batch);

@@ -1070,6 +1070,20 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
   avg_exact_ = !(c.flags & ARROYO_B200_FLAG_AVG_F64);
   acc_kind_[0] = ACC_ROWS;
   acc_val_[0] = 0;
+  // Exact-sum AVG shares the integer sum of its column, and promote_avg later adds one f64 accumulator per AVG
+  // column.  A plan without room for those starts in f64 AVG mode (as with FLAG_AVG_F64), where every aggregate
+  // takes at most one accumulator: every accepted plan fits MAX_ACC and no promotion can fail mid-stream.
+  if (avg_exact_) {
+    std::set<std::pair<int, int>> exact_accs;  // (kind, column), AVG counted as SUM
+    std::set<int> avg_cols;
+    for (int g = 0; g < n_aggs_; ++g) {
+      const int kind = c.aggs[g].kind;
+      if (kind == ARROYO_B200_AGG_COUNT_STAR) continue;
+      exact_accs.emplace(kind == ARROYO_B200_AGG_AVG_I64 ? ARROYO_B200_AGG_SUM_I64 : kind, c.aggs[g].input_col);
+      if (kind == ARROYO_B200_AGG_AVG_I64) avg_cols.insert(c.aggs[g].input_col);
+    }
+    avg_exact_ = 1 + exact_accs.size() + avg_cols.size() <= (size_t)MAX_ACC;
+  }
   for (int g = 0; g < n_aggs_; ++g) {
     int kind = c.aggs[g].kind;
     agg_kind_[g] = kind;
@@ -1480,6 +1494,11 @@ void WindowAggOp::promote_avg() {
   if (!avg_exact_) return;
   AB_REQUIRE(in_flight_.empty(), ARROYO_B200_RUNTIME, "promote with launches in flight");
   const int old_n_acc = n_acc_;
+  // the constructor leaves room for these; checked before any state changes so a failure leaves the operator whole
+  std::set<int> avg_srcs;
+  for (int g = 0; g < n_aggs_; ++g)
+    if (agg_kind_[g] == ARROYO_B200_AGG_AVG_I64) avg_srcs.insert(agg_acc_[g]);
+  AB_REQUIRE(old_n_acc + (int)avg_srcs.size() <= MAX_ACC, ARROYO_B200_RUNTIME, "too many accumulators after AVG promotion");
   std::vector<std::pair<int, int>> f64_from;
   for (int g = 0; g < n_aggs_; ++g) {
     if (agg_kind_[g] != ARROYO_B200_AGG_AVG_I64) continue;
@@ -1488,7 +1507,6 @@ void WindowAggOp::promote_avg() {
     for (auto& pr : f64_from)
       if (pr.second == src) found = pr.first;
     if (found < 0) {
-      AB_REQUIRE(n_acc_ < MAX_ACC, ARROYO_B200_RUNTIME, "too many accumulators after AVG promotion");
       found = n_acc_;
       acc_kind_[n_acc_] = ACC_SUM_F64;
       acc_val_[n_acc_] = acc_val_[src];
@@ -1677,14 +1695,8 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
+  require_aggregate_input_types(cols, keyed_ ? key_col_ : -1, val_cols_, n_vals_);
   if (keyed_) key_format_ = cols[key_col_].format;
-  for (int g = 0; g < n_aggs_; ++g)
-    if (agg_kind_[g] == ARROYO_B200_AGG_MIN_I64 || agg_kind_[g] == ARROYO_B200_AGG_MAX_I64 ||
-        agg_kind_[g] == ARROYO_B200_AGG_SUM_I64) {
-      const std::string& f = cols[cfg.aggs[g].input_col].format;
-      AB_REQUIRE(f != "g", ARROYO_B200_UNSUPPORTED, "float64 aggregate inputs are not supported");
-      if (agg_kind_[g] != ARROYO_B200_AGG_SUM_I64) agg_format_[g] = f;
-    }
   poll_releases(false);
   st_.rows_in += (uint64_t)n;
   if (n > 0 && panes_.empty() && max_bin_seen_ == LLONG_MIN) {

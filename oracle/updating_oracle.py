@@ -39,11 +39,12 @@ class UpdatingAggConfig:
 
 
 class _KeyState:
-    __slots__ = ("rows", "sums", "multi", "ts")
+    __slots__ = ("rows", "sums", "fsums", "multi", "ts")
 
     def __init__(self, n_aggs):
         self.rows = 0                                # count(*) / avg denominator / "has rows"
-        self.sums = [0] * n_aggs                     # wrapping int64 sums (sum, avg)
+        self.sums = [0] * n_aggs                     # wrapping int64 sums (sum)
+        self.fsums = [0.0] * n_aggs                  # f64 sums in row order (avg: each value cast to f64, then added)
         self.multi: List[Dict[int, int]] = [dict() for _ in range(n_aggs)]  # value -> count (min, max, count_distinct)
         self.ts: Dict[int, int] = {}                 # multiset of _timestamp (the trailing max(_timestamp) aggregate)
 
@@ -74,7 +75,7 @@ class IncrementalAggregatingFunc:
             elif k == "sum":
                 out.append(_wrap(st.sums[a]) if st.rows else None)
             elif k == "avg":
-                out.append(float(_wrap(st.sums[a])) / st.rows if st.rows else None)
+                out.append(st.fsums[a] / st.rows if st.rows else None)
             else:
                 live = [v for v, c in st.multi[a].items() if c > 0]
                 if k == "count_distinct":
@@ -108,8 +109,10 @@ class IncrementalAggregatingFunc:
             t = int(ts[i])
             st.ts[t] = st.ts.get(t, 0) + sign
             for a, agg in enumerate(self.cfg.aggs):
-                if agg.kind in ("sum", "avg"):
+                if agg.kind == "sum":
                     st.sums[a] += sign * int(batch[agg.col][i])
+                elif agg.kind == "avg":
+                    st.fsums[a] += sign * float(int(batch[agg.col][i]))
                 elif agg.kind in ("min", "max", "count_distinct"):
                     v = int(batch[agg.col][i])
                     c = st.multi[a].get(v)

@@ -12,7 +12,8 @@ import numpy as np
 import pytest
 
 from oracle import arroyo_oracle as O
-from tests.test_gpu_parity import S, assert_same, gen_stream
+from tests.test_gpu_agg_plans import PLANS
+from tests.test_gpu_parity import S, assert_same, gen_multi_stream, gen_stream
 
 pytestmark = pytest.mark.gpu
 
@@ -68,13 +69,17 @@ def _run_prefix(op, ctx, out, gen, batches, adapt=lambda b: b):
 
 
 @pytest.mark.parametrize("kind", ["sliding", "tumbling"])
-@pytest.mark.parametrize("aggs", [AGGS, SUM_ONLY, MINMAX], ids=["sum_avg_count", "sum_only", "min_max"])
+@pytest.mark.parametrize("aggs", [AGGS, SUM_ONLY, MINMAX, PLANS["P3"], PLANS["P4"], PLANS["P5"]],
+                         ids=["sum_avg_count", "sum_only", "min_max", "P3", "P4", "P5"])
 def test_checkpoint_tables_match_and_restore_both_ways(kind, aggs):
     import arroyo_b200 as ab
     from tests.gpu_ops import from_arrow, to_arrow
 
     rng = np.random.default_rng(77)
-    batches = gen_stream(rng, 60_000, 1_500, rate_per_s=10_000, batch=3000)
+    if any(a.col not in (None, "value") for a in aggs):  # the multi-column plans read a, b, c, d
+        batches = gen_multi_stream(rng, 60_000, 1_500, rate_per_s=10_000, batch=3000)
+    else:
+        batches = gen_stream(rng, 60_000, 1_500, rate_per_s=10_000, batch=3000)
     cfg = _cfg(kind, aggs)
     want = O.run_single_input(_oracle_cls(kind)(cfg), batches, S).batches
     half = len(batches) // 2
@@ -112,7 +117,7 @@ def test_checkpoint_tables_match_and_restore_both_ways(kind, aggs):
             assert list(b.cols) == list(o_state[t][0].cols)  # partial_schema column order
 
     rest = batches[half:]
-    fcols = ("avg",) if any(a.kind == "avg" for a in aggs) else ()
+    fcols = tuple(a.name for a in aggs if a.kind == "avg")
 
     def finish(op, ctx, out, gen, adapt=lambda b: b):
         _run_prefix(op, ctx, out, gen, rest, adapt=adapt)

@@ -38,6 +38,54 @@ def gen_stream(rng, n_rows, n_keys, rate_per_s, disorder=50, key_dist="uniform",
     return O.source_batches(cols, batch)
 
 
+I64MIN, I64MAX = -(1 << 63), (1 << 63) - 1
+
+
+def gen_multi_stream(rng, n_rows, n_keys, rate_per_s, key_dist="uniform", regime="R1", batch=4096, disorder=50):
+    """Rows with the value columns a, b, c, d, in arrival order like `gen_stream` (no row is late for a 1 s
+    watermark delay at these rates).
+
+    key_dist: uniform | hot (75 % on one key) | u64 (UInt64 keys >= 2^63).
+    regime R1: every value |v| < 2^31, so every AVG path is exact.
+    regime R2: R1 plus INT64_MIN / INT64_MAX in every column (the MIN / MAX identities), keys whose only value in a
+               column is one of them, and values near 2^62 that make SUMs wrap.
+    regime R3: R1 until the middle of the stream, then values >= 2^31 in column d only (value slot 3 of a plan that
+               reads a, b, c, d in that order), and from three quarters on in b as well."""
+    idx = np.arange(n_rows, dtype=np.int64)
+    if disorder > 1:
+        idx = np.concatenate([rng.permutation(min(disorder, n_rows - s)) + s for s in range(0, n_rows, disorder)])
+    ts = T0 + (idx * (S // rate_per_s)).astype(np.int64)
+    if key_dist == "hot":
+        keys = np.where(rng.random(n_rows) < 0.75, 42, rng.integers(0, n_keys, n_rows, dtype=np.int64))
+    else:
+        keys = rng.integers(0, n_keys, n_rows, dtype=np.int64) * 7919 - 13
+    lim = (1 << 31) - 1
+    vals = {c: rng.integers(-lim, lim + 1, n_rows, dtype=np.int64) for c in "abcd"}
+    if regime == "R2":
+        for c in "abcd":
+            v = vals[c]
+            v[rng.random(n_rows) < 0.01] = I64MIN
+            v[rng.random(n_rows) < 0.01] = I64MAX
+            big = rng.random(n_rows) < 0.02
+            v[big] = (1 << 62) + rng.integers(0, 1 << 20, int(big.sum()), dtype=np.int64)
+        # keys with a single row each: their only value of a column is an identity value
+        lone = rng.choice(n_rows, 40, replace=False)
+        keys[lone] = 10_000_000 + np.arange(40)
+        for j, r in enumerate(lone):
+            for c in "abcd":
+                vals[c][r] = I64MAX if (j + "abcd".index(c)) % 2 else I64MIN
+    elif regime == "R3":
+        half, late = n_rows // 2, 3 * n_rows // 4
+        d = vals["d"]
+        d[half::97] = (1 << 40) + 12345
+        d[half + 5::389] = -(1 << 61)
+        vals["b"][late::151] = (1 << 35) - 7
+    if key_dist == "u64":
+        keys = (keys.view(np.uint64) & np.uint64(0xFFFFFFFF)) | np.uint64(1 << 63)
+    cols = {"key": keys, **vals, O.TIMESTAMP: ts}
+    return O.source_batches(cols, batch)
+
+
 def run_both(G, make_oracle, make_gpu, batches, delay_ns=S):
     want = O.run_single_input(make_oracle(), batches, delay_ns).batches
     gop = make_gpu()
