@@ -88,6 +88,24 @@ inline void require_aggregate_input_types(const std::vector<InColumn>& cols, int
   }
 }
 
+// The joins compare raw 64-bit key patterns, which is equality only for integer-like keys of one type: an Int64,
+// UInt64 or timestamp[ns] key, the same type on both sides (INTEGRATION.md §1).  A Float64 key (-0.0 = 0.0) or an
+// Int64 key against a UInt64 key is refused.  `seen_*`: the key format an earlier batch of this / the other side
+// carried ("" while unknown).
+inline int join_key_class(const std::string& f) {
+  if (f == "l") return 1;
+  if (f == "L") return 2;
+  if (f.compare(0, 4, "tsn:") == 0) return 3;
+  return 0;
+}
+inline void require_join_key_type(const std::string& f, const std::string& seen_this, const std::string& seen_other) {
+  const int k = join_key_class(f);
+  if (k == 0) throw Error(ARROYO_B200_UNSUPPORTED, "join key of type '" + f + "' (supported: l, L, tsn:)");
+  for (const std::string* s : {&seen_this, &seen_other})
+    if (!s->empty() && join_key_class(*s) != k)
+      throw Error(ARROYO_B200_UNSUPPORTED, "join key of type '" + f + "' after keys of type '" + *s + "'");
+}
+
 // ---- export -------------------------------------------------------------------------------
 struct OutColumn {
   std::string name;

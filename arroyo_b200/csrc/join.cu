@@ -207,6 +207,7 @@ struct Side {
   int n_cols = 0, ts_col = 0, key_col = 0, n_routing = 0;
   std::vector<int> payload;             // input column indices that appear in the output
   std::vector<std::string> formats;     // Arrow format per input column
+  std::string key_format;               // the key's format once a host batch has shown it
   std::vector<DevBuf> cols, cols_alt;   // arenas (and the compaction target)
   int64_t n = 0, cap = 0;
   DevBuf elig, cnt, off;
@@ -276,6 +277,9 @@ InstantJoinOp::InstantJoinOp(const ArroyoB200OpConfig& c) {
     AB_REQUIRE(n_cols >= 2 && n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad join side n_cols");
     AB_REQUIRE(ts_col >= 0 && ts_col < n_cols && key_col >= 0 && key_col < n_cols && n_routing >= 0 && n_routing < n_cols,
                ARROYO_B200_INVALID_ARGUMENT, "bad join side columns");
+    // the routing copies never reach the device: the key and the timestamp must be payload columns
+    AB_REQUIRE(key_col >= n_routing && ts_col >= n_routing, ARROYO_B200_INVALID_ARGUMENT,
+               "join key or timestamp column among the routing columns");
     s.n_cols = n_cols;
     s.ts_col = ts_col;
     s.key_col = key_col;
@@ -330,6 +334,8 @@ void InstantJoinOp::reserve(Side& s, int64_t extra) {
   if (s.n + extra <= s.cap) return;
   int64_t nc = std::max<int64_t>(s.cap * 2, 1 << 16);
   while (nc < s.n + extra) nc *= 2;
+  // rows are numbered as int (pairs) and as row + 1 in 32 bits (table slots)
+  AB_REQUIRE(nc < (1ll << 31), ARROYO_B200_RUNTIME, "join side holds more than 2^31 rows");
   for (int c = 0; c < s.n_cols; ++c) {
     if (c < s.n_routing) continue;
     DevBuf nb((size_t)nc * 8);
@@ -360,8 +366,10 @@ void InstantJoinOp::process_batch(uint32_t index, uint32_t in_partitions, ArrowA
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == s.n_cols, ARROYO_B200_INVALID_ARGUMENT, "join side has the wrong number of columns");
+  require_join_key_type(cols[s.key_col].format, s.key_format, side_[1 - sd].key_format);
   AB_REQUIRE(n > 0, ARROYO_B200_PANIC, "should have max timestamp (empty batch; instant_join.rs:123)");
   for (int c = 0; c < s.n_cols; ++c) s.formats[c] = cols[c].format;
+  s.key_format = cols[s.key_col].format;
   const uint64_t* ptrs[ARROYO_B200_MAX_COLS];
   for (int c = 0; c < s.n_cols; ++c) ptrs[c] = cols[c].data;
   append(s, ptrs, n, true);
@@ -377,6 +385,7 @@ void InstantJoinOp::process_device_batch(uint32_t index, uint32_t in_partitions,
   AB_CUDA(cudaSetDevice(device_));
   AB_REQUIRE(in_partitions >= 2 && in_partitions % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
   const int sd = (int)(index / (in_partitions / 2));
+  AB_REQUIRE(sd == 0 || sd == 1, ARROYO_B200_INVALID_ARGUMENT, "bad input index");
   Side& s = side_[sd];
   AB_REQUIRE(n_cols == s.n_cols, ARROYO_B200_INVALID_ARGUMENT, "join side has the wrong number of columns");
   if (n_rows <= 0) return;
@@ -425,6 +434,8 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
              "device-resident join output is only available for inner joins (no validity bitmaps)");
   Side& L = side_[0];
   Side& R = side_[1];
+  AB_REQUIRE(out_host != nullptr || L.payload.size() + R.payload.size() + 1 <= ARROYO_B200_MAX_COLS, ARROYO_B200_UNSUPPORTED,
+             "device-resident join output has more than ARROYO_B200_MAX_COLS columns");
   unsigned long long* sc = scalars_.as<unsigned long long>();
   unsigned long long init[8] = {0, 0, (unsigned long long)LLONG_MAX, (unsigned long long)LLONG_MAX, 0, 0, 0, 0};
   AB_CUDA(cudaMemcpyAsync(sc, init, sizeof init, cudaMemcpyHostToDevice, stream_));

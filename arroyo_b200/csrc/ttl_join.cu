@@ -131,6 +131,7 @@ struct TSide {
   int n_cols = 0, ts_col = 0, key_col = 0, n_routing = 0;
   std::vector<int> payload;
   std::vector<std::string> formats;
+  std::string key_format;  // the key's format once a batch has shown it
   std::vector<DevBuf> cols;
   DevBuf next, tab;
   int64_t n = 0, cap = 0;
@@ -189,7 +190,7 @@ TtlJoinOp::TtlJoinOp(const ArroyoB200OpConfig& c) {
              "JoinWithExpiration: only inner joins of append-only inputs are supported");
   auto init_side = [&](TSide& s, int n_cols, int ts_col, int key_col, int n_routing) {
     AB_REQUIRE(n_cols >= 2 && n_cols <= ARROYO_B200_MAX_COLS && ts_col >= 0 && ts_col < n_cols && key_col >= 0 &&
-                   key_col < n_cols && n_routing >= 0 && n_routing < n_cols && key_col >= n_routing,
+                   key_col < n_cols && n_routing >= 0 && n_routing < n_cols && key_col >= n_routing && ts_col >= n_routing,
                ARROYO_B200_INVALID_ARGUMENT, "bad join side columns");
     s.n_cols = n_cols;
     s.ts_col = ts_col;
@@ -247,18 +248,19 @@ void TtlJoinOp::reserve(TSide& s, int64_t extra) {
 void TtlJoinOp::ensure_table(TSide& s, uint64_t more_rows) {
   const uint64_t need = (s.keys_bound + more_rows) * 2 + 1024;
   if (s.tab_cap >= need) return;
-  uint32_t nc = std::max<uint32_t>(s.tab_cap * 2, 1u << 16);
+  uint64_t nc = std::max<uint64_t>((uint64_t)s.tab_cap * 2, 1u << 16);
   while (nc < need) nc *= 2;
+  AB_REQUIRE(nc <= (1ull << 31), ARROYO_B200_RUNTIME, "join side's key table would exceed 2^31 slots");
   DevBuf nt((size_t)nc * sizeof(MSlot));
   AB_CUDA(cudaMemsetAsync(nt.p, 0, (size_t)nc * sizeof(MSlot), stream_));
   if (s.tab_cap) {
-    tj_rehash_kernel<<<grid_for(s.tab_cap), TJ, 0, stream_>>>(s.tab.as<MSlot>(), s.tab_cap, nt.as<MSlot>(), nc - 1);
+    tj_rehash_kernel<<<grid_for(s.tab_cap), TJ, 0, stream_>>>(s.tab.as<MSlot>(), s.tab_cap, nt.as<MSlot>(), (uint32_t)(nc - 1));
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
   }
   AB_CUDA(cudaStreamSynchronize(stream_));
   s.tab = std::move(nt);
-  s.tab_cap = nc;
+  s.tab_cap = (uint32_t)nc;
 }
 
 void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* batch, const ArrowSchema* schema, BatchesPriv* out) {
@@ -271,7 +273,9 @@ void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* b
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == s.n_cols, ARROYO_B200_INVALID_ARGUMENT, "join side has the wrong number of columns");
+  require_join_key_type(cols[s.key_col].format, s.key_format, o.key_format);
   for (int c = 0; c < s.n_cols; ++c) s.formats[c] = cols[c].format;
+  s.key_format = cols[s.key_col].format;
   st_.rows_in += (uint64_t)n;
   if (n == 0) {
     if (batch->release) batch->release(batch);

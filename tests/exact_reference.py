@@ -1,6 +1,7 @@
-"""Exact group-by reference for the window and updating aggregates, computed straight from the raw input rows with
-numpy and Python integers.  It shares no code or arithmetic with oracle/, so it can catch mistakes the oracle and
-the CUDA operators would make together (an AVG taken over a wrapped integer sum, a float32 or double-rounded mean).
+"""Exact group-by reference for the window and updating aggregates, and exact reference joins (`instant_join`,
+`expiring_join`), computed straight from the raw input rows with numpy and Python integers.  It shares no code or
+arithmetic with oracle/, so it can catch mistakes the oracle and the CUDA operators would make together (an AVG taken
+over a wrapped integer sum, a float32 or double-rounded mean, a join that matches on part of its key).
 
 AVG rule (`check_avg`): when the absolute values of a group's inputs sum to less than 2^53, every f64 or exact-integer
 AVG path is exact up to its one final division, so the result must be bit-identical to the correctly rounded mean.
@@ -184,3 +185,212 @@ def mismatches(want: dict, got_rows, key_of):
     for g in want.keys() - seen:
         errs.append(f"missing group {g}")
     return errs
+
+
+# ---- joins ------------------------------------------------------------------------------------------------------
+# A join input batch is a mapping {column name: numpy array of a 64-bit type} in schema order (or anything with such
+# a mapping as `.cols`).  Keys are grouped by their Python value (`tolist()`: Int64 signed, UInt64 unsigned), every
+# other value travels as its 64-bit pattern, so Float64 payloads keep NaN payloads and -0.0 and UInt64 values >= 2^63
+# stay exact.  Output columns: the left side's columns that are neither routing nor `_timestamp`, then the right
+# side's (a name the left side already has gets `_right`), then `_timestamp`.
+INT64_MAX = (1 << 63) - 1
+
+
+def _columns(batch):
+    return batch.cols if hasattr(batch, "cols") else batch
+
+
+def _bits(a) -> np.ndarray:
+    a = np.ascontiguousarray(a)
+    if a.dtype.itemsize != 8:
+        raise TypeError(f"join columns are 64-bit, got {a.dtype}")
+    return a.view(np.uint64)
+
+
+class Rows:
+    """A multiset of join output rows: `names`, `vals` ((n, k) uint64, each value's 64-bit pattern, 0 where null) and
+    `valid` ((n, k) bool)."""
+
+    def __init__(self, names, vals, valid):
+        self.names = list(names)
+        k = len(self.names)
+        self.vals = np.asarray(vals, dtype=np.uint64).reshape(-1, k)
+        self.valid = np.asarray(valid, dtype=bool).reshape(self.vals.shape)
+        self.vals = np.where(self.valid, self.vals, np.uint64(0))
+
+    @classmethod
+    def from_columns(cls, names, cols, valid=None):
+        """`cols`: one 64-bit array per name; `valid`: {name: bool array} for the columns that have nulls."""
+        valid = valid or {}
+        n = len(cols[0]) if cols else 0
+        vals = np.stack([_bits(c) for c in cols], axis=1) if n else np.zeros((0, len(names)), np.uint64)
+        ok = np.stack([np.asarray(valid[c], bool) if c in valid else np.ones(n, bool) for c in names], axis=1) \
+            if n else np.zeros((0, len(names)), bool)
+        return cls(names, vals, ok)
+
+    def __len__(self):
+        return len(self.vals)
+
+    def tuples(self, rows=None):
+        idx = range(len(self)) if rows is None else rows
+        return [tuple(int(v) if ok else None for v, ok in zip(self.vals[i], self.valid[i])) for i in idx]
+
+    def _sorted(self):
+        """Rows as one (n, k + 1) array [values, validity bits] in a canonical order: by a 64-bit fingerprint of the
+        row.  Equal rows have equal fingerprints, so two equal multisets sort to equal arrays; the comparison itself is
+        on the full rows (a fingerprint collision can only make equal multisets compare unequal)."""
+        bits = (self.valid.astype(np.uint64) << np.arange(self.valid.shape[1], dtype=np.uint64)).sum(axis=1, dtype=np.uint64)
+        a = np.concatenate([self.vals, bits[:, None]], axis=1)
+        h = np.full(len(a), 0xCBF29CE484222325, dtype=np.uint64)
+        with np.errstate(over="ignore"):
+            for c in range(a.shape[1]):
+                h = (h ^ a[:, c]) * np.uint64(0x100000001B3)
+                h ^= h >> np.uint64(29)
+            h = (h ^ (h >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+            h ^= h >> np.uint64(31)
+        return a[np.argsort(h)]
+
+
+def join_mismatches(want: Rows, got: Rows, limit: int = 10):
+    """Differences between two multisets of rows (empty: equal)."""
+    if want.names != got.names:
+        return [f"columns {got.names}, want {want.names}"]
+    a, b = want._sorted(), got._sorted()
+    if a.shape == b.shape and np.array_equal(a, b):
+        return []
+    from collections import Counter
+    cw, cg = Counter(want.tuples()), Counter(got.tuples())
+    errs = [f"{len(got)} rows, want {len(want)}"]
+    errs += [f"missing {r} x{n}" for r, n in (cw - cg).items()][:limit]
+    errs += [f"unexpected {r} x{n}" for r, n in (cg - cw).items()][:limit]
+    return errs
+
+
+class _JoinSide:
+    """The rows one join input has sent so far: payload bits, timestamps and key values, by arrival number."""
+
+    def __init__(self, on, routing):
+        self.on, self.routing = on, tuple(routing)
+        self.names = None
+        self.chunks, self.ts, self.keys = [], [], []
+        self._vals = None
+
+    def add(self, batch):
+        cols = _columns(batch)
+        names = [c for c in cols if c not in self.routing and c != TIMESTAMP]
+        if self.names is None:
+            self.names = names
+        first = len(self.ts)
+        if len(cols[TIMESTAMP]):
+            self.chunks.append(np.stack([_bits(cols[c]) for c in names], axis=1))
+        self.ts += np.asarray(cols[TIMESTAMP]).astype(np.int64).tolist()
+        self.keys += np.asarray(cols[self.on]).tolist()
+        self._vals = None
+        return range(first, len(self.ts))
+
+    def vals(self):
+        if self._vals is None:
+            self._vals = np.concatenate(self.chunks) if self.chunks else np.zeros((0, len(self.names or [])), np.uint64)
+        return self._vals
+
+
+def _output(sides, li, ri):
+    """Gathers the output rows of the (left row, right row) pairs (-1: that side is null)."""
+    lnames = sides[0].names or []
+    rnames = sides[1].names or []
+    names = list(lnames)
+    for c in rnames:
+        names.append(c if c not in names else c + "_right")
+    names.append(TIMESTAMP)
+    li = np.asarray(li, dtype=np.int64)
+    ri = np.asarray(ri, dtype=np.int64)
+    n = len(li)
+    parts, ok = [], []
+    lts = np.full(n, np.iinfo(np.int64).min, dtype=np.int64)
+    rts = lts.copy()
+    for side, idx, tsv in ((sides[0], li, lts), (sides[1], ri, rts)):
+        k = len(side.names or [])
+        has = idx >= 0
+        v = np.zeros((n, k), dtype=np.uint64)
+        if has.any():
+            v[has] = side.vals()[idx[has]]
+            tsv[has] = np.asarray(side.ts, dtype=np.int64)[idx[has]]
+        parts.append(v)
+        ok.append(np.repeat(has[:, None], k, axis=1))
+    parts.append(np.maximum(lts, rts).view(np.uint64)[:, None])  # a null side's timestamp is INT64_MIN
+    ok.append(np.ones((n, 1), dtype=bool))
+    return Rows(names, np.concatenate(parts, axis=1), np.concatenate(ok, axis=1))
+
+
+def _cross(pairs_l, pairs_r, ls, rs):
+    """Appends every (l, r) pair of two lists of row numbers, l-major."""
+    pairs_l.append(np.repeat(np.asarray(ls, dtype=np.int64), len(rs)))
+    pairs_r.append(np.tile(np.asarray(rs, dtype=np.int64), len(ls)))
+
+
+def instant_join(events, join_type, left_on, right_on, left_routing=(), right_routing=()):
+    """The windowed join.  `events`: a sequence of (side, batch) with side 0 = left, 1 = right, and ("wm", w).  At
+    each watermark w every buffered row with `_timestamp < w` joins the other side's rows with equal (`_timestamp`,
+    key); in a left / right / full join a left / right row without a match leaves once with the other side null.
+    Rows with `_timestamp >= w` stay buffered.  A batch with a row older than the last watermark raises ValueError
+    (the reference panics).  Returns one Rows per watermark, in order."""
+    keep = (join_type in ("left", "full"), join_type in ("right", "full"))
+    sides = (_JoinSide(left_on, left_routing), _JoinSide(right_on, right_routing))
+    buffered = ([], [])
+    last_wm = None
+    out = []
+    for ev, arg in events:
+        if ev != "wm":
+            rows = sides[ev].add(arg)
+            if last_wm is not None and any(sides[ev].ts[r] < last_wm for r in rows):
+                raise ValueError("a row older than the watermark")
+            buffered[ev].extend(rows)
+            continue
+        w = min(int(arg), INT64_MAX)
+        groups = {}
+        for s in (0, 1):
+            ts, keys = sides[s].ts, sides[s].keys
+            still = []
+            for r in buffered[s]:
+                if ts[r] < w:
+                    groups.setdefault((ts[r], keys[r]), ([], []))[s].append(r)
+                else:
+                    still.append(r)
+            buffered[s][:] = still
+        pl, pr = [], []
+        for ls, rs in groups.values():
+            if ls and rs:
+                _cross(pl, pr, ls, rs)
+            elif ls and keep[0]:
+                _cross(pl, pr, ls, [-1])
+            elif rs and keep[1]:
+                _cross(pl, pr, [-1], rs)
+        cat = lambda p: np.concatenate(p) if p else np.zeros(0, np.int64)  # noqa: E731
+        out.append(_output(sides, cat(pl), cat(pr)))
+        last_wm = w
+    return out
+
+
+def expiring_join(events, left_on, right_on, left_routing=(), right_routing=()):
+    """The join with expiration (inner, append-only inputs, no expiry inside a run).  `events`: a sequence of
+    (side, batch).  Each arriving batch joins every earlier row of the other side with an equal key; `_timestamp` =
+    max(left, right).  Returns one Rows per batch, in order."""
+    sides = (_JoinSide(left_on, left_routing), _JoinSide(right_on, right_routing))
+    by_key = ({}, {})
+    out = []
+    for s, batch in events:
+        rows = sides[s].add(batch)
+        mine = {}
+        for r in rows:
+            mine.setdefault(sides[s].keys[r], []).append(r)
+        pn, po = [], []
+        for k, new in mine.items():
+            old = by_key[1 - s].get(k)
+            if old:
+                _cross(pn, po, new, old)
+        for k, new in mine.items():
+            by_key[s].setdefault(k, []).extend(new)
+        cat = lambda p: np.concatenate(p) if p else np.zeros(0, np.int64)  # noqa: E731
+        pn, po = cat(pn), cat(po)
+        out.append(_output(sides, pn, po) if s == 0 else _output(sides, po, pn))
+    return out
