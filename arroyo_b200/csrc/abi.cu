@@ -1,5 +1,6 @@
 // extern "C" entry points of libarroyo_b200.so (see include/arroyo_b200.h for the contract and the
 // reference interfaces each one replaces).  Nothing unwinds across this boundary.
+#include <algorithm>
 #include <chrono>
 #include <new>
 
@@ -49,6 +50,15 @@ void set_err(char* err, uint64_t len, const char* msg) {
   if (err && len) {
     snprintf(err, (size_t)len, "%s", msg);
   }
+}
+
+// Writes the first max_out windows of `v` to `out`; the rest stay queued, in order, for the next
+// handle_watermark_device_poll.  The emission has already left the operator, so nothing may be dropped here.
+int64_t hand_out(OpBase* o, std::vector<ArroyoB200DeviceBatch>& v, ArroyoB200DeviceBatch* out, int64_t max_out) {
+  const size_t n = (size_t)std::min<int64_t>((int64_t)v.size(), std::max<int64_t>(max_out, 0));
+  for (size_t i = 0; i < n; ++i) out[i] = v[i];
+  o->pending_dev.assign(v.begin() + n, v.end());
+  return (int64_t)n;
 }
 
 }  // namespace
@@ -345,19 +355,25 @@ int32_t arroyo_b200_op_handle_watermark_device(ArroyoB200Op* op, int64_t waterma
   if (!op) return ARROYO_B200_INVALID_ARGUMENT;
   WallTimer wt(op->host_watermark_ms);
   return guarded(op, [&](OpBase* o) {
-    AB_REQUIRE(n_out != nullptr && (out != nullptr || max_out == 0), ARROYO_B200_INVALID_ARGUMENT, "null out");
+    AB_REQUIRE(n_out != nullptr && (out != nullptr || max_out <= 0), ARROYO_B200_INVALID_ARGUMENT, "null out");
+    // the queued windows live in the output buffers the next emission would write
+    AB_REQUIRE(o->pending_dev.empty(), ARROYO_B200_INVALID_ARGUMENT,
+               "windows of the previous emission are still queued (handle_watermark_device_poll)");
     std::vector<ArroyoB200DeviceBatch> v;
     o->handle_watermark(watermark_ns, nullptr, &v);
-    AB_REQUIRE((int64_t)v.size() <= max_out, ARROYO_B200_RUNTIME, "more windows emitted than max_out");
-    for (size_t i = 0; i < v.size(); ++i) out[i] = v[i];
-    *n_out = (int64_t)v.size();
+    *n_out = hand_out(o, v, out, max_out);
   });
 }
 
 int32_t arroyo_b200_op_handle_watermark_device_begin(ArroyoB200Op* op, int64_t watermark_ns) {
   if (!op) return ARROYO_B200_INVALID_ARGUMENT;
   WallTimer wt(op->host_watermark_ms);
-  return guarded(op, [&](OpBase* o) { o->begin_watermark_device(watermark_ns); });
+  return guarded(op, [&](OpBase* o) {
+    // the queued windows live in the output buffers the next emission would write (every operator kind)
+    AB_REQUIRE(o->pending_dev.empty(), ARROYO_B200_INVALID_ARGUMENT,
+               "windows of the previous emission are still queued (handle_watermark_device_poll)");
+    o->begin_watermark_device(watermark_ns);
+  });
 }
 
 int32_t arroyo_b200_op_handle_watermark_device_poll(ArroyoB200Op* op, ArroyoB200DeviceBatch* out, int64_t max_out,
@@ -366,12 +382,10 @@ int32_t arroyo_b200_op_handle_watermark_device_poll(ArroyoB200Op* op, ArroyoB200
   if (!op) return ARROYO_B200_INVALID_ARGUMENT;
   WallTimer wt(op->host_watermark_ms);
   return guarded(op, [&](OpBase* o) {
-    AB_REQUIRE(n_out != nullptr && (out != nullptr || max_out == 0), ARROYO_B200_INVALID_ARGUMENT, "null out");
+    AB_REQUIRE(n_out != nullptr && (out != nullptr || max_out <= 0), ARROYO_B200_INVALID_ARGUMENT, "null out");
     std::vector<ArroyoB200DeviceBatch> v;
     o->poll_watermark_device(&v);
-    AB_REQUIRE((int64_t)v.size() <= max_out, ARROYO_B200_RUNTIME, "more windows emitted than max_out");
-    for (size_t i = 0; i < v.size(); ++i) out[i] = v[i];
-    *n_out = (int64_t)v.size();
+    *n_out = hand_out(o, v, out, max_out);
   });
 }
 

@@ -20,9 +20,13 @@ namespace ab {
 
 constexpr int64_t NO_TIME = INT64_MIN;
 
+// Floor division: a negative watermark (the first timestamps of a stream are smaller than the watermark delay) bins
+// below zero, so it makes no row late and closes no window.  Truncation would round it up towards zero.
 inline int64_t bin_start(int64_t ts, int64_t width) {
   if (width == 0) return ts;
-  return ts - ts % width;
+  int64_t r = ts % width;
+  if (r < 0) r += width;
+  return ts - r;
 }
 
 struct PlanStep {
@@ -185,8 +189,16 @@ class SlidingPlanner {
       tier_.erase(tier_.begin());
     }
     if (tier_.empty()) {
+      // The reference looks only at the table here, so panes that received rows while the store was non-empty and
+      // were never checkpointed (the first batch after a gap longer than the window, rows far ahead) would never be
+      // emitted.  Their earliest bin is a candidate too: no on-time row is lost.
       int64_t mt;
-      if (table_.get_min_time(&mt)) {
+      bool has = table_.get_min_time(&mt);
+      if (!execs_.empty() && (!has || execs_.begin()->first < mt)) {
+        mt = execs_.begin()->first;
+        has = true;
+      }
+      if (has) {
         state_ = ONLY_BUFFERED;
         t_ = bin_start(mt, slide_);
       } else {

@@ -45,7 +45,7 @@ constexpr int MAX_ACC = ARROYO_B200_MAX_AGGS + 1;
 constexpr int MAX_SEGS = 512;
 constexpr int MAX_RING = 4096;
 constexpr int RING_INLINE = 64;
-constexpr int MAX_MERGE = 4096;
+constexpr int MAX_MERGE = 4096;  // initial size of the emit kernel's pane table (grown on demand)
 constexpr long long FREE_BIN = LLONG_MIN;
 
 constexpr int THREADS = 256;
@@ -1004,6 +1004,9 @@ class WindowAggOp final : public OpBase {
   PinnedBuf h_out_counts_;
   bool defer_counts_ = false;
   int count_slots_used_ = 0;
+  // slot of the last window whose count was deferred, or -1 when the last run_emit read its count at once (windows past
+  // COUNT_SLOTS do): after the emission the device counter holds that window's count
+  int last_count_slot_ = -1;
   bool counts_pending_ = false;
   cudaEvent_t counts_done_ = nullptr;
   void resolve_deferred();
@@ -1531,15 +1534,29 @@ void WindowAggOp::promote_avg() {
   relayout_blocks(old_n_acc, f64_from);
 }
 
+// Gives pane `bin` a ring slot, creating the pane if needed.  Only called with no launch in flight (the slot_rows of a
+// launch are attributed to the panes that hold the slots when it is absorbed).
 void WindowAggOp::ensure_pane(int64_t bin) {
-  if (panes_.count(bin)) return;
+  auto it = panes_.find(bin);
+  if (it != panes_.end() && it->second.slot >= 0) return;
   const uint64_t q = (uint64_t)bin / (uint64_t)slide_;
+  uint32_t slot;
   while (true) {
-    uint32_t slot = (uint32_t)q & (ring_ - 1);
+    slot = (uint32_t)q & (ring_ - 1);
     if (h_pane_bins_[slot] == FREE_BIN) break;
+    if (ring_ == MAX_RING) {
+      // Live panes MAX_RING slides apart (a row far ahead of the stream, a long gap before the watermark catches up):
+      // the pane in the slot gives it up and keeps its block.  Rows that arrive for it later are deferred, and it gets
+      // a slot back the same way, so a ring slot is a cache entry and the event-time spread of live panes is unbounded.
+      auto old = panes_.find(h_pane_bins_[slot]);
+      AB_REQUIRE(old != panes_.end(), ARROYO_B200_RUNTIME, "ring slot of an unknown pane");
+      old->second.slot = -1;
+      h_pane_bins_[slot] = FREE_BIN;
+      h_pane_ptrs_[slot] = nullptr;
+      ring_dirty_ = true;
+      break;
+    }
     // slot conflict: double the ring and re-place every live pane
-    AB_REQUIRE(ring_ * 2 <= MAX_RING, ARROYO_B200_RUNTIME,
-               "event-time spread of live panes exceeds the pane ring (4096 panes)");
     ring_ *= 2;
     std::fill(h_pane_bins_.begin(), h_pane_bins_.end(), FREE_BIN);
     std::fill(h_pane_ptrs_.begin(), h_pane_ptrs_.end(), nullptr);
@@ -1552,13 +1569,15 @@ void WindowAggOp::ensure_pane(int64_t bin) {
     }
     ring_dirty_ = true;
   }
-  Pane p;
-  p.bin = bin;
-  p.dev = acquire_block();
-  p.slot = (int)((uint32_t)q & (ring_ - 1));
-  h_pane_bins_[p.slot] = bin;
-  h_pane_ptrs_[p.slot] = p.dev;
-  panes_[bin] = p;
+  if (it == panes_.end()) {
+    Pane p;
+    p.bin = bin;
+    p.dev = acquire_block();
+    it = panes_.emplace(bin, p).first;
+  }
+  it->second.slot = (int)slot;
+  h_pane_bins_[slot] = bin;
+  h_pane_ptrs_[slot] = it->second.dev;
   ring_dirty_ = true;
 }
 
@@ -1935,7 +1954,8 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
   p.slide_div = FastDivU64::make((uint64_t)slide_);
   p.slide = slide_;
   p.late_bin = late_bin_;
-  p.late_q = late_bin_ == LLONG_MIN ? 0ull : (unsigned long long)late_bin_ / (unsigned long long)slide_;
+  // no watermark yet, or a negative one: no row with a timestamp >= 0 is late
+  p.late_q = late_bin_ <= 0 ? 0ull : (unsigned long long)late_bin_ / (unsigned long long)slide_;
   p.guard_vals = avg_exact_ ? guard_vals_ : 0u;
   p.combine = (cfg.flags & ARROYO_B200_FLAG_NO_COMBINE) ? 0 : 1;
   p.rows_slot = rows_slot_;
@@ -2113,10 +2133,15 @@ void WindowAggOp::drain_deferred() {
     explicit Guard(bool& x) : f(x) { f = true; }
     ~Guard() { f = false; }
   } guard(draining_);
-  for (int iter = 0; iter < 64; ++iter) {
+  // Each pass places what it can; panes that alias one ring slot at MAX_RING get it one per pass (ensure_pane), so the
+  // number of passes is not bounded, only their progress: give up after 64 passes in a row that deferred no fewer rows.
+  uint64_t prev = UINT64_MAX;
+  for (int stalls = 0; stalls < 64;) {
     if (!have_counters_ || last_counters_.deferred == 0) return;
     AB_REQUIRE(in_flight_.empty(), ARROYO_B200_RUNTIME, "drain with launches in flight");
     const uint64_t n = last_counters_.deferred;
+    stalls = n < prev ? 0 : stalls + 1;
+    prev = n;
     AB_REQUIRE(n <= defer_cap_, ARROYO_B200_RUNTIME, "deferred overflow");
     st_.rows_deferred += n;
     // which panes do the deferred rows need?
@@ -2226,13 +2251,19 @@ WindowAggOp::OutSet* WindowAggOp::out_set(size_t i, uint64_t cap) {
 // Runs the merge/emit kernel; returns the number of output rows (synchronises on the count).
 int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& blocks, int n_add, bool use_running,
                               bool partial, int64_t wstart, int64_t wend, int64_t ts, OutSet* os) {
-  AB_REQUIRE(blocks.size() <= (size_t)MAX_MERGE, ARROYO_B200_RUNTIME, "too many panes in one window");
+  AB_REQUIRE(blocks.size() <= (size_t)INT_MAX, ARROYO_B200_RUNTIME, "too many panes in one window");
   const uint32_t n_ids = n_keys_host_;
   EmitParams p{};
   p.panes_inline = blocks.size() <= (size_t)EMIT_INLINE ? 1 : 0;
   if (p.panes_inline) {
     for (size_t i = 0; i < blocks.size(); ++i) p.inline_panes[i] = blocks[i];
   } else {
+    // a window re-merges every pane block it holds, two per pane after a checkpoint or a restore: grow the table
+    // (earlier emit kernels may still read the old one)
+    if (blocks.size() * sizeof(void*) > d_emit_panes_.bytes) {
+      AB_CUDA(cudaStreamSynchronize(stream_));
+      d_emit_panes_.alloc(std::max(blocks.size(), d_emit_panes_.bytes / sizeof(void*) * 2) * sizeof(void*));
+    }
     AB_CUDA(cudaMemcpyAsync(d_emit_panes_.p, blocks.data(), blocks.size() * sizeof(void*), cudaMemcpyHostToDevice, stream_));
   }
   p.panes = d_emit_panes_.as<const unsigned long long*>();
@@ -2322,6 +2353,7 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
   ++st_.emit_launches;
   if (deferred) {
     const int slot = count_slots_used_++;
+    last_count_slot_ = slot;
     AB_CUDA(cudaMemcpyAsync(h_out_counts_.as<unsigned int>() + slot, d_out_count_.p, sizeof(unsigned int),
                             cudaMemcpyDeviceToHost, stream_));
     counts_pending_ = true;
@@ -2334,6 +2366,7 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
   const unsigned int out_now = *h_out_count_.as<unsigned int>();
   const int64_t n_out = (int64_t)(unsigned int)(out_now - out_count_base_);
   out_count_base_ = out_now;
+  last_count_slot_ = -1;
   for (auto& d : dup_cols)
     if (n_out) AB_CUDA(cudaMemcpyAsync(d.second, d.first, (size_t)n_out * 8, cudaMemcpyDeviceToDevice, stream_));
   return n_out;
@@ -2605,7 +2638,7 @@ void WindowAggOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vecto
     ring_dirty_ = true;
   }
   // make the pane at the watermark resident so the next rows do not defer
-  if (wm != INT64_MAX && max_bin_seen_ != LLONG_MIN) {
+  if (wm != INT64_MAX && max_bin_seen_ != LLONG_MIN && late_bin_ >= 0) {
     if (!panes_.count(late_bin_)) {
       uint32_t slot = (uint32_t)((uint64_t)late_bin_ / (uint64_t)slide_) & (ring_ - 1);
       if (h_pane_bins_[slot] == FREE_BIN && late_bin_ <= max_bin_seen_ + 2 * slide_) ensure_pane(late_bin_);
@@ -2658,7 +2691,10 @@ void WindowAggOp::resolve_deferred() {
     if (d.n_rows) kept.push_back(d);
   }
   pending_dev.swap(kept);
-  if (count_slots_used_ > 0) out_count_base_ = h[count_slots_used_ - 1];  // the counter's value after its last restart
+  // the counter's value after its last restart: the last deferred window's count, unless windows past COUNT_SLOTS were
+  // counted at once after it (run_emit has already set the base from the counter then)
+  if (last_count_slot_ >= 0) out_count_base_ = h[last_count_slot_];
+  last_count_slot_ = -1;
   count_slots_used_ = 0;
   collect_emit_times();
 }

@@ -298,27 +298,39 @@ class _WindowAggregate(_NativeOperator):
         _check(self._lib, self._h, st)
 
     def handle_watermark_device(self, wm: int, max_out: int = 64):
-        """Emission left on the device: list of (n_rows, [device pointers])."""
+        """Emission left on the device: list of (n_rows, [device pointers]).  The library hands out at most `max_out`
+        windows per call and queues the rest; they are collected here with further polls."""
         out = getattr(self, "_dev_out", None)
         if out is None or len(out) < max_out:
             out = self._dev_out = (ffi.DeviceBatch * max_out)()  # reused: building it costs more than the call
         n = C.c_int64(0)
         st = self._lib.arroyo_b200_op_handle_watermark_device(self._h, clamp_watermark(wm), out, max_out, C.byref(n))
         _check(self._lib, self._h, st)
-        return [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+        got = [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+        return got + self._drain_device(max_out, n.value)
+
+    def _drain_device(self, max_out: int, n: int):
+        got = []
+        while n == max_out and max_out > 0:
+            more = self.handle_watermark_device_poll(max_out, drain=False)
+            got += more
+            n = len(more)
+        return got
 
     def handle_watermark_device_begin(self, wm: int):
         """First half of handle_watermark_device: the emission is enqueued, its row counts are not awaited."""
         _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark_device_begin(self._h, clamp_watermark(wm)))
 
-    def handle_watermark_device_poll(self, max_out: int = 64):
-        """Second half: the windows of the outstanding emission, list of (n_rows, [device pointers])."""
+    def handle_watermark_device_poll(self, max_out: int = 64, drain: bool = True):
+        """Second half: the windows of the outstanding emission, list of (n_rows, [device pointers]).  With `drain`,
+        polls until the library has no window queued (it hands out at most `max_out` per call)."""
         out = getattr(self, "_dev_out", None)
         if out is None or len(out) < max_out:
             out = self._dev_out = (ffi.DeviceBatch * max_out)()
         n = C.c_int64(0)
         _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark_device_poll(self._h, out, max_out, C.byref(n)))
-        return [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+        got = [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+        return got + (self._drain_device(max_out, n.value) if drain else [])
 
     def handle_checkpoint(self, barrier, ctx: OperatorContext, collector: Collector):
         if not self.created:
@@ -488,7 +500,11 @@ class SessionAggregatingWindowFunc(_NativeOperator):
         n = C.c_int64(0)
         st = self._lib.arroyo_b200_op_handle_watermark_device(self._h, clamp_watermark(wm), out, max_out, C.byref(n))
         _check(self._lib, self._h, st)
-        return [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+        got = [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+        while n.value == max_out and max_out > 0:  # windows beyond max_out stay queued in the library
+            _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark_device_poll(self._h, out, max_out, C.byref(n)))
+            got += [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+        return got
 
 
 class UpdatingAggregatingFunc(_NativeOperator):

@@ -342,7 +342,10 @@ int32_t arroyo_b200_op_run_batches(ArroyoB200Op* op, struct ArrowArray* batches,
                                     ArroyoB200Batches* out, int64_t* n_consumed);
 
 /* Same, leaving the emitted windows on the device.  `out` must have room for `max_out`
- * entries; `*n_out` receives the number written (excess windows are an error). */
+ * entries; `*n_out` receives the number written.  Windows beyond the first `max_out` stay queued, in
+ * order, and handle_watermark_device_poll returns them (again at most `max_out` per call): no emitted
+ * window is lost.  While windows are queued, handle_watermark_device and _begin refuse a new emission
+ * with INVALID_ARGUMENT (the queued windows live in the buffers it would write). */
 int32_t arroyo_b200_op_handle_watermark_device(ArroyoB200Op* op, int64_t watermark_ns,
                                                ArroyoB200DeviceBatch* out, int64_t max_out, int64_t* n_out);
 

@@ -645,7 +645,10 @@ class SlidingAggregatingWindowFunc:
             for p in ex.finished:
                 self.tier.insert(p, b)
         table.flush_timestamp(bin_end)
-        table.expire_timestamp(bin_end - self.width + self.slide)
+        # The reference expires bin_end - width + slide here: the oldest pane of the NEXT window, which its in-memory
+        # tier still holds.  A checkpoint taken now would then restore that window without it.  Expire the pane that
+        # has just left instead, so the table always holds what the tier holds.
+        table.expire_timestamp(bin_end - self.width)
         interval_start, interval_end = bin_end - self.width, bin_end
         partials: List[Batch] = []
         cur = interval_start
@@ -654,7 +657,11 @@ class SlidingAggregatingWindowFunc:
             cur += self.slide
         self.tier.delete_before(bin_end + self.slide - self.width)
         if self.tier.is_empty():
+            # the reference consults only the table here and would never emit the panes still pending in `execs`
+            # (rows that arrived while the store was non-empty and were not checkpointed): they are candidates too
             mt = table.get_min_time()
+            if self.execs and (mt is None or min(self.execs) < mt):
+                mt = min(self.execs)
             self.state = (self.ONLY_BUFFERED, bin_start(mt, self.slide)) if mt is not None else (self.NO_DATA, None)
         else:
             self.state = (self.IN_MEMORY, bin_end)

@@ -41,7 +41,11 @@ static inline uint64_t mix64(uint64_t x) {
   return z ^ (z >> 31);
 }
 
-static inline int64_t bin_start(int64_t ts, int64_t w) { return w == 0 ? ts : ts - ts % w; }
+static inline int64_t bin_start(int64_t ts, int64_t w) {  /* floor: a negative watermark bins below zero */
+  if (w == 0) return ts;
+  int64_t r = ts % w;
+  return ts - (r < 0 ? r + w : r);
+}
 
 /* ---------------- group hash table (key -> accumulators) ---------------- */
 typedef struct {
@@ -383,9 +387,10 @@ static void sliding_advance(OracleOp* op, OracleOut* out) {
   }
   /* flush_timestamp(bin_end) */
   if (set_erase(&op->to_flush, bin_end)) set_insert(&op->flushed, bin_end);
-  /* expire_timestamp(bin_end - width + slide) */
-  set_erase(&op->flushed, bin_end - op->width + op->slide);
-  set_erase(&op->to_flush, bin_end - op->width + op->slide);
+  /* expire_timestamp: the pane that has just left (the reference expires bin_end - width + slide, the oldest pane of the
+     NEXT window, which its tier still holds; see oracle/arroyo_oracle.py) */
+  set_erase(&op->flushed, bin_end - op->width);
+  set_erase(&op->to_flush, bin_end - op->width);
   emit_window(op, bin_end - op->width, bin_end, out);
   /* delete_before(bin_end + slide - width) */
   int64_t cutoff = bin_start(bin_end + op->slide - op->width, op->slide);
@@ -400,8 +405,15 @@ static void sliding_advance(OracleOp* op, OracleOut* out) {
     ++i;
   }
   if (tier_empty) {
+    /* panes still pending (not in the tier) are candidates as well as the table: the reference looks only at the
+       table and would never emit rows that arrived while the store was non-empty and were not checkpointed */
     int64_t mt;
-    if (tbl_min(op, &mt)) { op->state = ST_ONLY_BUFFERED; op->state_t = bin_start(mt, op->slide); }
+    int has = tbl_min(op, &mt);
+    for (size_t i = 0; i < op->n_panes; ++i) {
+      const Pane* q = &op->panes[i];
+      if (!q->in_tier && (!has || q->bin < mt)) { mt = q->bin; has = 1; }
+    }
+    if (has) { op->state = ST_ONLY_BUFFERED; op->state_t = bin_start(mt, op->slide); }
     else op->state = ST_NO_DATA;
   } else {
     op->state = ST_IN_MEMORY;

@@ -8,6 +8,8 @@ AVG path is exact up to its one final division, so the result must be bit-identi
 Otherwise |got - mean| <= 2u * sum|x| + 2u * |mean| with u = 2^-53: that is n * 2u * sum|x| on the sum, the error
 bound of an f64 sum of n terms in any order including the rounding of each input, divided by n, plus the final
 division."""
+import bisect
+import itertools
 from fractions import Fraction
 
 import numpy as np
@@ -108,31 +110,190 @@ def window_rows(batches, key_name, aggs, width, slide=None):
     """Expected output of a tumbling (slide None) or sliding window aggregate over rows that are never late:
     {(window_start, key or None): {column: value}} with window_end, _timestamp = window_end - 1 and the
     aggregates (AVG as a Mean)."""
+    emitted, _ = window_emissions([("batch", b) for b in batches] + [("wm", INT64_MAX)], key_name, aggs, width, slide)
+    return emitted[0]
+
+
+def _bin(t: int, slide: int) -> int:
+    return t - t % slide  # Python's % floors: a negative watermark bins below zero
+
+
+class _Panes:
+    """Per-(pane, key) partial states of the on-time rows: {pane: {key: [rows, state per aggregate]}}.  A state is
+    the wrapping-free exact sum (SUM), the value (MIN / MAX) or (exact sum, sum of |x|) (AVG); COUNT uses `rows`."""
+
+    def __init__(self, key_name, aggs, slide):
+        self.key_name, self.aggs, self.slide = key_name, list(aggs), slide
+        self.by_pane = {}
+
+    def add(self, cols, ts):
+        n = len(ts)
+        if n == 0:
+            return
+        panes = ts - ts % np.int64(self.slide)
+        key = np.asarray(cols[self.key_name]) if self.key_name else np.zeros(n, dtype=np.int64)
+        uniq, inv, n_groups = _group_keys(key, panes)
+        vals = _aggregate(cols, inv, n_groups, self.aggs)
+        count = np.bincount(inv, minlength=n_groups)
+        for g in range(n_groups):
+            pane, k = int(uniq[0, g]), int(uniq[1, g])
+            new = [int(count[g])]
+            for a in self.aggs:
+                v = vals[a.name][g]
+                new.append((int(v.exact * int(count[g])), v.abs_sum) if a.kind == "avg" else int(v))
+            keys = self.by_pane.setdefault(pane, {})
+            old = keys.get(k)
+            keys[k] = new if old is None else self._merge(old, new)
+
+    def _merge(self, x, y):
+        out = [x[0] + y[0]]
+        for i, a in enumerate(self.aggs, 1):
+            if a.kind == "min":
+                out.append(min(x[i], y[i]))
+            elif a.kind == "max":
+                out.append(max(x[i], y[i]))
+            elif a.kind == "avg":
+                out.append((x[i][0] + y[i][0], x[i][1] + y[i][1]))
+            else:  # count (unused: rows), sum (exact, wrapped on output)
+                out.append(x[i] + y[i])
+        return out
+
+    def windows(self, starts, width, key_out):
+        """Rows of the windows starting at `starts` (ascending) that hold at least one row, in (start, key) order."""
+        per_key = {}
+        for pane in sorted(self.by_pane):
+            for k, st in self.by_pane[pane].items():
+                per_key.setdefault(k, []).append((pane, st))
+        starts = np.asarray(starts, dtype=object)
+        rows = []
+        for k, items in per_key.items():
+            bins = [p for p, _ in items]
+            i0 = [bisect.bisect_left(bins, s) for s in starts]
+            i1 = [bisect.bisect_left(bins, s + width) for s in starts]
+            pre = [list(itertools.accumulate((st[0] for _, st in items), initial=0))]
+            mins = {}
+            for i, a in enumerate(self.aggs, 1):
+                if a.kind in ("min", "max"):
+                    mins[i] = _RangeExtreme([st[i] for _, st in items], a.kind)
+                    pre.append(None)
+                elif a.kind == "avg":
+                    pre.append((list(itertools.accumulate((st[i][0] for _, st in items), initial=0)),
+                                list(itertools.accumulate((st[i][1] for _, st in items), initial=0))))
+                else:
+                    pre.append(list(itertools.accumulate((st[i] for _, st in items), initial=0)))
+            for s, a0, a1 in zip(starts, i0, i1):
+                if a1 <= a0:
+                    continue
+                n = pre[0][a1] - pre[0][a0]
+                row = {"window_start": int(s), "window_end": int(s) + width, TIMESTAMP: int(s) + width - 1}
+                if self.key_name:
+                    row[self.key_name] = key_out(k)
+                for i, a in enumerate(self.aggs, 1):
+                    if a.kind == "count":
+                        row[a.name] = n
+                    elif a.kind == "sum":
+                        row[a.name] = _wrap(pre[i][a1] - pre[i][a0])
+                    elif a.kind == "avg":
+                        ex, ab = pre[i]
+                        row[a.name] = Mean(Fraction(ex[a1] - ex[a0], n), ab[a1] - ab[a0])
+                    else:
+                        row[a.name] = mins[i].query(a0, a1)
+                rows.append(row)
+        rows.sort(key=lambda r: (r["window_start"], -1 if r.get(self.key_name) is None else r[self.key_name]))
+        return rows
+
+    def prune(self, below: int):
+        for p in [p for p in self.by_pane if p < below]:
+            del self.by_pane[p]
+
+
+def _wrap(x: int) -> int:
+    x &= (1 << 64) - 1
+    return x - (1 << 64) if x >= 1 << 63 else x
+
+
+class _RangeExtreme:
+    """MIN or MAX over index ranges [i0, i1) of a list: a sparse table."""
+
+    def __init__(self, vals, kind):
+        self.f = min if kind == "min" else max
+        self.levels = [list(vals)]
+        j = 1
+        while 2 * j <= len(vals):
+            prev = self.levels[-1]
+            self.levels.append([self.f(prev[i], prev[i + j]) for i in range(len(prev) - j)])
+            j *= 2
+
+    def query(self, i0, i1):
+        lv = (i1 - i0).bit_length() - 1
+        t = self.levels[lv]
+        return self.f(t[i0], t[i1 - (1 << lv)])
+
+
+def window_emissions(events, key_name, aggs, width, slide=None):
+    """The event-time behaviour of the tumbling (slide None) and sliding window aggregates, from these rules
+    (tumbling_aggregating_window.rs:282-291 and :321-392, sliding_aggregating_window.rs:631-633 and :676-691):
+
+    * bin(t) = t - t mod slide with floor division (tumbling: slide = width);
+    * a row is late iff bin(ts) < bin(w) for the last watermark w before its batch; before the first watermark nothing
+      is late; a late row counts in no window;
+    * an on-time row belongs to the windows starting at bin(ts) - k * slide, 0 <= k < width / slide;
+    * watermark w emits, in ascending window_start, every window that holds an on-time row, has not been emitted
+      and ends at or before bin(w) (start + width <= bin(w)); end of data is INT64_MAX;
+    * a restart (checkpoint, new operator, on_start) changes nothing.
+
+    `events`: ("batch", cols), ("wm", w) or ("restart",); watermarks must not decrease.  Returns (one
+    {(window_start, key or None): row} per watermark, in emission order, the number of late rows)."""
     slide = slide or width
-    assert width % slide == 0
-    cols = _concat(batches)
-    ts = cols[TIMESTAMP].astype(np.int64)
-    first = ts - ts % np.int64(slide)
-    reps = width // slide
-    starts = np.concatenate([first - np.int64(k * slide) for k in range(reps)])
-    rows = np.tile(np.arange(len(ts)), reps)
-    expanded = {c: v[rows] for c, v in cols.items()}
-    key = expanded[key_name] if key_name else np.zeros(len(rows), dtype=np.int64)
-    uniq, inv, n = _group_keys(key, starts)
-    vals = _aggregate(expanded, inv, n, aggs)
-    out = {}
-    for g in range(n):
-        ws = int(uniq[0, g])
-        kv = None
-        if key_name:
-            kv = int(np.int64(uniq[1, g]).view(np.uint64)) if cols[key_name].dtype == np.uint64 else int(uniq[1, g])
-        row = {"window_start": ws, "window_end": ws + width, TIMESTAMP: ws + width - 1}
-        if key_name:
-            row[key_name] = kv
-        for a in aggs:
-            row[a.name] = vals[a.name][g]
-        out[(ws, kv)] = row
-    return out
+    assert width % slide == 0 and slide > 0
+    panes = _Panes(key_name, aggs, slide)
+    last_wm, bound, late = None, None, 0
+    dtype = None
+    out = []
+    for ev in events:
+        if ev[0] == "restart":
+            continue
+        if ev[0] == "batch":
+            cols = {c: np.asarray(v) for c, v in _columns(ev[1]).items()}
+            ts = cols[TIMESTAMP].astype(np.int64)
+            if key_name and len(ts):
+                dtype = cols[key_name].dtype
+            keep = np.ones(len(ts), dtype=bool)
+            if last_wm is not None:
+                keep = (ts - ts % np.int64(slide)) >= _bin(last_wm, slide)
+            late += int((~keep).sum())
+            panes.add({c: v[keep] for c, v in cols.items()}, ts[keep])
+            continue
+        assert ev[0] == "wm", ev
+        w = min(int(ev[1]), INT64_MAX)
+        if last_wm is not None and w < last_wm:
+            raise ValueError("watermarks must not decrease")
+        last_wm = w
+        new_bound = _bin(w, slide)
+        lo = None if bound is None else bound - width  # windows starting at or below lo were emitted
+        hi = new_bound - width
+        # the windows a pane belongs to start in [pane - width + slide, pane]: merge those runs, keep (lo, hi]
+        starts, run = [], None
+        for pane in sorted(panes.by_pane):
+            a, b = pane - width + slide, min(pane, hi)
+            if lo is not None:
+                a = max(a, lo + slide)
+            if a > b:
+                continue
+            if run is not None and a <= run[1] + slide:
+                run[1] = max(run[1], b)
+                continue
+            if run is not None:
+                starts.extend(range(run[0], run[1] + 1, slide))
+            run = [a, b]
+        if run is not None:
+            starts.extend(range(run[0], run[1] + 1, slide))
+        key_out = (lambda k: int(np.int64(k).view(np.uint64))) if dtype == np.uint64 else int
+        rows = panes.windows(starts, width, key_out)
+        out.append({(r["window_start"], r[key_name] if key_name else None): r for r in rows})
+        bound = new_bound if bound is None else max(bound, new_bound)
+        panes.prune(bound - width + 1)
+    return out, late
 
 
 def updating_rows(batches, key_name, aggs):

@@ -79,6 +79,43 @@ def test_exact_reference_avg_rule():
     assert not X.check_avg(0.0, big)
 
 
+
+# ---- event time: the window oracle against window_emissions, watermark by watermark ----
+TIME_SHAPES = ["T1", "T2", "T3", "T4:1", "T4:n-1", "T4:n", "T4:n+1", "T4:4095", "T4:4096", "T4:4097", "T4:1000000", "T5", "T5:wide",
+               "T6:1", "T6:2", "T6:4", "T6:4095", "T6:4096", "T6:4097", "T6:5000", "T6:1000000", "T7:16", "T7:17",
+               "T7:600", "T7:3600", "T7:4096", "T7:4097", "T8:zero", "T8:neg", "T8:big@30d", "T8:zero@2", "T8:zero@3",
+               "T8:big@p", "T8:big@2^32-1", "T8:big@2^32+1", "T8:neg@p", "T9"]
+
+
+@pytest.mark.parametrize("kind", ["tumbling", "running"])
+def test_window_oracle_event_time_matches_exact_reference(kind):
+    from tests import test_gpu_window_time as T
+    for i, shape in enumerate(TIME_SHAPES):
+        keys = ("few", "many", "none")[i % 3]
+        plan = ("ints", "minmax")[i % 2]
+        st = T._shape(shape, kind)(keys)
+        cfg = T.config(st, kind, plan)
+        want, _ = T.reference(st, cfg)
+        T.check_emissions(want, T.run_oracle(st, kind, cfg), cfg, f"oracle {shape}")
+
+
+def test_window_emissions_by_hand():
+    """The event-time rules on a stream small enough to follow by hand (tumbling width 10, sliding 20 / 10)."""
+    aggs = [A("count", None, "n"), A("sum", "a", "s")]
+    b1 = {"a": np.array([1, 2, 3, 4], dtype=np.int64), X.TIMESTAMP: np.array([3, 12, 19, 25], dtype=np.int64)}
+    b2 = {"a": np.array([10, 20, 30, 40], dtype=np.int64), X.TIMESTAMP: np.array([9, 10, 14, 15], dtype=np.int64)}
+    ev = [("wm", -25), ("batch", b1), ("wm", 15), ("batch", b2), ("restart",), ("wm", 20), ("wm", 20), ("wm", X.INT64_MAX)]
+    out, late = X.window_emissions(ev, None, aggs, 10)
+    assert late == 1  # ts 9: bin 0 < bin(15) = 10; ts 10 and 14 are in [bin(w), w), ts 15 is at w
+    assert [list(o) for o in out] == [[], [(0, None)], [(10, None)], [], [(20, None)]]
+    assert out[1][(0, None)]["n"] == 1 and out[2][(10, None)]["s"] == 2 + 3 + 20 + 30 + 40
+    out, late = X.window_emissions(ev, None, aggs, 20, 10)
+    assert late == 1
+    assert [list(o) for o in out] == [[], [(-10, None)], [(0, None)], [], [(10, None), (20, None)]]
+    assert out[2][(0, None)]["n"] == 6 and out[4][(20, None)]["s"] == 4
+    with pytest.raises(ValueError):
+        X.window_emissions([("wm", 5), ("wm", 4)], None, aggs, 10)
+
 # ---- joins: the oracles' InstantJoin (numpy and C) and JoinWithExpiration against the exact reference joins ----
 INSTANT_SHAPES = ["left_smaller", "right_smaller", "equal", "zero_eligible", "left_only", "right_only", "build_1",
                   "build_511", "build_513", "edge_keys", "u64_keys", "ts_keys", "many_instants", "ts_2p32", "ts_eq_wm",
