@@ -29,6 +29,8 @@
 #include <climits>
 #include <cstdlib>
 
+#include <cub/device/device_segmented_sort.cuh>
+
 #include "dict.cuh"
 #include "op.h"
 #include "scan.cuh"
@@ -77,8 +79,11 @@ struct SessCtx {
 };
 
 enum : unsigned long long { ERR_POOL = 1, ERR_ADD_FLUSHED = 2, ERR_BEFORE_START = 4, ERR_OUT = 8, ERR_LOOP = 16 };
-// every device loop over the linked lists is bounded: a corrupted list must surface as an error, never as a hang
-constexpr int LOOP_GUARD = 1 << 20;
+// Every device loop over the linked lists is bounded: a corrupted list must surface as an error, never as a hang.  The
+// bound is what a sound list can take: a list holds at most node_cap nodes; a fill visits each node at most twice
+// (pop_first's walk, then add_batch) and allocates its remainders from the same pool; and every session a watermark
+// opens consumes at least one pending row, so it opens and closes at most node_cap sessions.
+__device__ __forceinline__ unsigned long long loop_guard(const SessCtx& c) { return 3 * c.node_cap + 8; }
 
 struct RowsRef {
   const long long* ts;
@@ -216,11 +221,12 @@ __device__ void pending_insert(const SessCtx& c, uint32_t id, int node) {
   if (node < 0) return;
   const long long start = c.n_start[node];
   int prev = -1, cur = c.head[id];
-  int guard = 0;
+  unsigned long long guard = 0;
+  const unsigned long long limit = loop_guard(c);
   while (cur >= 0 && c.n_start[cur] <= start) {
     prev = cur;
     cur = c.n_next[cur];
-    if (++guard > LOOP_GUARD) {
+    if (++guard > limit) {
       set_err(c, ERR_LOOP);
       return;
     }
@@ -241,9 +247,10 @@ __device__ RowsRef pool_rows(const SessCtx& c, int node) {
 
 // KeyComputingHolder::fill_active_session (:610-643)
 __device__ void fill_active_session(const SessCtx& c, uint32_t id, Tally& tally) {
-  int guard = 0;
+  unsigned long long guard = 0;
+  const unsigned long long limit = loop_guard(c);
   while (true) {
-    if (++guard > LOOP_GUARD) {
+    if (++guard > limit) {
       set_err(c, ERR_LOOP);
       return;
     }
@@ -255,7 +262,7 @@ __device__ void fill_active_session(const SessCtx& c, uint32_t id, Tally& tally)
     int tail = h;
     while (c.n_next[tail] >= 0 && c.n_start[c.n_next[tail]] == first) {
       tail = c.n_next[tail];
-      if (++guard > LOOP_GUARD) {
+      if (++guard > limit) {
         set_err(c, ERR_LOOP);
         return;
       }
@@ -263,7 +270,7 @@ __device__ void fill_active_session(const SessCtx& c, uint32_t id, Tally& tally)
     c.head[id] = c.n_next[tail];
     c.n_next[tail] = -1;
     for (int node = h; node >= 0;) {
-      if (++guard > LOOP_GUARD) {
+      if (++guard > limit) {
         set_err(c, ERR_LOOP);
         return;
       }
@@ -318,9 +325,10 @@ __device__ void finish_session(const SessCtx& c, uint32_t id, Tally& tally) {
 
 // KeyComputingHolder::watermark_update (:557-603)
 __device__ void watermark_update(const SessCtx& c, uint32_t id, long long wm, bool in_add, Tally& tally) {
-  int guard = 0;
+  unsigned long long guard = 0;
+  const unsigned long long limit = loop_guard(c);
   while (true) {
-    if (++guard > LOOP_GUARD) {
+    if (++guard > limit) {
       set_err(c, ERR_LOOP);
       return;
     }
@@ -367,6 +375,7 @@ struct PrepParams {
   long long wm;
   int keyed, n_vals;
   DictView dict;
+  unsigned int* min_key_seen;  // set when a row with the INT64_MIN key (id 0, not counted by the dictionary) is kept
   // launch arena (unordered)
   unsigned int* a_id;
   unsigned int* a_seq;
@@ -400,6 +409,7 @@ __global__ void __launch_bounds__(ST) prep_kernel(const __grid_constant__ PrepPa
     }
     if (keep && p.keyed) {
       const long long key = __ldcs(p.key + i);
+      if (key == EMPTY_KEY) *p.min_key_seen = 1u;
       id = key == EMPTY_KEY ? 0u : dict_insert(p.dict, key, dict_home((uint64_t)key, p.dict.cap));
       if (id >= ID_OVERFLOW) {
         atomicOr(p.ctr + 5, (unsigned long long)ERR_POOL);
@@ -432,9 +442,9 @@ __global__ void __launch_bounds__(ST) prep_kernel(const __grid_constant__ PrepPa
 
 struct GroupParams {
   const unsigned int* a_id;
-  const unsigned int* a_seq;
-  const long long* a_ts;
-  const long long* a_val[SV];
+  unsigned int* a_seq;  // written back only by the segmented sort of big keys, which parks rows here
+  long long* a_ts;
+  long long* a_val[SV];
   unsigned long long n;
   int n_vals;
   const unsigned long long* offset;  // per id
@@ -453,6 +463,56 @@ __global__ void __launch_bounds__(ST) group_kernel(const __grid_constant__ Group
     p.g_seq[o] = p.a_seq[i];
     p.g_ts[o] = p.a_ts[i];
     for (int v = 0; v < p.n_vals; ++v) p.g_val[v][o] = p.a_val[v][i];
+  }
+}
+
+// Keys with more rows than this in one launch are sorted by a device-wide segmented sort instead of one thread.
+constexpr unsigned int SMALL_SORT = 16;
+
+// the keys with more than SMALL_SORT rows in this launch: their grouped ranges [begin, end)
+__global__ void big_keys_kernel(unsigned int n_ids, const unsigned int* count, const unsigned long long* offset,
+                                unsigned int* seg_begin, unsigned int* seg_end, unsigned int* n_seg) {
+  unsigned int id = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned int stride = gridDim.x * blockDim.x;
+  for (; id < n_ids; id += stride) {
+    const unsigned int cnt = count[id];
+    if (cnt <= SMALL_SORT) continue;
+    const unsigned int s = atomicAdd(n_seg, 1u);
+    seg_begin[s] = (unsigned int)offset[id];
+    seg_end[s] = (unsigned int)(offset[id] + cnt);
+  }
+}
+
+// one block per big key: park its grouped rows in the (now unused) launch arena at the same positions, and seed the
+// sort with the timestamps and the identity permutation
+__global__ void big_park_kernel(const unsigned int* seg_begin, const unsigned int* seg_end, GroupParams g,
+                                long long* key, unsigned int* idx) {
+  const unsigned int b = seg_begin[blockIdx.x], e = seg_end[blockIdx.x];
+  for (unsigned int i = b + threadIdx.x; i < e; i += blockDim.x) {
+    g.a_seq[i] = g.g_seq[i];
+    g.a_ts[i] = g.g_ts[i];
+    for (int v = 0; v < g.n_vals; ++v) g.a_val[v][i] = g.g_val[v][i];
+    key[i] = g.g_ts[i];
+    idx[i] = i;
+  }
+}
+
+// after the stable sort by ts: the batch number of each row, in that order, as the key of the second stable sort
+__global__ void big_seq_kernel(const unsigned int* seg_begin, const unsigned int* seg_end, const unsigned int* a_seq,
+                               const unsigned int* idx, unsigned int* seq) {
+  const unsigned int b = seg_begin[blockIdx.x], e = seg_end[blockIdx.x];
+  for (unsigned int i = b + threadIdx.x; i < e; i += blockDim.x) seq[i] = a_seq[idx[i]];
+}
+
+// rows back into the row pool in (batch, ts) order
+__global__ void big_gather_kernel(const unsigned int* seg_begin, const unsigned int* seg_end, GroupParams g,
+                                  const unsigned int* idx) {
+  const unsigned int b = seg_begin[blockIdx.x], e = seg_end[blockIdx.x];
+  for (unsigned int i = b + threadIdx.x; i < e; i += blockDim.x) {
+    const unsigned int src = idx[i];
+    g.g_seq[i] = g.a_seq[src];
+    g.g_ts[i] = g.a_ts[src];
+    for (int v = 0; v < g.n_vals; ++v) g.g_val[v][i] = g.a_val[v][src];
   }
 }
 
@@ -480,8 +540,9 @@ __global__ void __launch_bounds__(128) apply_kernel(const __grid_constant__ Appl
     p.count[id] = 0;
     p.cursor[id] = 0;
     const unsigned long long off = p.offset[id];
-    // order this key's rows by (batch, ts): insertion sort -- a key has few rows per launch
-    for (unsigned int i = 1; i < cnt; ++i) {
+    // order this key's rows by (batch, ts).  A key with more than SMALL_SORT rows in this launch was ordered by the
+    // segmented sort (sort_big_keys); the few rows of any other key are ordered here, at a cost bounded by SMALL_SORT^2.
+    for (unsigned int i = 1; i < cnt && cnt <= SMALL_SORT; ++i) {
       const unsigned int s = p.g_seq[off + i];
       const long long t = p.g_ts[off + i];
       long long vv[SV];
@@ -602,7 +663,18 @@ class SessionOp final : public OpBase {
   void on_close(int, BatchesPriv*) override { flush(); }
   void flush() override;
   void stats(ArroyoB200Stats* out) override {
-    st_.n_keys = keyed_ ? (n_keys_ > 0 ? n_keys_ - 1 : 0) : 0;
+    unsigned long long late = 0;  // current, not as of the last watermark
+    AB_CUDA(cudaMemcpyAsync(&late, late_.p, 8, cudaMemcpyDeviceToHost, stream_));
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    st_.rows_late = late;
+    st_.n_keys = 0;
+    if (keyed_) {
+      // the dictionary's count (ids 1.., id 0 is INT64_MIN's) and whether an INT64_MIN key was accepted
+      unsigned int nk[2] = {1, 0};
+      AB_CUDA(cudaMemcpyAsync(nk, n_keys_dev_.p, sizeof nk, cudaMemcpyDeviceToHost, stream_));
+      AB_CUDA(cudaStreamSynchronize(stream_));
+      st_.n_keys = (uint64_t)(nk[0] - 1) + (nk[1] ? 1 : 0);
+    }
     *out = st_;
   }
 
@@ -640,6 +712,9 @@ class SessionOp final : public OpBase {
   // launch arena
   uint64_t arena_cap_ = 0;
   DevBuf a_id_, a_seq_, a_ts_, a_val_[SV], g_seq_;
+  // segmented sort of the keys with more than SMALL_SORT rows in a launch (sized on first use)
+  uint64_t sort_cap_ = 0;
+  DevBuf s_key_, s_key_out_, s_idx_, s_idx_out_, s_seq_, s_seq_out_, s_begin_, s_end_, s_nseg_, s_tmp_;
   uint64_t arena_rows_bound_ = 0;  // rows prepped since the last apply (upper bound incl. late rows)
   uint32_t seq_ = 0;
   bool has_wm_ = false;
@@ -671,6 +746,7 @@ class SessionOp final : public OpBase {
   void check_err();
   void prep(const long long* key, const long long* ts, const long long* const* vals, int64_t n);
   void apply_pending();
+  void sort_big_keys(const GroupParams& g, uint64_t n);
   void maybe_compact();
   void release_inputs(bool wait);
 };
@@ -753,7 +829,8 @@ SessionOp::SessionOp(const ArroyoB200OpConfig& c) {
   }
   AB_CUDA(cudaMemsetAsync(ctr_.p, 0, 8 * sizeof(unsigned long long), stream_));
   AB_CUDA(cudaMemsetAsync(late_.p, 0, 8, stream_));
-  n_keys_dev_.alloc(sizeof(unsigned int));
+  n_keys_dev_.alloc(2 * sizeof(unsigned int));  // [dictionary count, INT64_MIN key seen]
+  AB_CUDA(cudaMemsetAsync(n_keys_dev_.p, 0, 2 * sizeof(unsigned int), stream_));
   uint64_t want = c.expected_keys ? c.expected_keys : (1ull << 16);
   alloc_keys(keyed_ ? ((want + want / 8 + 2 + 1023) / 1024) * 1024 : 1024);
   AB_CUDA(cudaStreamSynchronize(stream_));
@@ -985,6 +1062,7 @@ void SessionOp::prep(const long long* key, const long long* ts, const long long*
   p.dict.slots = slots_.as<Slot>();
   p.dict.id_keys = id_keys_.as<long long>();
   p.dict.n_keys = n_keys_dev_.as<unsigned int>();
+  p.min_key_seen = n_keys_dev_.as<unsigned int>() + 1;
   p.dict.cap = keyed_ ? (uint32_t)dict_cap_ : 1;
   p.dict.id_cap = (uint32_t)std::min<uint64_t>(id_cap_, 0xFFFFFFF0ull);
   p.dict.dbase = 0;
@@ -1104,6 +1182,7 @@ void SessionOp::apply_pending() {
   }
   group_kernel<<<grid_for(n, ST), ST, 0, stream_>>>(g);
   AB_CUDA(cudaGetLastError());
+  sort_big_keys(g, n);
   ApplyParams a{};
   a.c = ctx();
   a.n_ids = n_keys_;
@@ -1122,6 +1201,62 @@ void SessionOp::apply_pending() {
   st_.kernel_launches += 5;
   read_ctr();
   check_err();
+}
+
+// Orders the grouped rows of every key with more than SMALL_SORT rows in this launch by (batch, ts): two stable
+// segmented sorts (by ts, then by batch) over those keys' ranges, then one gather.  The cost is O(n log n) in the
+// key's rows, where one thread's insertion sort was O(n^2): a hot key, or the unkeyed operator, can hold millions of
+// rows in one launch.
+void SessionOp::sort_big_keys(const GroupParams& g, uint64_t n) {
+  const uint64_t max_seg = n / (SMALL_SORT + 1);
+  if (max_seg == 0) return;
+  if (sort_cap_ < n) {
+    sort_cap_ = std::max<uint64_t>(n, 2 * sort_cap_);
+    s_key_.alloc(sort_cap_ * 8);
+    s_key_out_.alloc(sort_cap_ * 8);
+    s_idx_.alloc(sort_cap_ * 4);
+    s_idx_out_.alloc(sort_cap_ * 4);
+    s_seq_.alloc(sort_cap_ * 4);
+    s_seq_out_.alloc(sort_cap_ * 4);
+    s_begin_.alloc((sort_cap_ / (SMALL_SORT + 1) + 1) * 4);
+    s_end_.alloc((sort_cap_ / (SMALL_SORT + 1) + 1) * 4);
+    s_nseg_.alloc(4);
+  }
+  AB_CUDA(cudaMemsetAsync(s_nseg_.p, 0, 4, stream_));
+  big_keys_kernel<<<grid_for(n_keys_, 256), 256, 0, stream_>>>(n_keys_, count_.as<unsigned int>(), offset_.as<unsigned long long>(),
+                                                               s_begin_.as<unsigned int>(), s_end_.as<unsigned int>(),
+                                                               s_nseg_.as<unsigned int>());
+  AB_CUDA(cudaGetLastError());
+  unsigned int n_seg = 0;
+  AB_CUDA(cudaMemcpyAsync(&n_seg, s_nseg_.p, 4, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  st_.kernel_launches += 1;
+  if (n_seg == 0) return;
+  const unsigned int* sb = s_begin_.as<unsigned int>();
+  const unsigned int* se = s_end_.as<unsigned int>();
+  big_park_kernel<<<n_seg, ST, 0, stream_>>>(sb, se, g, s_key_.as<long long>(), s_idx_.as<unsigned int>());
+  AB_CUDA(cudaGetLastError());
+  size_t t1 = 0, t2 = 0;
+  AB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(nullptr, t1, s_key_.as<long long>(), s_key_out_.as<long long>(),
+                                                    s_idx_.as<unsigned int>(), s_idx_out_.as<unsigned int>(), (int)n,
+                                                    (int)n_seg, sb, se, stream_));
+  AB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(nullptr, t2, s_seq_.as<unsigned int>(), s_seq_out_.as<unsigned int>(),
+                                                    s_idx_out_.as<unsigned int>(), s_idx_.as<unsigned int>(), (int)n,
+                                                    (int)n_seg, sb, se, stream_));
+  const size_t tb = std::max<size_t>(std::max(t1, t2), 1);
+  if (s_tmp_.bytes < tb) s_tmp_.alloc(tb);
+  AB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(s_tmp_.p, t1, s_key_.as<long long>(), s_key_out_.as<long long>(),
+                                                    s_idx_.as<unsigned int>(), s_idx_out_.as<unsigned int>(), (int)n,
+                                                    (int)n_seg, sb, se, stream_));
+  big_seq_kernel<<<n_seg, ST, 0, stream_>>>(sb, se, g.a_seq, s_idx_out_.as<unsigned int>(), s_seq_.as<unsigned int>());
+  AB_CUDA(cudaGetLastError());
+  t2 = s_tmp_.bytes;
+  AB_CUDA(cub::DeviceSegmentedSort::StableSortPairs(s_tmp_.p, t2, s_seq_.as<unsigned int>(), s_seq_out_.as<unsigned int>(),
+                                                    s_idx_out_.as<unsigned int>(), s_idx_.as<unsigned int>(), (int)n,
+                                                    (int)n_seg, sb, se, stream_));
+  big_gather_kernel<<<n_seg, ST, 0, stream_>>>(sb, se, g, s_idx_.as<unsigned int>());
+  AB_CUDA(cudaGetLastError());
+  st_.kernel_launches += 5;
 }
 
 void SessionOp::flush() {
@@ -1165,10 +1300,18 @@ void SessionOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int
   if (start_time != INT64_MIN) {
     has_wm_ = true;
     wm_ = start_time;
+    // the replayed rows were counted by the operator that accepted them: rows_in and rows_late count only what the
+    // caller hands in, so the counters are put back after the replay (rows before start_time count as late there)
+    const uint64_t rows_in = st_.rows_in;
+    unsigned long long late = 0;
+    AB_CUDA(cudaMemcpyAsync(&late, late_.p, 8, cudaMemcpyDeviceToHost, stream_));
     for (int64_t i = 0; i < n; ++i) {
       process_batch(0, 1, &state[i], &schemas[i]);
       apply_pending();  // every stored batch is its own input batch
     }
+    st_.rows_in = rows_in;
+    AB_CUDA(cudaMemcpyAsync(late_.p, &late, 8, cudaMemcpyHostToDevice, stream_));
+    AB_CUDA(cudaStreamSynchronize(stream_));
   } else {
     AB_REQUIRE(n == 0, ARROYO_B200_INVALID_ARGUMENT, "session restore: state batches without a start time (table 'e')");
   }

@@ -421,9 +421,21 @@ class SessionAggregatingWindowFunc(_NativeOperator):
             C.CFUNCTYPE(None, C.c_void_p)(sch.release)(C.addressof(sch))
         _check(self._lib, self._h, st)
 
+    def _set_watermark(self, ctx: OperatorContext):
+        """A new operator takes the last watermark before its first batch (on_start with nothing to restore): the
+        library only learns watermarks from handle_watermark and on_start, and without one it would treat every row as
+        on time."""
+        wm = ctx.last_present_watermark()
+        if wm is None or not self.created:
+            return
+        arrs, schs = (ffi.ArrowArray * 1)(), (ffi.ArrowSchema * 1)()
+        _check(self._lib, self._h, self._lib.arroyo_b200_op_on_start(self._h, arrs, schs, 0, clamp_watermark(wm),
+                                                                     ffi.INT64_MIN))
+
     def process_batch(self, batch: pa.RecordBatch, ctx: OperatorContext, collector: Collector):
         if not self.created:
             self._build(batch.schema.names)
+            self._set_watermark(ctx)
         # Table "s" holds the raw input rows that passed the late filter, keyed by the batch's newest timestamp
         # (session_aggregating_window.rs:858-883).  The shim owns the table: it keeps the on-time rows of the batch it
         # is about to hand over (the reference also sorts them; restore re-sorts, :829, so the order is not state).
@@ -465,6 +477,7 @@ class SessionAggregatingWindowFunc(_NativeOperator):
         """session_aggregating_window.rs:802-847."""
         starts = [v for v in ctx.global_table("e").values() if v is not None]
         if not starts:
+            self._set_watermark(ctx)
             return
         start_time = min(starts)
         table = ctx.table("s", int(self.config.gap) * 100)

@@ -9,6 +9,7 @@ Otherwise |got - mean| <= 2u * sum|x| + 2u * |mean| with u = 2^-53: that is n * 
 bound of an f64 sum of n terms in any order including the rounding of each input, divided by n, plus the final
 division."""
 import bisect
+import heapq
 import itertools
 from fractions import Fraction
 
@@ -554,4 +555,261 @@ def expiring_join(events, left_on, right_on, left_routing=(), right_routing=()):
         cat = lambda p: np.concatenate(p) if p else np.zeros(0, np.int64)  # noqa: E731
         pn, po = cat(pn), cat(po)
         out.append(_output(sides, pn, po) if s == 0 else _output(sides, po, pn))
+    return out
+
+
+# ---- session windows --------------------------------------------------------------------------------------------
+class _SessionAcc:
+    """Exact running aggregates of one session: rows, and per value column (exact sum, sum of |x|, min, max)."""
+    __slots__ = ("rows", "cols")
+
+    def __init__(self, names):
+        self.rows = 0
+        self.cols = {c: [0, 0, None, None] for c in names}
+
+    def add(self, cols, lo, hi):
+        if hi <= lo:
+            return
+        self.rows += hi - lo
+        for c, st in self.cols.items():
+            v = cols[c][lo:hi]
+            if len(v) <= 64:
+                xs = v.tolist()
+                s, a = sum(xs), sum(abs(x) for x in xs)
+            else:
+                sg, ab = _exact_sums(v, np.zeros(len(v), dtype=np.int64), 1)
+                s, a = sg[0], ab[0]
+            st[0] += s
+            st[1] += a
+            mn, mx = int(v.min()), int(v.max())
+            st[2] = mn if st[2] is None else min(st[2], mn)
+            st[3] = mx if st[3] is None else max(st[3], mx)
+
+    def row(self, aggs):
+        out = {}
+        for a in aggs:
+            if a.kind == "count":
+                out[a.name] = self.rows
+                continue
+            s, ab, mn, mx = self.cols[a.col]
+            out[a.name] = {"sum": lambda: _wrap(s), "min": lambda: mn, "max": lambda: mx,
+                           "avg": lambda: Mean(Fraction(s, self.rows), ab)}[a.kind]()
+        return out
+
+
+class _SessionKey:
+    """One key's state: the active session [ds, de, acc] or None, and the pending runs, a heap of (first ts, insertion
+    number, ts, cols)."""
+    __slots__ = ("active", "pending")
+
+    def __init__(self):
+        self.active, self.pending = None, []
+
+
+def session_emissions(events, key_name, aggs, gap):
+    """The session window aggregate's output, from these rules (session_aggregating_window.rs:60-279, :397-691,
+    :802-925):
+
+    Late rows and runs.  Once a watermark w has been seen, a row with ts < w is late; before the first watermark
+    nothing is late.  A batch's on-time rows of one key, sorted by ts, form one run.  Each key keeps an optional
+    active session (ds, de, rows taken) and pending runs ordered by (first ts, insertion order).
+
+    add(run) under the last watermark w: insert the run; with no watermark yet, stop; if a session is active, fill;
+    then advance(w), which must close nothing (the reference bails if it does).
+
+    fill: while the smallest pending start is <= de + gap, pop every run with that start, in insertion order, and
+    absorb each one; re-insert any remainder.
+
+    absorb(t[0..n)): (1) if t[n-1] < de + gap, take all rows, de = max(de, t[n-1]), ds = min(ds, t[0]).  (2) Else if
+    de + gap < t[0], the whole run is the remainder.  (3) Else ds = min(ds, t[0]) (t[0] < ds - gap is an error), and
+    scan from i = 1: v = t[i], i += 1; if v < de continue; if v < de + gap, de = v and continue; otherwise break.  If
+    i == n take all rows, else take t[0..i) and the remainder is t[i..n).  On this path the row that breaks the scan is
+    taken without extending de, and the first row never extends de.
+
+    advance(w): loop: an active session with de + gap < w closes (window_start = ds, window_end = de + gap,
+    _timestamp = de + gap - 1) and the loop goes on; an active session otherwise stops it.  With no active session,
+    stop if nothing is pending or w + gap < the smallest start; otherwise open a session with ds = de = that start
+    and fill.
+
+    Watermark w: advance only the keys whose next action is < w: de + gap for an active session, else the smallest
+    pending start - gap.  So a pending start of exactly w + gap is not opened by the watermark, but by an add under
+    the same w.  End of data is w = INT64_MAX.
+
+    Restart.  Each batch's on-time rows are kept in table "s" under the batch's largest ts.  A checkpoint under
+    watermark w drops the entries whose largest ts is below w - 100 gap.  On restore, start = the smallest on-time ts
+    the operator accepted (table "e"; nothing is restored without one); the entries whose largest ts is
+    >= start - 100 gap are replayed in ascending largest ts (ties in insertion order), each filtered to ts >= start
+    and added as its own batch under watermark start; then the operator advances to the restored watermark and drops
+    what that closes.  Unlike the window operators, a restart can change the results.
+
+    Rows with equal ts inside one run are taken in an unspecified order: streams whose equal-ts rows carry different
+    values on both sides of a break have no single answer.
+
+    `events`: ("batch", cols), ("wm", w) or ("restart",); watermarks must not decrease.  Returns (one
+    {(key or None, window_start): row} per watermark, the number of late rows, the number of distinct keys the last
+    operator lifetime accepted rows for)."""
+    names = sorted({a.col for a in aggs if a.kind != "count"})
+    keys, table, out = {}, [], []
+    st = {"w": None, "late": 0, "min": None, "n": 0, "keys": set()}
+
+    def absorb(k, t, cols):
+        a = k.active
+        ds, de, acc = a
+        n = len(t)
+        if t[n - 1] < de + gap:
+            a[0], a[1] = min(ds, int(t[0])), max(de, int(t[n - 1]))
+            acc.add(cols, 0, n)
+            return None
+        if de + gap < t[0]:
+            return 0
+        if t[0] < ds - gap:
+            raise ValueError("a run starts before data_start - gap")
+        a[0] = min(ds, int(t[0]))
+        i = 1
+        while i < n:
+            v = int(t[i])
+            i += 1
+            if v < de:
+                continue
+            if v < de + gap:
+                de = v
+                continue
+            break
+        a[1] = de
+        acc.add(cols, 0, i)
+        return None if i == n else i
+
+    def push(k, t, cols):
+        heapq.heappush(k.pending, (int(t[0]), st["n"], t, cols))
+        st["n"] += 1
+
+    def fill(k):
+        while k.pending and k.pending[0][0] <= k.active[1] + gap:
+            first, batch = k.pending[0][0], []
+            while k.pending and k.pending[0][0] == first:
+                batch.append(heapq.heappop(k.pending))
+            for _, _, t, cols in batch:
+                i = absorb(k, t, cols)
+                if i is not None:
+                    push(k, t[i:], {c: v[i:] for c, v in cols.items()})
+
+    def advance(key, k, w, emit):
+        while True:
+            if k.active is not None:
+                ds, de, acc = k.active
+                if not de + gap < w:
+                    return
+                if emit is None:
+                    raise ValueError("a session closed while adding a run")
+                row = {"window_start": ds, "window_end": de + gap, TIMESTAMP: de + gap - 1, **acc.row(aggs)}
+                if key_name:
+                    row[key_name] = key
+                assert (key, ds) not in emit
+                emit[(key, ds)] = row
+                k.active = None
+                continue
+            if not k.pending or w + gap < k.pending[0][0]:
+                return
+            s0 = k.pending[0][0]
+            k.active = [s0, s0, _SessionAcc(names)]
+            fill(k)
+
+    def add_batch(cols, w):
+        ts = np.asarray(cols[TIMESTAMP]).astype(np.int64)
+        if not len(ts):
+            return
+        key = np.asarray(cols[key_name]) if key_name else np.zeros(len(ts), dtype=np.int64)
+        kl = key.tolist()
+        order = np.lexsort((ts, key.view(np.int64) if key.dtype == np.uint64 else key.astype(np.int64)))
+        vals = {c: np.asarray(cols[c]).astype(np.int64)[order] for c in names}
+        ts, kl = ts[order], [kl[i] for i in order.tolist()]
+        m = int(ts.min())
+        st["min"] = m if st["min"] is None else min(st["min"], m)
+        lo = 0
+        while lo < len(ts):
+            hi = lo + 1
+            while hi < len(ts) and kl[hi] == kl[lo]:
+                hi += 1
+            kv = kl[lo] if key_name else None
+            st["keys"].add(kv)
+            k = keys.setdefault(kv, _SessionKey())
+            push(k, ts[lo:hi], {c: v[lo:hi] for c, v in vals.items()})
+            if w is not None:
+                if k.active is not None:
+                    fill(k)
+                advance(kv, k, w, None)
+            lo = hi
+
+    def next_action(k):
+        if k.active is not None:
+            return k.active[1] + gap
+        return k.pending[0][0] - gap if k.pending else None
+
+    def watermark(w, emit):
+        for kv, k in keys.items():
+            na = next_action(k)
+            if na is not None and na < w:
+                advance(kv, k, w, emit)
+
+    for ev in events:
+        if ev[0] == "batch":
+            cols = {c: np.asarray(v) for c, v in _columns(ev[1]).items()}
+            ts = cols[TIMESTAMP].astype(np.int64)
+            keep = np.ones(len(ts), dtype=bool) if st["w"] is None else ts >= st["w"]
+            st["late"] += int((~keep).sum())
+            if not keep.any():
+                continue
+            cols = {c: v[keep] for c, v in cols.items()}
+            table.append((int(cols[TIMESTAMP].astype(np.int64).max()), len(table), cols))
+            add_batch(cols, st["w"])
+        elif ev[0] == "wm":
+            w = min(int(ev[1]), INT64_MAX)
+            if st["w"] is not None and w < st["w"]:
+                raise ValueError("watermarks must not decrease")
+            st["w"] = w
+            emit = {}
+            watermark(w, emit)
+            out.append(emit)
+        else:
+            assert ev[0] == "restart", ev
+            w, start = st["w"], st["min"]
+            if w is not None:
+                table = [e for e in table if e[0] >= w - 100 * gap]
+            keys.clear()
+            st["keys"], st["min"] = set(), None
+            if start is None:
+                continue
+            for _, _, cols in sorted((e for e in table if e[0] >= start - 100 * gap), key=lambda e: (e[0], e[1])):
+                keep = cols[TIMESTAMP].astype(np.int64) >= start
+                if keep.any():
+                    add_batch({c: v[keep] for c, v in cols.items()}, start)
+            if w is not None:
+                watermark(w, {})
+    return out, st["late"], len(st["keys"])
+
+
+def session_chains(events, key_name, gap):
+    """The declarative form of a session, for streams without restarts, with at most one row per key per batch and
+    no two rows of a key exactly `gap` apart: every session is a maximal chain of a key's on-time rows whose
+    consecutive distances are < gap.  Returns {(key or None, first ts): (last ts + gap, rows)}."""
+    w, per_key = None, {}
+    for ev in events:
+        if ev[0] == "wm":
+            w = min(int(ev[1]), INT64_MAX)
+            continue
+        assert ev[0] == "batch", ev
+        cols = _columns(ev[1])
+        ts = np.asarray(cols[TIMESTAMP]).astype(np.int64).tolist()
+        ks = np.asarray(cols[key_name]).tolist() if key_name else [None] * len(ts)
+        for k, t in zip(ks, ts):
+            if w is None or t >= w:
+                per_key.setdefault(k, []).append(t)
+    out = {}
+    for k, ts in per_key.items():
+        ts.sort()
+        first = 0
+        for i in range(1, len(ts) + 1):
+            if i == len(ts) or ts[i] - ts[i - 1] >= gap:
+                out[(k, ts[first])] = (ts[i - 1] + gap, i - first)
+                first = i
     return out

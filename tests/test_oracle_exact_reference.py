@@ -208,3 +208,97 @@ def test_exact_reference_joins_by_hand():
     assert not X.join_mismatches(a, b)
     b.vals[0, 1] ^= np.uint64(1)
     assert X.join_mismatches(a, b)
+
+
+# ---- session windows: the numpy and C session oracles against exact_reference.session_emissions ----------------------
+def _session_shapes():
+    from tests import test_gpu_session_time as T
+    # UInt64 keys are left out: the numpy oracle builds its output key column from Python ints and turns keys >= 2^63
+    # into Float64 (the C oracle takes Int64 keys only)
+    return [(s, k, g, p) for s, k, g, p, _ in T.CASES if k != "u64"]
+
+
+@pytest.mark.parametrize("impl", ["numpy", "c"])
+def test_session_oracle_matches_exact_reference(impl):
+    from tests import test_gpu_session_time as T
+    ran = 0
+    for shape, keys, gap, plan in _session_shapes():
+        st = T.make(shape, keys, gap)
+        cfg = T.config(st, plan)
+        # session_oracle.c: one value column, no checkpoint / restore
+        if impl == "c" and (len({a.col for a in cfg.aggs if a.col}) > 1 or any(ev[0] == "restart" for ev in st.events)):
+            continue
+        want, _, _ = T.reference(st, cfg)
+        T.check_emissions(want, T.run_oracle(st, cfg, impl), cfg, f"{impl} {shape}/{keys}/{gap}/{plan}")
+        ran += 1
+    assert ran >= (20 if impl == "numpy" else 10)
+
+
+def _chain_stream(seed, keys, gap, n_batches=60):
+    """At most one row per key per batch, no two rows of a key exactly `gap` apart, watermarks behind the data."""
+    from tests import test_gpu_session_time as T
+    st = T.Stream(seed, keys, gap)
+    rng, o, used = st.rng, T.ORIGIN, {}
+    ks = [None] if keys == "none" else st.keyset()
+    st.wm(o - 10 * gap)
+    for b in range(n_batches):
+        tss, kk = [], []
+        for k in ks:
+            if rng.random() < 0.3:
+                continue
+            while True:
+                t = o + int(rng.integers(0, 40 * gap)) + (b * gap) // 2
+                if all(abs(t - u) != gap for u in used.get(k, ())):
+                    break
+            used.setdefault(k, []).append(t)
+            tss.append(t)
+            kk.append(k)
+        if tss:
+            st.batch(tss, None if keys == "none" else np.asarray(kk, dtype=object))
+        if b % 7 == 6:
+            st.wm(o + (b - 14) * gap // 2)
+    return st.end()
+
+
+@pytest.mark.parametrize("keys", ["few", "none", "edge"])
+@pytest.mark.parametrize("gap", [1, 999, 5 * S])
+def test_session_emissions_match_chains(keys, gap):
+    """In the restricted class of streams, every emitted session is a maximal chain of the key's on-time rows whose
+    consecutive distances are < gap: the rule statement of session_emissions against the declarative definition."""
+    from tests import test_gpu_session_time as T
+    st = _chain_stream(abs(hash((keys, gap))) % 1000, keys, gap)
+    cfg = T.config(st, "count")
+    out, _, _ = T.reference(st, cfg)
+    got = {}
+    for emitted in out:
+        for (k, s), r in emitted.items():
+            assert (k, s) not in got
+            got[(k, s)] = (r["window_end"], r["n"])
+    want = X.session_chains(st.events, cfg.key_names[0] if cfg.key_names else None, gap)
+    assert got == want
+
+
+def test_session_emissions_by_hand():
+    """The session rules on streams small enough to follow by hand (gap 10)."""
+    aggs = [A("count", None, "n"), A("sum", "a", "s")]
+
+    def b(ts, a):
+        return {"a": np.array(a, dtype=np.int64), X.TIMESTAMP: np.array(ts, dtype=np.int64)}
+
+    # one run [0, 5, 25, 26] under a watermark: 25 breaks the scan and is taken without extending data_end
+    out, late, n_keys = X.session_emissions([("wm", -100), ("batch", b([0, 5, 25, 26], [1, 2, 3, 4])),
+                                             ("wm", 15), ("wm", 16), ("wm", X.INT64_MAX)], None, aggs, 10)
+    assert late == 0 and n_keys == 1
+    assert out[0] == {} and out[1] == {} and list(out[2]) == [(None, 0)]  # w = 15 = data_end + gap does not close
+    assert out[2][(None, 0)]["n"] == 3 and out[2][(None, 0)]["window_end"] == 15 and out[2][(None, 0)]["s"] == 6
+    assert list(out[3]) == [(None, 26)] and out[3][(None, 26)]["n"] == 1
+    # inside one run, a row exactly gap after the first breaks the scan and is still taken; ts < w is late, ts = w not
+    out, late, _ = X.session_emissions([("batch", b([0, 10], [1, 2])), ("wm", 10), ("wm", 11), ("batch", b([11, 9], [5, 6])),
+                                        ("wm", 21), ("wm", 22)], None, aggs, 10)
+    assert late == 1
+    assert out[0] == {} and list(out[1]) == [(None, 0)] and out[1][(None, 0)]["n"] == 2
+    assert out[1][(None, 0)]["window_end"] == 10 and out[2] == {} and out[3][(None, 11)]["s"] == 5
+    # a restart after the session at 0 closed: table "s" replays from start = 0, the restored watermark drops it again
+    out, _, _ = X.session_emissions([("batch", b([0], [1])), ("wm", 11), ("batch", b([30], [2])), ("restart",),
+                                     ("wm", X.INT64_MAX)], None, aggs, 10)
+    assert list(out[0]) == [(None, 0)] and list(out[1]) == [(None, 30)]
