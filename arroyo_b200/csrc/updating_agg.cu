@@ -9,7 +9,9 @@
 // Here (append-only inputs: no `_updating_meta.is_retract` upstream; COUNT(*) / SUM / AVG / MIN / MAX over Int64):
 //   ingest  one thread per row: dense id from the bucketed key dictionary (bdict.cuh), one RED per accumulator, the
 //           trailing max(_timestamp) aggregate as a RED.max, and the key joins the touched list on its first row
-//           since the last flush (atomicExch on a per-id flag);
+//           since the last flush (atomicExch on a per-id flag).  A row whose bucket is out of ids is copied to a
+//           deferral buffer; at the next host sync point the host doubles the bucket count and re-ingests it
+//           (drain_deferred);
 //   flush   one thread per touched key: compares the accumulators with their values at the previous flush (kept per
 //           id: "the values it had before"), writes the retraction row (old values, old timestamp) and the append row
 //           (new values), and rolls the snapshot forward.
@@ -52,10 +54,22 @@ struct UIngest {
   const long long* val[4];
   long long n;
   int keyed;
+  int n_vals;
   BDict dict;
   UState st;
-  unsigned long long* lost;
+  // deferred rows: [key, ts, values...] columns with room for every row of the launch, and their count
+  long long* d_key;
+  long long* d_ts;
+  long long* d_val[4];
+  unsigned long long* deferred;
 };
+
+__device__ __noinline__ void upd_defer_row(const UIngest& p, long long i, long long key) {
+  const unsigned long long d = atomicAdd(p.deferred, 1ull);
+  p.d_key[d] = key;
+  p.d_ts[d] = p.ts[i];
+  for (int v = 0; v < p.n_vals; ++v) p.d_val[v][d] = p.val[v][i];
+}
 
 __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__ UIngest p) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -63,9 +77,10 @@ __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__
   for (; i < p.n; i += stride) {
     uint32_t id = 0;
     if (p.keyed) {
-      id = bd_lookup_or_insert(p.dict, __ldcs(p.key + i));
-      if (id >= ID_OVERFLOW) {
-        atomicAdd(p.lost, 1ull);
+      const long long key = __ldcs(p.key + i);
+      id = bd_lookup_or_insert(p.dict, key);
+      if (id >= ID_OVERFLOW) {  // the key's bucket is out of ids
+        upd_defer_row(p, i, key);
         continue;
       }
     }
@@ -203,12 +218,16 @@ class UpdatingAggOp final : public OpBase {
     AB_CUDA(cudaStreamSynchronize(stream_));
   }
   void stats(ArroyoB200Stats* out) override {
+    st_.n_keys = 0;
     if (keyed_) {
       AB_CUDA(cudaSetDevice(device_));
-      AB_CUDA(cudaMemcpyAsync(&total_keys_, n_total_.p, 4, cudaMemcpyDeviceToHost, stream_));
+      drain_deferred();  // also reads the dictionary's count (ids from BD_ID_BASE on)
+      // id 0 is the INT64_MIN key's: it has rows once that key arrived
+      unsigned long long min_key_rows = 0;
+      AB_CUDA(cudaMemcpyAsync(&min_key_rows, cur_.p, 8, cudaMemcpyDeviceToHost, stream_));
       AB_CUDA(cudaStreamSynchronize(stream_));
+      st_.n_keys = (uint64_t)total_keys_ + (min_key_rows ? 1 : 0);
     }
-    st_.n_keys = keyed_ ? total_keys_ : 0;
     *out = st_;
   }
 
@@ -228,9 +247,13 @@ class UpdatingAggOp final : public OpBase {
   uint64_t n_buckets_ = 1, id_cap_ = 0;
   uint32_t total_keys_ = 0;
   DevBuf slots_, bucket_nkeys_, id_keys_, n_total_;
-  DevBuf cur_, prev_, cur_ts_, prev_ts_, touched_, list_, counters_;  // counters_: [n_touched, retractions, appends, pad] u32 + lost u64
+  DevBuf cur_, prev_, cur_ts_, prev_ts_, touched_, list_, counters_;  // counters_: [n_touched, retractions, appends, pad] u32 + deferred u64
   DevBuf staging_;
   uint64_t staging_cap_ = 0;
+  // deferred rows (key, ts, values): two sets, one re-ingested while the other takes the rows that defer again
+  DevBuf defer_[2][2 + 4];
+  uint64_t defer_cap_[2] = {0, 0};
+  int defer_cur_ = 0;
   uint64_t out_cap_ = 0;
   DevBuf o_key_, o_ts_, o_agg_[ARROYO_B200_MAX_AGGS];
   ArroyoB200Stats st_{};
@@ -239,6 +262,8 @@ class UpdatingAggOp final : public OpBase {
   UState state_view() const;
   void alloc_state(uint64_t n_buckets);
   void grow();
+  void reserve_defer(int set, uint64_t rows);
+  void drain_deferred();
   void ensure_room(uint64_t new_rows);
   void ingest(const long long* key, const long long* ts, const long long* const* vals, int64_t n);
   void flush_to(BatchesPriv* out);
@@ -381,7 +406,10 @@ void UpdatingAggOp::alloc_state(uint64_t n_buckets) {
 }
 
 // Doubles the bucket count: keys are re-inserted (ids change), the per-id state and the touched list follow the map.
+// A bucket's keys split between the two buckets that replace it, so the rehash itself never runs out of ids.
 void UpdatingAggOp::grow() {
+  // refused before anything moves: the operator stays usable
+  AB_REQUIRE(bd_id_cap(n_buckets_ * 2) < (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
   const BDict old_d = dict_view();
   const UState old_s = state_view();
   const uint32_t old_ids = (uint32_t)(BD_ID_BASE + n_buckets_ * BD_CAPB);
@@ -410,11 +438,52 @@ void UpdatingAggOp::grow() {
   st_.kernel_launches += 3;
 }
 
+void UpdatingAggOp::reserve_defer(int set, uint64_t rows) {
+  if (rows <= defer_cap_[set]) return;
+  defer_cap_[set] = std::max<uint64_t>(rows, defer_cap_[set] * 2);
+  for (int c = 0; c < 2 + n_vals_; ++c) defer_[set][c].alloc(defer_cap_[set] * 8);
+}
+
+// Re-ingests the rows the last launch deferred (their bucket was out of ids), doubling the bucket count before each
+// pass.  Keys that share a bucket at several sizes need several passes; after DRAIN_STALLS passes in a row that placed
+// none of the rows it gives up: RUNTIME, the rows are dropped and the operator stays usable.  Also reads the
+// dictionary's key count into total_keys_.
+void UpdatingAggOp::drain_deferred() {
+  constexpr int DRAIN_STALLS = 4;
+  unsigned long long* d_count = reinterpret_cast<unsigned long long*>((char*)counters_.p + 16);
+  auto read = [&]() {
+    unsigned long long n = 0;
+    AB_CUDA(cudaMemcpyAsync(&n, d_count, 8, cudaMemcpyDeviceToHost, stream_));
+    AB_CUDA(cudaMemcpyAsync(&total_keys_, n_total_.p, 4, cudaMemcpyDeviceToHost, stream_));
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    return (uint64_t)n;
+  };
+  uint64_t n = read(), prev = UINT64_MAX;
+  try {
+    for (int stalls = 0; n > 0; prev = n, n = read()) {
+      stalls = n < prev ? 0 : stalls + 1;
+      AB_REQUIRE(stalls < DRAIN_STALLS, ARROYO_B200_RUNTIME,
+                 "updating aggregate: rows whose dictionary bucket is out of ids still defer after the dictionary grew");
+      st_.rows_deferred += n;
+      grow();
+      const int full = defer_cur_;
+      defer_cur_ ^= 1;
+      AB_CUDA(cudaMemsetAsync(d_count, 0, 8, stream_));
+      const long long* vals[4] = {nullptr, nullptr, nullptr, nullptr};
+      for (int v = 0; v < n_vals_; ++v) vals[v] = defer_[full][2 + v].as<long long>();
+      ingest(defer_[full][0].as<long long>(), defer_[full][1].as<long long>(), vals, (int64_t)n);
+    }
+  } catch (...) {
+    cudaMemsetAsync(d_count, 0, 8, stream_);  // a failed drain must not fail every later call
+    cudaStreamSynchronize(stream_);
+    throw;
+  }
+}
+
 // every row of the batch may bring a new key: keep the mean bucket fill at or under the target
 void UpdatingAggOp::ensure_room(uint64_t new_rows) {
   if (!keyed_) return;
-  AB_CUDA(cudaMemcpyAsync(&total_keys_, n_total_.p, 4, cudaMemcpyDeviceToHost, stream_));
-  AB_CUDA(cudaStreamSynchronize(stream_));
+  drain_deferred();
   while ((uint64_t)total_keys_ + new_rows > n_buckets_ * (uint64_t)BD_MEAN) grow();
 }
 
@@ -426,9 +495,16 @@ void UpdatingAggOp::ingest(const long long* key, const long long* ts, const long
   for (int v = 0; v < n_vals_; ++v) p.val[v] = vals[v];
   p.n = n;
   p.keyed = keyed_ ? 1 : 0;
+  p.n_vals = n_vals_;
   p.dict = dict_view();
   p.st = state_view();
-  p.lost = reinterpret_cast<unsigned long long*>((char*)counters_.p + 16);
+  if (keyed_) {  // every row of the launch may defer (all rows of a key whose bucket is full do)
+    reserve_defer(defer_cur_, (uint64_t)n);
+    p.d_key = defer_[defer_cur_][0].as<long long>();
+    p.d_ts = defer_[defer_cur_][1].as<long long>();
+    for (int v = 0; v < n_vals_; ++v) p.d_val[v] = defer_[defer_cur_][2 + v].as<long long>();
+  }
+  p.deferred = reinterpret_cast<unsigned long long*>((char*)counters_.p + 16);
   const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms_ * 8);
   upd_ingest_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(p);
   AB_CUDA(cudaGetLastError());
@@ -492,13 +568,12 @@ static void* d2h_part(const void* dev, size_t off_rows, int64_t n, void* host, s
 // flush (:637-738): one batch [key?, aggregates..., _timestamp, is_retract], or nothing when no key changed
 void UpdatingAggOp::flush_to(BatchesPriv* out) {
   AB_CUDA(cudaSetDevice(device_));
+  if (keyed_) drain_deferred();
   struct {
     unsigned int touched, retracts, appends, pad;
-    unsigned long long lost;
   } h{};
-  AB_CUDA(cudaMemcpyAsync(&h, counters_.p, 24, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaMemcpyAsync(&h, counters_.p, 16, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
-  AB_REQUIRE(h.lost == 0, ARROYO_B200_RUNTIME, "updating aggregate: a dictionary bucket ran out of ids");
   const unsigned int n = h.touched;
   if (n == 0 || !out) return;
   if (2ull * n > out_cap_) {
@@ -526,7 +601,7 @@ void UpdatingAggOp::flush_to(BatchesPriv* out) {
   AB_CUDA(cudaGetLastError());
   ++st_.kernel_launches;
   ++st_.emit_launches;
-  AB_CUDA(cudaMemcpyAsync(&h, counters_.p, 24, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaMemcpyAsync(&h, counters_.p, 16, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaMemsetAsync(counters_.p, 0, 16, stream_));  // touched list and output counters start over
   AB_CUDA(cudaStreamSynchronize(stream_));
   const int64_t nr = h.retracts, na = h.appends, total = nr + na;

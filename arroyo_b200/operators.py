@@ -532,11 +532,17 @@ class UpdatingAggregatingFunc(_NativeOperator):
         super().__init__(**kw)
         self.config = config
         self.updating_input = updating_input
+        self._key_type = None
         if input_schema is not None:
             self._build(input_schema.names)
+            self._note_key_type(input_schema)
 
     def name(self):
         return "UpdatingAggregatingFunc"
+
+    def _note_key_type(self, schema: pa.Schema):
+        if self.config.key_names:
+            self._key_type = schema.field(self.config.key_names[0]).type
 
     def tables(self):
         return {"a": 0, "b": 0}  # accumulator state / batch state (:963-988): restore is not implemented
@@ -567,6 +573,7 @@ class UpdatingAggregatingFunc(_NativeOperator):
     def process_batch(self, batch: pa.RecordBatch, ctx: OperatorContext, collector: Collector):
         if not self.created:
             self._build(batch.schema.names)
+        self._note_key_type(batch.schema)
         arr, sch = export_batch(batch)
         st = self._lib.arroyo_b200_op_process_batch(self._h, 0, 1, C.byref(arr), C.byref(sch))
         if st != ffi.OK and arr.release:
@@ -575,13 +582,28 @@ class UpdatingAggregatingFunc(_NativeOperator):
             C.CFUNCTYPE(None, C.c_void_p)(sch.release)(C.addressof(sch))
         _check(self._lib, self._h, st)
 
+    def process_device_batch(self, cols: List[int], n_rows: int):
+        """`cols` = device pointers (ints), one per input column; needs `input_schema` at construction."""
+        arr = (C.c_uint64 * len(cols))(*cols)
+        _check(self._lib, self._h, self._lib.arroyo_b200_op_process_device_batch(self._h, 0, 1, arr, len(cols), n_rows))
+
+    def process_device_batches(self, cols_flat, n_rows, n_cols: int):
+        """A run of device batches in one FFI call; `cols_flat`/`n_rows` are prebuilt ctypes arrays
+        ((c_uint64 * (n_batches * n_cols)), (c_int64 * n_batches))."""
+        st = self._lib.arroyo_b200_op_process_device_batches(self._h, 0, 1, cols_flat, n_cols, n_rows, len(n_rows))
+        _check(self._lib, self._h, st)
+
     def handle_watermark(self, watermark, ctx: OperatorContext, collector: Collector):
         return watermark
 
     def _emit(self, out, collector: Collector):
         names = self.output_names()
         for b in import_batches(self._lib, out):
-            collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+            cols = b.columns
+            # device batches carry no Arrow types: the key column leaves with the input schema's key type
+            if self._key_type is not None and cols[0].type != self._key_type:
+                cols = [cols[0].view(self._key_type)] + cols[1:]
+            collector.collect(pa.RecordBatch.from_arrays(cols, names=names))
 
     def handle_tick(self, tick, ctx: OperatorContext, collector: Collector):
         if not self.created:

@@ -321,6 +321,120 @@ def updating_rows(batches, key_name, aggs):
     return out
 
 
+def _batch_partials(cols, key_name, aggs):
+    """{key or None: [rows, state per aggregate, max ts]} of one batch's rows.  A state is the exact sum (SUM), the
+    value (MIN / MAX) or [exact sum, sum of |x|] (AVG); COUNT uses `rows`."""
+    ts = np.asarray(cols[TIMESTAMP]).astype(np.int64)
+    n = len(ts)
+    if n == 0:
+        return {}
+    key = np.asarray(cols[key_name]) if key_name else np.zeros(n, dtype=np.int64)
+    uniq, inv, n_groups = _group_keys(key)
+    count = np.bincount(inv, minlength=n_groups)
+    tmax = np.full(n_groups, np.iinfo(np.int64).min, dtype=np.int64)
+    np.maximum.at(tmax, inv, ts)
+    per_agg = []
+    for a in aggs:
+        if a.kind == "count":
+            per_agg.append(None)
+            continue
+        v = np.ascontiguousarray(cols[a.col]).astype(np.int64, copy=False)
+        if a.kind in ("sum", "avg"):
+            signed, abs_sum = _exact_sums(v, inv, n_groups)
+            per_agg.append(signed if a.kind == "sum" else list(zip(signed, abs_sum)))
+        else:
+            ii = np.iinfo(np.int64)
+            s = np.full(n_groups, ii.max if a.kind == "min" else ii.min, dtype=np.int64)
+            (np.minimum if a.kind == "min" else np.maximum).at(s, inv, v)
+            per_agg.append(s.tolist())
+    keys = [None] * n_groups
+    if key_name:
+        keys = uniq[0].view(np.uint64).tolist() if key.dtype == np.uint64 else uniq[0].tolist()
+    out = {}
+    counts, tmaxs = count.tolist(), tmax.tolist()
+    for g in range(n_groups):
+        st = [counts[g]]
+        for a, vals in zip(aggs, per_agg):
+            st.append(None if vals is None else (list(vals[g]) if a.kind == "avg" else vals[g]))
+        st.append(tmaxs[g])
+        out[keys[g]] = st
+    return out
+
+
+def _merge_state(old, new, aggs):
+    if old is None:
+        return new
+    out = [old[0] + new[0]]
+    for i, a in enumerate(aggs, 1):
+        x, y = old[i], new[i]
+        out.append(None if a.kind == "count" else min(x, y) if a.kind == "min" else max(x, y) if a.kind == "max"
+                   else [x[0] + y[0], x[1] + y[1]] if a.kind == "avg" else x + y)
+    out.append(max(old[-1], new[-1]))
+    return out
+
+
+def _state_row(st, key, key_name, aggs):
+    row = {TIMESTAMP: st[-1]}
+    if key_name:
+        row[key_name] = key
+    for i, a in enumerate(aggs, 1):
+        if a.kind == "count":
+            row[a.name] = st[0]
+        elif a.kind == "sum":
+            row[a.name] = _wrap(st[i])
+        elif a.kind == "avg":
+            row[a.name] = Mean(Fraction(st[i][0], st[0]), st[i][1])
+        else:
+            row[a.name] = st[i]
+    return row
+
+
+def updating_changes(events, key_name, aggs):
+    """The updating (non-windowed GROUP BY) aggregate's change stream, flush by flush, from these rules
+    (incremental_aggregator.rs:637-738, :826-883), over append-only rows:
+
+    * state_f(k) is the aggregates of every row of key k received before flush f, and `_timestamp` = the max of those
+      rows' timestamps.  COUNT is exact, SUM wraps at 64 bits, MIN and MAX are exact, AVG is a Mean;
+    * k is touched at flush f if at least one of its rows arrived since flush f - 1 (the start, for the first flush);
+    * only touched keys appear in flush f.  A key that had no rows at flush f - 1 gets an append of state_f only.
+      Otherwise, if any output other than `_timestamp` differs between state_{f-1} and state_f, it gets a retraction
+      of state_{f-1} (its `_timestamp` included) and an append of state_f; else it is suppressed;
+    * AVG counts as changed when the correctly rounded f64 means (float of the exact mean) differ;
+    * the retraction carries state_{f-1} even when flush f - 1 suppressed the key: its `_timestamp` moved then, and
+      the reference reads its "before" values at the key's first touch after flush f - 1.
+
+    With a key whose sum of |x| reaches 2^53, put COUNT in the plan: the operators sum AVG inputs in f64, in an order
+    the caller does not control, so suppression must not depend on an AVG alone.
+
+    `events`: ("batch", cols) and ("flush",).  Returns one (retractions, appends) per flush, each {key or None: row}
+    with the key column (keyed), every aggregate (AVG as a Mean) and `_timestamp`."""
+    def outputs(st):
+        return tuple(st[0] if a.kind == "count" else float(Fraction(st[i][0], st[0])) if a.kind == "avg"
+                     else _wrap(st[i]) if a.kind == "sum" else st[i] for i, a in enumerate(aggs, 1))
+
+    state, before, out = {}, {}, []
+    for ev in events:
+        if ev[0] == "batch":
+            for k, part in _batch_partials(_columns(ev[1]), key_name, aggs).items():
+                old = state.get(k)
+                if k not in before:
+                    before[k] = old  # the values at the previous flush (None: the key had no rows)
+                state[k] = _merge_state(old, part, aggs)
+            continue
+        assert ev[0] == "flush", ev
+        retract, append = {}, {}
+        for k, old in before.items():
+            new = state[k]
+            if old is not None:
+                if outputs(old) == outputs(new):
+                    continue
+                retract[k] = _state_row(old, k, key_name, aggs)
+            append[k] = _state_row(new, k, key_name, aggs)
+        out.append((retract, append))
+        before = {}
+    return out
+
+
 def mismatches(want: dict, got_rows, key_of):
     """Compares output rows (dicts) with `want` ({group: row}); `key_of(row)` gives a row's group.  Integer columns
     must be equal, AVG columns must pass `check_avg`.  Returns a list of readable differences (empty: all equal)."""

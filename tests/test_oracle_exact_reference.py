@@ -302,3 +302,90 @@ def test_session_emissions_by_hand():
     out, _, _ = X.session_emissions([("batch", b([0], [1])), ("wm", 11), ("batch", b([30], [2])), ("restart",),
                                      ("wm", X.INT64_MAX)], None, aggs, 10)
     assert list(out[0]) == [(None, 0)] and list(out[1]) == [(None, 30)]
+
+
+# ---- the updating aggregate: the oracle's change stream against exact_reference.updating_changes -------------------
+def _oracle_changes(st, aggs):
+    """The oracle on a stream of tests/test_gpu_updating_changes.py: one (retraction rows, append rows) per flush."""
+    cfg = U.UpdatingAggConfig([st.key_name()] if st.key_type else [], aggs)
+    op, out = U.IncrementalAggregatingFunc(cfg), []
+    for ev in st.events:
+        if ev[0] == "batch":
+            op.process_batch(O.Batch(ev[1]))
+            continue
+        b = op.flush()
+        rows = [] if b is None else b.rows()
+        out.append(([r for r in rows if r[U.IS_RETRACT]], [r for r in rows if not r[U.IS_RETRACT]]))
+    return out
+
+
+def _updating_cpu_shapes():
+    from tests import test_gpu_updating_changes as T
+    return [
+        ("random", "P2", lambda: T.s_random(1)), ("random_u64", "P7", lambda: T.s_random(2, "u64", every=3)),
+        ("random_ts", "P8", lambda: T.s_random(3, "ts", every=1)), ("quiet_P1", "P1", lambda: T.s_quiet(4, "P1")),
+        ("quiet_MM", "MM", lambda: T.s_quiet(5, "MM")), ("quiet_AMM", "AMM", lambda: T.s_quiet(6, "AMM")),
+        ("quiet_flush_P1", "P1", lambda: T.s_quiet(7, "P1", whole_flush=True)),
+        ("quiet_flush_AMM", "AMM", lambda: T.s_quiet(8, "AMM", "u64", whole_flush=True)),
+        ("ts_backwards", "P1", lambda: T.s_ts_backwards(9)), ("double_tick", "P4", lambda: T.s_cadence(10, "double")),
+        ("tick_first", "COUNT", lambda: T.s_cadence(11, "tick_first")),
+        ("empty_and_one", "P3", lambda: T.s_cadence(12, "empty_and_one")),
+        ("edge_keys", "P5", lambda: T.s_edge_keys(13)), ("edge_keys_u64", "P6b", lambda: T.s_edge_keys(14, "u64")),
+        ("unkeyed", "P2", lambda: T.s_unkeyed(15)), ("growth", "P1", lambda: T.s_growth(16, 3000)),
+        ("edge_values", "P3", lambda: T.s_edge_values(17)), ("crowded_spread", "P6a", lambda: T.s_crowded(18, 1400, True)),
+    ]
+
+
+@pytest.mark.parametrize("case", _updating_cpu_shapes(), ids=lambda c: c[0])
+def test_updating_oracle_change_stream_matches_exact_reference(case):
+    """Flush by flush, the oracle's retractions and appends equal updating_changes' on every column (the flag by the
+    split, _timestamp exactly, AVG by its rule)."""
+    from tests import test_gpu_updating_changes as T
+    name, plan, make = case
+    st = make()
+    aggs = T.PLANS[plan]
+    key = st.key_name()
+    want = X.updating_changes(st.events, key, aggs)
+    got = _oracle_changes(st, aggs)
+    assert len(got) == len(want)
+    n_rows = 0
+    for i, ((gr, ga), (wr, wa)) in enumerate(zip(got, want)):
+        for g, w in ((gr, wr), (ga, wa)):
+            errs = X.mismatches(w, g, lambda r: int(r[key]) if key else None)
+            assert not errs, (name, "flush", i, errs[:8])
+        n_rows += len(gr) + len(ga)
+    assert n_rows > 0
+    if name.startswith("quiet_flush"):
+        assert want[3] == ({}, {})  # a period of quiet rows only
+
+
+def test_updating_changes_by_hand():
+    """The change-stream rules on a stream small enough to follow by hand."""
+    aggs = [A("sum", "a", "s"), A("max", "a", "mx")]
+
+    def b(k, a, ts):
+        return ("batch", {"k": np.array(k, dtype=np.int64), "a": np.array(a, dtype=np.int64),
+                          X.TIMESTAMP: np.array(ts, dtype=np.int64)})
+    ev = [("flush",), b([1, 2], [5, 3], [10, 20]), ("flush",),
+          b([1, 1], [2, -2], [30, 31]),   # key 1: SUM and MAX unchanged, _timestamp 10 -> 31: suppressed
+          ("flush",), ("flush",),
+          b([1, 2], [7, 0], [5, 40]),     # key 1 changes: the retraction carries _timestamp 31; key 2 suppressed
+          ("flush",)]
+    out = X.updating_changes(ev, "k", aggs)
+    assert out[0] == ({}, {})
+    assert out[1][0] == {} and out[1][1] == {1: {"k": 1, "s": 5, "mx": 5, X.TIMESTAMP: 10},
+                                             2: {"k": 2, "s": 3, "mx": 3, X.TIMESTAMP: 20}}
+    assert out[2] == ({}, {}) and out[3] == ({}, {})
+    assert out[4] == ({1: {"k": 1, "s": 5, "mx": 5, X.TIMESTAMP: 31}}, {1: {"k": 1, "s": 12, "mx": 7, X.TIMESTAMP: 31}})
+    # unkeyed, SUM wrapping at 64 bits, and an AVG whose exact mean moves below one f64 ulp: suppressed
+    big = (1 << 62)
+    ev = [("batch", {"a": np.array([big, big], dtype=np.int64), X.TIMESTAMP: np.array([1, 2], dtype=np.int64)}),
+          ("flush",),
+          ("batch", {"a": np.array([big + 1], dtype=np.int64), X.TIMESTAMP: np.array([3], dtype=np.int64)}),
+          ("flush",)]
+    out = X.updating_changes(ev, None, [A("avg", "a", "av")])
+    assert list(out[0][1]) == [None] and float(out[0][1][None]["av"].exact) == float(big)
+    assert out[1] == ({}, {})
+    out = X.updating_changes(ev, None, [A("sum", "a", "s")])
+    assert out[0][1][None]["s"] == -(1 << 63) and out[1][0][None]["s"] == -(1 << 63)
+    assert out[1][1][None]["s"] == -(1 << 63) + big + 1
