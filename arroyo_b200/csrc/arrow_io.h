@@ -4,6 +4,7 @@
 // (arroyo-udf/arroyo-udf-common/src/lib.rs:12-69).
 #pragma once
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -104,6 +105,34 @@ inline void require_join_key_type(const std::string& f, const std::string& seen_
   for (const std::string* s : {&seen_this, &seen_other})
     if (!s->empty() && join_key_class(*s) != k)
       throw Error(ARROYO_B200_UNSUPPORTED, "join key of type '" + f + "' after keys of type '" + *s + "'");
+}
+
+// One input of a join: its columns are the leading `_key_*` routing copies (`n_routing` of them), then the key, the
+// timestamp and the payload in any order.  The routing copies are stripped from the output like `unkeyed_batch`
+// does (arroyo-rpc/src/df.rs:359-367) and never reach the device.
+struct JoinSide {
+  int n_cols = 0, ts_col = 0, key_col = 0, n_routing = 0;
+  std::vector<int> payload;          // input column indices that appear in the output
+  std::vector<std::string> formats;  // Arrow format per input column
+  std::string key_format;            // the key's format once a host batch has shown it
+  std::vector<DevBuf> cols;          // device columns (the routing columns stay empty)
+};
+
+inline void init_join_side(JoinSide& s, int n_cols, int ts_col, int key_col, int n_routing) {
+  AB_REQUIRE(n_cols >= 2 && n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad join side n_cols");
+  AB_REQUIRE(ts_col >= 0 && ts_col < n_cols && key_col >= 0 && key_col < n_cols && n_routing >= 0 && n_routing < n_cols,
+             ARROYO_B200_INVALID_ARGUMENT, "bad join side columns");
+  AB_REQUIRE(key_col >= n_routing && ts_col >= n_routing, ARROYO_B200_INVALID_ARGUMENT,
+             "join key or timestamp column among the routing columns");
+  s.n_cols = n_cols;
+  s.ts_col = ts_col;
+  s.key_col = key_col;
+  s.n_routing = n_routing;
+  for (int i = n_routing; i < n_cols; ++i)
+    if (i != ts_col) s.payload.push_back(i);
+  s.formats.assign(n_cols, "l");
+  s.formats[ts_col] = "tsn:";
+  s.cols.resize(n_cols);
 }
 
 // ---- export -------------------------------------------------------------------------------
@@ -216,6 +245,47 @@ inline void batches_finish(BatchesPriv* p, ArroyoB200Batches* out) {
   out->arrays = p->arrays.empty() ? nullptr : p->arrays.data();
   out->schemas = p->schemas.empty() ? nullptr : p->schemas.data();
   out->private_data = p;
+}
+
+// Device-to-host copy of `bytes` into a pooled pinned buffer (8 bytes at least, so an empty column still owns one),
+// enqueued on `s`; `*d2h_bytes` counts the bytes copied.
+inline void* d2h_pinned(const void* dev, size_t bytes, cudaStream_t s, uint64_t* d2h_bytes) {
+  void* h = PinnedPool::get().alloc(std::max<size_t>(bytes, 8));
+  if (bytes) AB_CUDA(cudaMemcpyAsync(h, dev, bytes, cudaMemcpyDeviceToHost, s));
+  *d2h_bytes += bytes;
+  return h;
+}
+
+// Appends the windowed output batch of the window and session aggregates to `out`: the columns `[key?, aggs...]`
+// with the `window{start, end}` struct inserted at `window_pos` (no struct when `wstart` is null), then `_timestamp`
+// (arroyo-planner extension/aggregate.rs:306-389).  `key` is null when the operator is unkeyed.  The columns are
+// copied on `s`: nothing may read the batch before `s` has passed the copies.
+inline void export_window_batch(BatchesPriv* out, int64_t n, cudaStream_t s, uint64_t* d2h_bytes, const void* key,
+                                const std::string& key_format, const DevBuf* aggs,
+                                const std::vector<std::string>& agg_formats, const void* wstart, const void* wend,
+                                int window_pos, const void* ts) {
+  auto column = [&](const std::string& name, const std::string& format, const void* dev) {
+    OutColumn c;
+    c.name = name;
+    c.format = format;
+    c.data = d2h_pinned(dev, (size_t)n * 8, s, d2h_bytes);
+    return c;
+  };
+  std::vector<OutColumn> cols;
+  if (key) cols.push_back(column("key", key_format, key));
+  for (size_t g = 0; g < agg_formats.size(); ++g)
+    cols.push_back(column("agg" + std::to_string(g), agg_formats[g], aggs[g].p));
+  if (wstart) {
+    OutColumn w;
+    w.name = "window";
+    w.format = "+s";
+    w.children = {column("start", "tsn:", wstart), column("end", "tsn:", wend)};
+    cols.insert(cols.begin() + window_pos, w);
+  }
+  cols.push_back(column("_timestamp", "tsn:", ts));
+  out->arrays.emplace_back();
+  out->schemas.emplace_back();
+  export_batch(cols, n, &out->arrays.back(), &out->schemas.back());
 }
 
 inline void batches_release(ArroyoB200Batches* b) {

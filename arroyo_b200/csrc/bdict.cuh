@@ -26,13 +26,6 @@ constexpr int BD_CAPB = 1280;      // ids per bucket
 constexpr int BD_MEAN = 1024;      // target keys per bucket when sizing n_buckets
 constexpr uint32_t BD_ID_BASE = 2;  // id 0 = the key that equals the empty sentinel, id 1 unused (keeps bucket ranges 16-byte aligned)
 
-#ifndef AB_ID_CONSTANTS
-#define AB_ID_CONSTANTS
-constexpr uint32_t ID_UNSET = 0xFFFFFFFFu;
-constexpr uint32_t ID_OVERFLOW = 0xFFFFFFFEu;
-constexpr long long EMPTY_KEY = LLONG_MIN;
-#endif
-
 struct alignas(16) BSlot {
   long long key;
   uint32_t idx;  // index inside the bucket

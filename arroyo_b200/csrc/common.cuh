@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <climits>
 #include <cstdio>
 #include <cstring>
 #include <map>
@@ -36,6 +37,12 @@ inline void cuda_check(cudaError_t e, const char* what, const char* file, int li
   do {                                                 \
     if (!(cond)) throw ::ab::Error((status), (msg));   \
   } while (0)
+
+// Key dictionaries (dict.cuh, bdict.cuh): the id of a slot not yet published, the id of a key that found no room,
+// and the key of an empty slot (the INT64_MIN key itself gets a reserved id instead of a slot).
+constexpr uint32_t ID_UNSET = 0xFFFFFFFFu;
+constexpr uint32_t ID_OVERFLOW = 0xFFFFFFFEu;
+constexpr long long EMPTY_KEY = LLONG_MIN;
 
 // ---------------------------------------------------------------------------------------------
 // exact unsigned 64-bit division by an invariant divisor (d >= 2), branch free.

@@ -203,12 +203,8 @@ __global__ void compact_kernel(const long long* __restrict__ src, const unsigned
     if (!elig[i]) dst[off[i]] = src[i];
 }
 
-struct Side {
-  int n_cols = 0, ts_col = 0, key_col = 0, n_routing = 0;
-  std::vector<int> payload;             // input column indices that appear in the output
-  std::vector<std::string> formats;     // Arrow format per input column
-  std::string key_format;               // the key's format once a host batch has shown it
-  std::vector<DevBuf> cols, cols_alt;   // arenas (and the compaction target)
+struct Side : JoinSide {
+  std::vector<DevBuf> cols_alt;  // compaction target of `cols`
   int64_t n = 0, cap = 0;
   DevBuf elig, cnt, off;
   int64_t scratch_cap = 0;
@@ -236,17 +232,13 @@ class InstantJoinOp final : public OpBase {
   void handle_checkpoint(int64_t, BatchesPriv*) override { flush(); }  // tables left/right are written by the shim
   void on_close(int, BatchesPriv*) override { flush(); }
   void flush() override {
-    AB_CUDA(cudaSetDevice(device_));
+    set_device();
     AB_CUDA(cudaStreamSynchronize(stream_));
     release_inputs();
   }
   void stats(ArroyoB200Stats* out) override { *out = st_; }
 
  private:
-  int device_;
-  cudaStream_t stream_ = nullptr;
-  bool own_stream_ = false;
-  int num_sms_ = 132;  // set from the device at creation
   int join_type_;
   Side side_[2];
   int64_t last_wm_ = INT64_MIN;
@@ -273,52 +265,20 @@ InstantJoinOp::InstantJoinOp(const ArroyoB200OpConfig& c) {
   name = "InstantJoin";
   join_type_ = c.join_type;
   AB_REQUIRE(join_type_ >= 0 && join_type_ <= 3, ARROYO_B200_INVALID_ARGUMENT, "bad join type");
-  auto init_side = [&](Side& s, int n_cols, int ts_col, int key_col, int n_routing) {
-    AB_REQUIRE(n_cols >= 2 && n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad join side n_cols");
-    AB_REQUIRE(ts_col >= 0 && ts_col < n_cols && key_col >= 0 && key_col < n_cols && n_routing >= 0 && n_routing < n_cols,
-               ARROYO_B200_INVALID_ARGUMENT, "bad join side columns");
-    // the routing copies never reach the device: the key and the timestamp must be payload columns
-    AB_REQUIRE(key_col >= n_routing && ts_col >= n_routing, ARROYO_B200_INVALID_ARGUMENT,
-               "join key or timestamp column among the routing columns");
-    s.n_cols = n_cols;
-    s.ts_col = ts_col;
-    s.key_col = key_col;
-    s.n_routing = n_routing;
-    for (int i = n_routing; i < n_cols; ++i)
-      if (i != ts_col) s.payload.push_back(i);
-    s.cols.resize(n_cols);
-    s.cols_alt.resize(n_cols);
-    s.formats.assign(n_cols, "l");
-    s.formats[ts_col] = "tsn:";
-  };
-  init_side(side_[0], c.n_cols, c.timestamp_col, c.left_key_col, c.left_n_routing);
-  init_side(side_[1], c.right_n_cols, c.right_timestamp_col, c.right_key_col, c.right_n_routing);
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0)
-    throw Error(ARROYO_B200_FATAL, "no CUDA device available: libarroyo_b200 has no CPU fallback");
-  device_ = c.device;
-  AB_REQUIRE(device_ >= 0 && device_ < count, ARROYO_B200_INVALID_ARGUMENT, "bad device ordinal");
-  AB_CUDA(cudaSetDevice(device_));
-  cudaDeviceProp prop{};
-  AB_CUDA(cudaGetDeviceProperties(&prop, device_));
-  num_sms_ = prop.multiProcessorCount;
-  if (c.stream) stream_ = (cudaStream_t)c.stream;
-  else {
-    AB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    own_stream_ = true;
-  }
+  init_join_side(side_[0], c.n_cols, c.timestamp_col, c.left_key_col, c.left_n_routing);
+  init_join_side(side_[1], c.right_n_cols, c.right_timestamp_col, c.right_key_col, c.right_n_routing);
+  for (Side& s : side_) s.cols_alt.resize(s.n_cols);
+  open_device(c);
   scalars_.alloc(8 * sizeof(unsigned long long));
   h_scalars_.alloc(8 * sizeof(unsigned long long));
 }
 
 InstantJoinOp::~InstantJoinOp() {
-  cudaSetDevice(device_);
-  cudaStreamSynchronize(stream_);
+  drain_stream();
   for (auto& p : pending_) {
     if (p.second.release) p.second.release(&p.second);
     cudaEventDestroy(p.first);
   }
-  if (own_stream_ && stream_) cudaStreamDestroy(stream_);
 }
 
 void InstantJoinOp::release_inputs() {
@@ -358,7 +318,7 @@ void InstantJoinOp::append(Side& s, const uint64_t* const* cols, int64_t n, bool
 }
 
 void InstantJoinOp::process_batch(uint32_t index, uint32_t in_partitions, ArrowArray* batch, const ArrowSchema* schema) {
-  AB_CUDA(cudaSetDevice(device_));
+  set_device();
   AB_REQUIRE(in_partitions >= 2 && in_partitions % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
   const int sd = (int)(index / (in_partitions / 2));  // instant_join.rs:249-253
   AB_REQUIRE(sd == 0 || sd == 1, ARROYO_B200_INVALID_ARGUMENT, "bad input index");
@@ -382,7 +342,7 @@ void InstantJoinOp::process_batch(uint32_t index, uint32_t in_partitions, ArrowA
 
 void InstantJoinOp::process_device_batch(uint32_t index, uint32_t in_partitions, const uint64_t* cols, int32_t n_cols,
                                          int64_t n_rows) {
-  AB_CUDA(cudaSetDevice(device_));
+  set_device();
   AB_REQUIRE(in_partitions >= 2 && in_partitions % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
   const int sd = (int)(index / (in_partitions / 2));
   AB_REQUIRE(sd == 0 || sd == 1, ARROYO_B200_INVALID_ARGUMENT, "bad input index");
@@ -420,15 +380,8 @@ void InstantJoinOp::compact(Side& s) {
   ++st_.kernel_launches;
 }
 
-static void* d2h(const void* dev, size_t bytes, cudaStream_t s, uint64_t* acc) {
-  void* h = PinnedPool::get().alloc(std::max<size_t>(bytes, 8));
-  if (bytes) AB_CUDA(cudaMemcpyAsync(h, dev, bytes, cudaMemcpyDeviceToHost, s));
-  *acc += bytes;
-  return h;
-}
-
 void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vector<ArroyoB200DeviceBatch>* out_dev) {
-  AB_CUDA(cudaSetDevice(device_));
+  set_device();
   // validated before any state changes: a refused call must leave the eligible rows where they are
   AB_REQUIRE(out_host != nullptr || join_type_ == ARROYO_B200_JOIN_INNER, ARROYO_B200_UNSUPPORTED,
              "device-resident join output is only available for inner joins (no validity bitmaps)");
@@ -575,13 +528,13 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
           OutColumn o;
           o.name = std::string(sd == 0 ? "l" : "r") + std::to_string(c);
           o.format = s.formats[c];
-          o.data = d2h(out_cols_[oc].p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
+          o.data = d2h_pinned(out_cols_[oc].p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
           if (nullable) {
             const size_t words = (size_t)((n_out + 31) / 32);
             if (bits.bytes < words * 4) bits.alloc(words * 4 + 64);
             pack_bits_kernel<<<grid_for(n_out), JT, 0, stream_>>>(out_valid_[oc].as<unsigned char>(), n_out, bits.as<unsigned int>());
             AB_CUDA(cudaGetLastError());
-            o.validity = d2h(bits.p, words * 4, stream_, &st_.d2h_bytes);
+            o.validity = d2h_pinned(bits.p, words * 4, stream_, &st_.d2h_bytes);
             AB_CUDA(cudaStreamSynchronize(stream_));  // `bits` is reused by the next column
             const unsigned int* w = (const unsigned int*)o.validity;
             int64_t set = 0;
@@ -600,7 +553,7 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
       OutColumn t;
       t.name = "_timestamp";
       t.format = "tsn:";
-      t.data = d2h(out_ts_.p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
+      t.data = d2h_pinned(out_ts_.p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
       cols.push_back(t);
       AB_CUDA(cudaStreamSynchronize(stream_));
       out_host->arrays.emplace_back();

@@ -16,7 +16,11 @@ class OpBase {
   std::string last_error;
   std::string name;
 
-  virtual ~OpBase() {}
+  // Destroys the stream the operator created.  Each operator's own destructor calls drain_stream() first: nothing may
+  // still run on the stream when its buffers and input batches are released.
+  virtual ~OpBase() {
+    if (own_stream_) cudaStreamDestroy(stream_);
+  }
   virtual void on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t watermark, int64_t table_min) = 0;
   virtual void process_batch(uint32_t index, uint32_t in_partitions, ArrowArray* batch, const ArrowSchema* schema) = 0;
   // process_batch for operators that emit from it (the TTL join); everything else emits nothing here
@@ -53,6 +57,38 @@ class OpBase {
     pending_dev.clear();
   }
   virtual void stats(ArroyoB200Stats* out) = 0;
+
+ protected:
+  int device_ = 0;
+  cudaStream_t stream_ = nullptr;
+  bool own_stream_ = false;
+  int num_sms_ = 132;  // set from the device by open_device
+
+  // Every constructor calls this once its config is valid, so a bad config is refused without touching CUDA: takes
+  // device `c.device` and the caller's stream `c.stream`, or a new non-blocking stream when none is given.
+  void open_device(const ArroyoB200OpConfig& c) {
+    int count = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0)
+      throw Error(ARROYO_B200_FATAL, "no CUDA device available: libarroyo_b200 has no CPU fallback");
+    AB_REQUIRE(c.device >= 0 && c.device < count, ARROYO_B200_INVALID_ARGUMENT, "bad device ordinal");
+    device_ = c.device;
+    set_device();
+    cudaDeviceProp prop{};
+    AB_CUDA(cudaGetDeviceProperties(&prop, device_));
+    num_sms_ = prop.multiProcessorCount;
+    if (c.stream) {
+      stream_ = (cudaStream_t)c.stream;
+    } else {
+      AB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+      own_stream_ = true;
+    }
+  }
+  void set_device() const { AB_CUDA(cudaSetDevice(device_)); }
+  // first step of a destructor (errors are ignored there)
+  void drain_stream() const {
+    cudaSetDevice(device_);
+    cudaStreamSynchronize(stream_);
+  }
 };
 
 OpBase* make_window_agg_op(const ArroyoB200OpConfig& cfg);

@@ -31,6 +31,7 @@
 
 #include <cub/device/device_segmented_sort.cuh>
 
+#include "agg_plan.h"
 #include "dict.cuh"
 #include "op.h"
 #include "scan.cuh"
@@ -38,15 +39,12 @@
 namespace ab {
 namespace {
 
-constexpr int SV = 4;                            // value columns
-constexpr int SA = ARROYO_B200_MAX_AGGS + 1;      // accumulators (0 = rows)
-enum : int { K_ROWS = 0, K_SUM_I64 = 1, K_SUM_F64 = 2, K_MIN = 3, K_MAX = 4 };
 constexpr int ST = 256;
 
 struct SessCtx {
   long long gap;
   int n_vals, n_acc;
-  int acc_kind[SA], acc_val[SA];
+  int acc_kind[MAX_ACC], acc_val[MAX_ACC];
   unsigned long long id_cap;
   // per key
   int* active;
@@ -61,7 +59,7 @@ struct SessCtx {
   int* n_len;
   // row pool
   long long* r_ts;
-  long long* r_val[SV];
+  long long* r_val[MAX_VALS];
   // cursors / counters: [0] node cursor, [1] row cursor, [2] dead nodes, [3] dead rows, [4] out count,
   // [5] error flags, [6] arena cursor, [7] sessions open
   unsigned long long* ctr;
@@ -87,7 +85,7 @@ __device__ __forceinline__ unsigned long long loop_guard(const SessCtx& c) { ret
 
 struct RowsRef {
   const long long* ts;
-  const long long* val[SV];
+  const long long* val[MAX_VALS];
   long long off;
   int n;
 };
@@ -118,12 +116,7 @@ __device__ __forceinline__ void publish_tally(const SessCtx& c, const Tally& t) 
 }
 
 __device__ void acc_reset(const SessCtx& c, uint32_t id) {
-  for (int a = 0; a < c.n_acc; ++a) {
-    unsigned long long v = 0;
-    if (c.acc_kind[a] == K_MIN) v = (unsigned long long)LLONG_MAX;
-    if (c.acc_kind[a] == K_MAX) v = (unsigned long long)LLONG_MIN;
-    c.acc[(unsigned long long)a * c.id_cap + id] = v;
-  }
+  for (int a = 0; a < c.n_acc; ++a) c.acc[(unsigned long long)a * c.id_cap + id] = acc_identity(c.acc_kind[a]);
 }
 
 // the session's Single-mode aggregate consumes rows [lo, hi) of r
@@ -132,7 +125,7 @@ __device__ void merge_rows(const SessCtx& c, uint32_t id, const RowsRef& r, int 
   for (int a = 0; a < c.n_acc; ++a) {
     unsigned long long* dst = c.acc + (unsigned long long)a * c.id_cap + id;
     const int kind = c.acc_kind[a];
-    if (kind == K_ROWS) {
+    if (kind == ACC_ROWS) {
       *dst += (unsigned long long)(hi - lo);
       continue;
     }
@@ -141,10 +134,10 @@ __device__ void merge_rows(const SessCtx& c, uint32_t id, const RowsRef& r, int 
     for (int i = lo; i < hi; ++i) {
       const long long v = src[i];
       switch (kind) {
-        case K_SUM_I64: cur += (unsigned long long)v; break;
-        case K_SUM_F64: cur = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cur) + (double)v); break;
-        case K_MIN: cur = (unsigned long long)min((long long)cur, v); break;
-        case K_MAX: cur = (unsigned long long)max((long long)cur, v); break;
+        case ACC_SUM_I64: cur += (unsigned long long)v; break;
+        case ACC_SUM_F64: cur = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cur) + (double)v); break;
+        case ACC_MIN_I64: cur = (unsigned long long)min((long long)cur, v); break;
+        case ACC_MAX_I64: cur = (unsigned long long)max((long long)cur, v); break;
       }
     }
     *dst = cur;
@@ -239,7 +232,7 @@ __device__ void pending_insert(const SessCtx& c, uint32_t id, int node) {
 __device__ RowsRef pool_rows(const SessCtx& c, int node) {
   RowsRef r;
   r.ts = c.r_ts;
-  for (int v = 0; v < SV; ++v) r.val[v] = c.r_val[v];
+  for (int v = 0; v < MAX_VALS; ++v) r.val[v] = c.r_val[v];
   r.off = c.n_off[node];
   r.n = c.n_len[node];
   return r;
@@ -307,18 +300,8 @@ __device__ void finish_session(const SessCtx& c, uint32_t id, Tally& tally) {
   c.o_end[o] = end;
   c.o_ts[o] = end - 1;
   const unsigned long long rows = c.acc[id];
-  for (int g = 0; g < c.n_aggs; ++g) {
-    unsigned long long v;
-    const unsigned long long a = c.acc[(unsigned long long)c.agg_acc[g] * c.id_cap + id];
-    switch (c.agg_kind[g]) {
-      case ARROYO_B200_AGG_COUNT_STAR: v = rows; break;
-      case ARROYO_B200_AGG_AVG_I64:
-        v = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) / (double)rows);
-        break;
-      default: v = a; break;
-    }
-    c.o_agg[g][o] = v;
-  }
+  for (int g = 0; g < c.n_aggs; ++g)
+    c.o_agg[g][o] = agg_finalise(c.agg_kind[g], c.acc[(unsigned long long)c.agg_acc[g] * c.id_cap + id], rows);
   c.active[id] = 0;
   tally.open -= 1;
 }
@@ -368,7 +351,7 @@ __device__ void add_run(const SessCtx& c, uint32_t id, unsigned long long node, 
 struct PrepParams {
   const long long* key;
   const long long* ts;
-  const long long* val[SV];
+  const long long* val[MAX_VALS];
   long long n;
   unsigned int seq;
   int has_wm;
@@ -380,7 +363,7 @@ struct PrepParams {
   unsigned int* a_id;
   unsigned int* a_seq;
   long long* a_ts;
-  long long* a_val[SV];
+  long long* a_val[MAX_VALS];
   unsigned int* count;  // rows per id in this launch
   unsigned long long* ctr;
   unsigned long long arena_cap;
@@ -444,14 +427,14 @@ struct GroupParams {
   const unsigned int* a_id;
   unsigned int* a_seq;  // written back only by the segmented sort of big keys, which parks rows here
   long long* a_ts;
-  long long* a_val[SV];
+  long long* a_val[MAX_VALS];
   unsigned long long n;
   int n_vals;
   const unsigned long long* offset;  // per id
   unsigned int* cursor;              // per id, zeroed
   unsigned int* g_seq;
   long long* g_ts;
-  long long* g_val[SV];
+  long long* g_val[MAX_VALS];
 };
 
 __global__ void __launch_bounds__(ST) group_kernel(const __grid_constant__ GroupParams p) {
@@ -524,7 +507,7 @@ struct ApplyParams {
   const unsigned long long* offset;
   unsigned int* g_seq;
   long long* g_ts;       // row pool + row_base: the grouping pass wrote this launch's rows straight into the pool
-  long long* g_val[SV];
+  long long* g_val[MAX_VALS];
   unsigned long long row_base, node_base;  // pool positions of grouped row 0 / of the node slot of grouped row 0
   int has_wm;
   long long wm;
@@ -545,7 +528,7 @@ __global__ void __launch_bounds__(128) apply_kernel(const __grid_constant__ Appl
     for (unsigned int i = 1; i < cnt && cnt <= SMALL_SORT; ++i) {
       const unsigned int s = p.g_seq[off + i];
       const long long t = p.g_ts[off + i];
-      long long vv[SV];
+      long long vv[MAX_VALS];
       for (int v = 0; v < p.c.n_vals; ++v) vv[v] = p.g_val[v][off + i];
       long long j = (long long)i - 1;
       while (j >= 0 && (p.g_seq[off + j] > s || (p.g_seq[off + j] == s && p.g_ts[off + j] > t))) {
@@ -614,7 +597,7 @@ struct CompactDst {
   long long* n_off;
   int* n_len;
   long long* r_ts;
-  long long* r_val[SV];
+  long long* r_val[MAX_VALS];
 };
 __global__ void compact_copy_kernel(SessCtx c, CompactDst d, unsigned int n_ids, const unsigned long long* node_off,
                                     const unsigned long long* row_off) {
@@ -668,7 +651,7 @@ class SessionOp final : public OpBase {
     AB_CUDA(cudaStreamSynchronize(stream_));
     st_.rows_late = late;
     st_.n_keys = 0;
-    if (keyed_) {
+    if (plan_.keyed) {
       // the dictionary's count (ids 1.., id 0 is INT64_MIN's) and whether an INT64_MIN key was accepted
       unsigned int nk[2] = {1, 0};
       AB_CUDA(cudaMemcpyAsync(nk, n_keys_dev_.p, sizeof nk, cudaMemcpyDeviceToHost, stream_));
@@ -679,18 +662,9 @@ class SessionOp final : public OpBase {
   }
 
  private:
-  int device_;
-  cudaStream_t stream_ = nullptr;
-  bool own_stream_ = false;
-  int num_sms_ = 132;  // set from the device at creation
-  bool keyed_;
-  int key_col_, ts_col_;
+  AggPlan plan_;
   int64_t gap_;
-  int n_vals_ = 0, val_cols_[SV];
-  int n_acc_ = 1, acc_kind_[SA], acc_val_[SA];
-  int n_aggs_, agg_kind_[ARROYO_B200_MAX_AGGS], agg_acc_[ARROYO_B200_MAX_AGGS];
   std::string key_format_ = "l";
-  std::vector<std::string> agg_format_;
 
   // dictionary + per-key state
   uint64_t id_cap_ = 0, dict_cap_ = 0;
@@ -699,19 +673,19 @@ class SessionOp final : public OpBase {
   DevBuf active_, data_start_, data_end_, acc_, head_, count_, cursor_, offset_;
   // pools
   uint64_t node_cap_ = 0, row_cap_ = 0;
-  DevBuf n_next_, n_start_, n_off_, n_len_, r_ts_, r_val_[SV];
+  DevBuf n_next_, n_start_, n_off_, n_len_, r_ts_, r_val_[MAX_VALS];
   // compaction copies the live nodes / rows into a second set of pools and swaps the sets; both sets and the scratch
   // arrays persist (a cudaMalloc / cudaFree per step synchronises the device -- and, behind an NCCL edge, waits for the
   // peers' progress: 145 ms per step at N = 2 before they were kept)
   uint64_t sp_node_cap_ = 0, sp_row_cap_ = 0;
-  DevBuf sp_next_, sp_start_, sp_off_, sp_len_, sp_rts_, sp_rval_[SV];
+  DevBuf sp_next_, sp_start_, sp_off_, sp_len_, sp_rts_, sp_rval_[MAX_VALS];
   DevBuf c_cn_, c_cr_, c_on_, c_orow_, c_tot_;
   uint64_t c_cap_ = 0;
   DevBuf ctr_;
   PinnedBuf h_ctr_;
   // launch arena
   uint64_t arena_cap_ = 0;
-  DevBuf a_id_, a_seq_, a_ts_, a_val_[SV], g_seq_;
+  DevBuf a_id_, a_seq_, a_ts_, a_val_[MAX_VALS], g_seq_;
   // segmented sort of the keys with more than SMALL_SORT rows in a launch (sized on first use)
   uint64_t sort_cap_ = 0;
   DevBuf s_key_, s_key_out_, s_idx_, s_idx_out_, s_seq_, s_seq_out_, s_begin_, s_end_, s_nseg_, s_tmp_;
@@ -730,7 +704,6 @@ class SessionOp final : public OpBase {
   DevBuf late_, earliest_;
   uint64_t compact_min_ = 1u << 16;  // pools smaller than this are never compacted (ARROYO_B200_SESSION_COMPACT_MIN)
 
-  void set_device() { AB_CUDA(cudaSetDevice(device_)); }
   int grid_for(uint64_t n, int threads) const {
     return (int)std::max<uint64_t>(1, std::min<uint64_t>((n + threads - 1) / threads, (uint64_t)num_sms_ * 16));
   }
@@ -756,68 +729,8 @@ SessionOp::SessionOp(const ArroyoB200OpConfig& c) {
   name = "session_window";
   AB_REQUIRE(c.gap_ns > 0, ARROYO_B200_INVALID_ARGUMENT, "session gap must be positive");
   gap_ = c.gap_ns;
-  AB_REQUIRE(c.n_key_cols == 0 || c.n_key_cols == 1, ARROYO_B200_UNSUPPORTED, "only 0 or 1 group-by key columns are supported");
-  keyed_ = c.n_key_cols == 1;
-  key_col_ = c.key_col;
-  ts_col_ = c.timestamp_col;
-  AB_REQUIRE(c.n_cols >= 1 && c.n_cols <= ARROYO_B200_MAX_COLS && ts_col_ >= 0 && ts_col_ < c.n_cols,
-             ARROYO_B200_INVALID_ARGUMENT, "bad input layout");
-  AB_REQUIRE(!keyed_ || (key_col_ >= 0 && key_col_ < c.n_cols), ARROYO_B200_INVALID_ARGUMENT, "bad key_col");
-  AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= ARROYO_B200_MAX_AGGS, ARROYO_B200_INVALID_ARGUMENT, "bad n_aggs");
-  n_aggs_ = c.n_aggs;
-  acc_kind_[0] = K_ROWS;
-  acc_val_[0] = 0;
-  for (int g = 0; g < n_aggs_; ++g) {
-    const int kind = c.aggs[g].kind;
-    agg_kind_[g] = kind;
-    agg_acc_[g] = 0;
-    if (kind == ARROYO_B200_AGG_COUNT_STAR) {
-      agg_format_.push_back("l");
-      continue;
-    }
-    const int col = c.aggs[g].input_col;
-    AB_REQUIRE(col >= 0 && col < c.n_cols, ARROYO_B200_INVALID_ARGUMENT, "aggregate input column out of range");
-    int vs = -1;
-    for (int v = 0; v < n_vals_; ++v)
-      if (val_cols_[v] == col) vs = v;
-    if (vs < 0) {
-      AB_REQUIRE(n_vals_ < SV, ARROYO_B200_UNSUPPORTED, "more than 4 distinct aggregate input columns");
-      vs = n_vals_;
-      val_cols_[n_vals_++] = col;
-    }
-    int ak;
-    switch (kind) {
-      case ARROYO_B200_AGG_SUM_I64: ak = K_SUM_I64; agg_format_.push_back("l"); break;
-      case ARROYO_B200_AGG_AVG_I64: ak = K_SUM_F64; agg_format_.push_back("g"); break;  // sequential f64 sum per key
-      case ARROYO_B200_AGG_MIN_I64: ak = K_MIN; agg_format_.push_back("l"); break;
-      case ARROYO_B200_AGG_MAX_I64: ak = K_MAX; agg_format_.push_back("l"); break;
-      default: throw Error(ARROYO_B200_UNSUPPORTED, "unsupported aggregate kind");
-    }
-    int found = -1;
-    for (int a = 1; a < n_acc_; ++a)
-      if (acc_kind_[a] == ak && acc_val_[a] == vs) found = a;
-    if (found < 0) {
-      found = n_acc_;
-      acc_kind_[n_acc_] = ak;
-      acc_val_[n_acc_] = vs;
-      ++n_acc_;
-    }
-    agg_acc_[g] = found;
-  }
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0)
-    throw Error(ARROYO_B200_FATAL, "no CUDA device available: libarroyo_b200 has no CPU fallback");
-  device_ = c.device;
-  AB_REQUIRE(device_ >= 0 && device_ < count, ARROYO_B200_INVALID_ARGUMENT, "bad device ordinal");
-  set_device();
-  cudaDeviceProp prop{};
-  AB_CUDA(cudaGetDeviceProperties(&prop, device_));
-  num_sms_ = prop.multiProcessorCount;
-  if (c.stream) stream_ = (cudaStream_t)c.stream;
-  else {
-    AB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    own_stream_ = true;
-  }
+  plan_ = AggPlan(c, ACC_SUM_F64);  // AVG: the sequential f64 sum per key
+  open_device(c);
   if (const char* e = getenv("ARROYO_B200_SESSION_COMPACT_MIN")) compact_min_ = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
   ctr_.alloc(8 * sizeof(unsigned long long));
   h_ctr_.alloc(8 * sizeof(unsigned long long));
@@ -832,18 +745,16 @@ SessionOp::SessionOp(const ArroyoB200OpConfig& c) {
   n_keys_dev_.alloc(2 * sizeof(unsigned int));  // [dictionary count, INT64_MIN key seen]
   AB_CUDA(cudaMemsetAsync(n_keys_dev_.p, 0, 2 * sizeof(unsigned int), stream_));
   uint64_t want = c.expected_keys ? c.expected_keys : (1ull << 16);
-  alloc_keys(keyed_ ? ((want + want / 8 + 2 + 1023) / 1024) * 1024 : 1024);
+  alloc_keys(plan_.keyed ? ((want + want / 8 + 2 + 1023) / 1024) * 1024 : 1024);
   AB_CUDA(cudaStreamSynchronize(stream_));
 }
 
 SessionOp::~SessionOp() {
-  cudaSetDevice(device_);
-  cudaStreamSynchronize(stream_);
+  drain_stream();
   for (auto& p : pending_) {
     if (p.second.release) p.second.release(&p.second);
     cudaEventDestroy(p.first);
   }
-  if (own_stream_ && stream_) cudaStreamDestroy(stream_);
 }
 
 void SessionOp::alloc_keys(uint64_t cap) {
@@ -853,7 +764,7 @@ void SessionOp::alloc_keys(uint64_t cap) {
   AB_CUDA(cudaMemcpyAsync(id_keys_.p, &k0, 8, cudaMemcpyHostToDevice, stream_));
   unsigned int one = 1;
   AB_CUDA(cudaMemcpyAsync(n_keys_dev_.p, &one, 4, cudaMemcpyHostToDevice, stream_));
-  if (keyed_) {
+  if (plan_.keyed) {
     dict_cap_ = dict_slots_for(cap);
     AB_REQUIRE(dict_cap_ <= (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
     slots_.alloc(dict_cap_ * sizeof(Slot));
@@ -863,7 +774,7 @@ void SessionOp::alloc_keys(uint64_t cap) {
   active_.alloc(cap * 4);
   data_start_.alloc(cap * 8);
   data_end_.alloc(cap * 8);
-  acc_.alloc((size_t)n_acc_ * cap * 8);
+  acc_.alloc((size_t)plan_.n_acc * cap * 8);
   head_.alloc(cap * 4);
   count_.alloc(cap * 4);
   cursor_.alloc(cap * 4);
@@ -910,8 +821,8 @@ void SessionOp::grow_keys(uint64_t need) {
     head_ = std::move(nb);
   }
   {
-    DevBuf nb((size_t)n_acc_ * nc * 8);
-    for (int a = 0; a < n_acc_; ++a)
+    DevBuf nb((size_t)plan_.n_acc * nc * 8);
+    for (int a = 0; a < plan_.n_acc; ++a)
       AB_CUDA(cudaMemcpyAsync(nb.as<unsigned long long>() + (size_t)a * nc, acc_.as<unsigned long long>() + (size_t)a * oc,
                               nv * 8, cudaMemcpyDeviceToDevice, stream_));
     AB_CUDA(cudaStreamSynchronize(stream_));
@@ -919,7 +830,7 @@ void SessionOp::grow_keys(uint64_t need) {
   }
   offset_.alloc(nc * 8);
   id_cap_ = nc;
-  if (keyed_) {
+  if (plan_.keyed) {
     dict_cap_ = dict_slots_for(nc);
     AB_REQUIRE(dict_cap_ <= (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
     slots_.alloc(dict_cap_ * sizeof(Slot));
@@ -957,7 +868,7 @@ void SessionOp::ensure_pools(uint64_t add_nodes, uint64_t add_rows) {
     uint64_t rc = std::max<uint64_t>(row_cap_ * 2, 1 << 16);
     while (rows + add_rows > rc) rc *= 2;
     regrow(r_ts_, 8, rows, rc);
-    for (int v = 0; v < n_vals_; ++v) regrow(r_val_[v], 8, rows, rc);
+    for (int v = 0; v < plan_.n_vals; ++v) regrow(r_val_[v], 8, rows, rc);
     row_cap_ = rc;
   }
 }
@@ -971,18 +882,18 @@ void SessionOp::ensure_arena(uint64_t rows) {
   a_seq_.alloc(nc * 4);
   a_ts_.alloc(nc * 8);
   g_seq_.alloc(nc * 4);  // grouped timestamps / values go straight into the row pool (apply_pending)
-  for (int v = 0; v < n_vals_; ++v) a_val_[v].alloc(nc * 8);
+  for (int v = 0; v < plan_.n_vals; ++v) a_val_[v].alloc(nc * 8);
   arena_cap_ = nc;
 }
 
 SessCtx SessionOp::ctx() {
   SessCtx c{};
   c.gap = gap_;
-  c.n_vals = n_vals_;
-  c.n_acc = n_acc_;
-  for (int a = 0; a < n_acc_; ++a) {
-    c.acc_kind[a] = acc_kind_[a];
-    c.acc_val[a] = acc_val_[a];
+  c.n_vals = plan_.n_vals;
+  c.n_acc = plan_.n_acc;
+  for (int a = 0; a < plan_.n_acc; ++a) {
+    c.acc_kind[a] = plan_.acc_kind[a];
+    c.acc_val[a] = plan_.acc_val[a];
   }
   c.id_cap = id_cap_;
   c.active = active_.as<int>();
@@ -995,7 +906,7 @@ SessCtx SessionOp::ctx() {
   c.n_off = n_off_.as<long long>();
   c.n_len = n_len_.as<int>();
   c.r_ts = r_ts_.as<long long>();
-  for (int v = 0; v < SV; ++v) c.r_val[v] = v < n_vals_ ? r_val_[v].as<long long>() : nullptr;
+  for (int v = 0; v < MAX_VALS; ++v) c.r_val[v] = v < plan_.n_vals ? r_val_[v].as<long long>() : nullptr;
   c.ctr = ctr_.as<unsigned long long>();
   c.node_cap = node_cap_;
   c.row_cap = row_cap_;
@@ -1004,14 +915,14 @@ SessCtx SessionOp::ctx() {
   c.o_start = o_start_.as<long long>();
   c.o_end = o_end_.as<long long>();
   c.o_ts = o_ts_.as<long long>();
-  c.n_aggs = n_aggs_;
-  for (int g = 0; g < n_aggs_; ++g) {
+  c.n_aggs = plan_.n_aggs;
+  for (int g = 0; g < plan_.n_aggs; ++g) {
     c.o_agg[g] = o_agg_[g].as<unsigned long long>();
-    c.agg_kind[g] = agg_kind_[g];
-    c.agg_acc[g] = agg_acc_[g];
+    c.agg_kind[g] = plan_.agg_kind[g];
+    c.agg_acc[g] = plan_.agg_acc[g];
   }
   c.out_cap = out_cap_;
-  c.keyed = keyed_ ? 1 : 0;
+  c.keyed = plan_.keyed ? 1 : 0;
   return c;
 }
 
@@ -1048,29 +959,27 @@ void SessionOp::prep(const long long* key, const long long* ts, const long long*
   if (arena_rows_bound_ + (uint64_t)n > (1ull << 22) && arena_rows_bound_ > 0) apply_pending();
   if (arena_rows_bound_ + (uint64_t)n > arena_cap_ && arena_rows_bound_ > 0) apply_pending();
   ensure_arena(arena_rows_bound_ + (uint64_t)n);
-  if (keyed_) grow_keys((uint64_t)n);
+  if (plan_.keyed) grow_keys((uint64_t)n);
   PrepParams p{};
   p.key = key;
   p.ts = ts;
-  for (int v = 0; v < n_vals_; ++v) p.val[v] = vals[v];
+  for (int v = 0; v < plan_.n_vals; ++v) p.val[v] = vals[v];
   p.n = n;
   p.seq = seq_++;
   p.has_wm = has_wm_ ? 1 : 0;
   p.wm = wm_;
-  p.keyed = keyed_ ? 1 : 0;
-  p.n_vals = n_vals_;
+  p.keyed = plan_.keyed ? 1 : 0;
+  p.n_vals = plan_.n_vals;
   p.dict.slots = slots_.as<Slot>();
   p.dict.id_keys = id_keys_.as<long long>();
   p.dict.n_keys = n_keys_dev_.as<unsigned int>();
   p.min_key_seen = n_keys_dev_.as<unsigned int>() + 1;
-  p.dict.cap = keyed_ ? (uint32_t)dict_cap_ : 1;
+  p.dict.cap = plan_.keyed ? (uint32_t)dict_cap_ : 1;
   p.dict.id_cap = (uint32_t)std::min<uint64_t>(id_cap_, 0xFFFFFFF0ull);
-  p.dict.dbase = 0;
-  p.dict.dn = 0;  // sessions keep every key in the slot array
   p.a_id = a_id_.as<unsigned int>();
   p.a_seq = a_seq_.as<unsigned int>();
   p.a_ts = a_ts_.as<long long>();
-  for (int v = 0; v < n_vals_; ++v) p.a_val[v] = a_val_[v].as<long long>();
+  for (int v = 0; v < plan_.n_vals; ++v) p.a_val[v] = a_val_[v].as<long long>();
   p.count = count_.as<unsigned int>();
   p.ctr = ctr_.as<unsigned long long>();
   p.arena_cap = arena_cap_;
@@ -1082,7 +991,7 @@ void SessionOp::prep(const long long* key, const long long* ts, const long long*
   ++st_.ingest_launches;
   arena_rows_bound_ += (uint64_t)n;
   // n_keys grows with the rows seen; keep a conservative host bound for capacity planning
-  n_keys_ = (uint32_t)std::min<uint64_t>((uint64_t)n_keys_ + (keyed_ ? (uint64_t)n : 0), id_cap_);
+  n_keys_ = (uint32_t)std::min<uint64_t>((uint64_t)n_keys_ + (plan_.keyed ? (uint64_t)n : 0), id_cap_);
 }
 
 void SessionOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const ArrowSchema* schema) {
@@ -1090,8 +999,8 @@ void SessionOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arrow
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
-  require_aggregate_input_types(cols, keyed_ ? key_col_ : -1, val_cols_, n_vals_);
-  if (keyed_) key_format_ = cols[key_col_].format;
+  require_aggregate_input_types(cols, plan_.keyed ? plan_.key_col : -1, plan_.val_cols, plan_.n_vals);
+  if (plan_.keyed) key_format_ = cols[plan_.key_col].format;
   release_inputs(false);
   st_.rows_in += (uint64_t)n;
   if (n == 0) {
@@ -1099,22 +1008,22 @@ void SessionOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arrow
     return;
   }
   // stage the used columns (the staging buffer is reused in stream order)
-  const int n_used = 2 + n_vals_;
+  const int n_used = 2 + plan_.n_vals;
   if ((uint64_t)n > staging_cap_) {
     AB_CUDA(cudaStreamSynchronize(stream_));
     staging_cap_ = std::max<uint64_t>((uint64_t)n, staging_cap_ * 2);
     staging_.alloc((size_t)n_used * staging_cap_ * 8);
   }
   long long* base = staging_.as<long long>();
-  const long long* vals[SV] = {nullptr, nullptr, nullptr, nullptr};
-  if (keyed_) AB_CUDA(cudaMemcpyAsync(base, cols[key_col_].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  AB_CUDA(cudaMemcpyAsync(base + staging_cap_, cols[ts_col_].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  for (int v = 0; v < n_vals_; ++v) {
-    AB_CUDA(cudaMemcpyAsync(base + (size_t)(2 + v) * staging_cap_, cols[val_cols_[v]].data, (size_t)n * 8,
+  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
+  if (plan_.keyed) AB_CUDA(cudaMemcpyAsync(base, cols[plan_.key_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
+  AB_CUDA(cudaMemcpyAsync(base + staging_cap_, cols[plan_.ts_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
+  for (int v = 0; v < plan_.n_vals; ++v) {
+    AB_CUDA(cudaMemcpyAsync(base + (size_t)(2 + v) * staging_cap_, cols[plan_.val_cols[v]].data, (size_t)n * 8,
                             cudaMemcpyHostToDevice, stream_));
     vals[v] = base + (size_t)(2 + v) * staging_cap_;
   }
-  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((keyed_ ? 1 : 0) + 1 + n_vals_);
+  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((plan_.keyed ? 1 : 0) + 1 + plan_.n_vals);
   cudaEvent_t ev;
   AB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   AB_CUDA(cudaEventRecord(ev, stream_));
@@ -1128,9 +1037,9 @@ void SessionOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols, i
   AB_REQUIRE(n_cols == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
   if (n_rows <= 0) return;
   st_.rows_in += (uint64_t)n_rows;
-  const long long* vals[SV] = {nullptr, nullptr, nullptr, nullptr};
-  for (int v = 0; v < n_vals_; ++v) vals[v] = (const long long*)cols[val_cols_[v]];
-  prep(keyed_ ? (const long long*)cols[key_col_] : nullptr, (const long long*)cols[ts_col_], vals, n_rows);
+  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
+  for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)cols[plan_.val_cols[v]];
+  prep(plan_.keyed ? (const long long*)cols[plan_.key_col] : nullptr, (const long long*)cols[plan_.ts_col], vals, n_rows);
 }
 
 // group the arena by key and run the per-key state machines over the new runs
@@ -1140,7 +1049,7 @@ void SessionOp::apply_pending() {
   check_err();
   const uint64_t n = h_ctr_.as<unsigned long long>()[6];
   unsigned int nk = 1;
-  if (keyed_) {
+  if (plan_.keyed) {
     AB_CUDA(cudaMemcpyAsync(&nk, n_keys_dev_.p, 4, cudaMemcpyDeviceToHost, stream_));
     AB_CUDA(cudaStreamSynchronize(stream_));
   }
@@ -1163,7 +1072,7 @@ void SessionOp::apply_pending() {
   g.a_seq = a_seq_.as<unsigned int>();
   g.a_ts = a_ts_.as<long long>();
   g.n = n;
-  g.n_vals = n_vals_;
+  g.n_vals = plan_.n_vals;
   g.offset = offset_.as<unsigned long long>();
   g.cursor = cursor_.as<unsigned int>();
   // This launch's rows go straight into the row pool at [row_base, row_base + n) in grouped order, and grouped
@@ -1176,7 +1085,7 @@ void SessionOp::apply_pending() {
   AB_CUDA(cudaMemcpyAsync(ctr_.as<unsigned long long>(), cur2, sizeof cur2, cudaMemcpyHostToDevice, stream_));
   g.g_seq = g_seq_.as<unsigned int>();
   g.g_ts = cx.r_ts + row_base;
-  for (int v = 0; v < n_vals_; ++v) {
+  for (int v = 0; v < plan_.n_vals; ++v) {
     g.a_val[v] = a_val_[v].as<long long>();
     g.g_val[v] = cx.r_val[v] + row_base;
   }
@@ -1191,7 +1100,7 @@ void SessionOp::apply_pending() {
   a.offset = offset_.as<unsigned long long>();
   a.g_seq = g_seq_.as<unsigned int>();
   a.g_ts = cx.r_ts + row_base;
-  for (int v = 0; v < n_vals_; ++v) a.g_val[v] = cx.r_val[v] + row_base;
+  for (int v = 0; v < plan_.n_vals; ++v) a.g_val[v] = cx.r_val[v] + row_base;
   a.row_base = row_base;
   a.node_base = node_base;
   a.has_wm = has_wm_ ? 1 : 0;
@@ -1371,7 +1280,7 @@ void SessionOp::maybe_compact() {
   }
   if (sp_row_cap_ < rcap) {
     sp_rts_.alloc(rcap * 8);
-    for (int v = 0; v < n_vals_; ++v) sp_rval_[v].alloc(rcap * 8);
+    for (int v = 0; v < plan_.n_vals; ++v) sp_rval_[v].alloc(rcap * 8);
     sp_row_cap_ = rcap;
   }
   CompactDst d{};
@@ -1380,7 +1289,7 @@ void SessionOp::maybe_compact() {
   d.n_off = sp_off_.as<long long>();
   d.n_len = sp_len_.as<int>();
   d.r_ts = sp_rts_.as<long long>();
-  for (int v = 0; v < n_vals_; ++v) d.r_val[v] = sp_rval_[v].as<long long>();
+  for (int v = 0; v < plan_.n_vals; ++v) d.r_val[v] = sp_rval_[v].as<long long>();
   compact_copy_kernel<<<grid_for(n_keys_, 128), 128, 0, stream_>>>(c, d, n_keys_, on.as<unsigned long long>(),
                                                                   orow.as<unsigned long long>());
   AB_CUDA(cudaGetLastError());
@@ -1392,17 +1301,10 @@ void SessionOp::maybe_compact() {
   std::swap(n_off_, sp_off_);
   std::swap(n_len_, sp_len_);
   std::swap(r_ts_, sp_rts_);
-  for (int v = 0; v < n_vals_; ++v) std::swap(r_val_[v], sp_rval_[v]);
+  for (int v = 0; v < plan_.n_vals; ++v) std::swap(r_val_[v], sp_rval_[v]);
   std::swap(node_cap_, sp_node_cap_);
   std::swap(row_cap_, sp_row_cap_);
   st_.kernel_launches += 8;
-}
-
-static void* d2h_col(const void* dev, int64_t n, cudaStream_t s, uint64_t* bytes) {
-  void* h = PinnedPool::get().alloc((size_t)std::max<int64_t>(n, 1) * 8);
-  if (n > 0) AB_CUDA(cudaMemcpyAsync(h, dev, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-  *bytes += (uint64_t)n * 8;
-  return h;
 }
 
 void SessionOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vector<ArroyoB200DeviceBatch>* out_dev) {
@@ -1421,7 +1323,7 @@ void SessionOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vector<
     o_start_.alloc(out_cap_ * 8);
     o_end_.alloc(out_cap_ * 8);
     o_ts_.alloc(out_cap_ * 8);
-    for (int g = 0; g < n_aggs_; ++g) o_agg_[g].alloc(out_cap_ * 8);
+    for (int g = 0; g < plan_.n_aggs; ++g) o_agg_[g].alloc(out_cap_ * 8);
   }
   ensure_pools(live_rows + 16, 0);  // remainders created while filling
   unsigned long long zero = 0;
@@ -1452,52 +1354,19 @@ void SessionOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vector<
     if (out_host) {
       // [key cols...] with the window struct inserted at window_index, [agg cols...], _timestamp
       // (session_aggregating_window.rs:316-382)
-      std::vector<OutColumn> cols;
-      if (keyed_) {
-        OutColumn k;
-        k.name = "key";
-        k.format = key_format_;
-        k.data = d2h_col(o_key_.p, n, stream_, &st_.d2h_bytes);
-        cols.push_back(k);
-      }
-      OutColumn w;
-      w.name = "window";
-      w.format = "+s";
-      OutColumn ws, we;
-      ws.name = "start";
-      ws.format = "tsn:";
-      ws.data = d2h_col(o_start_.p, n, stream_, &st_.d2h_bytes);
-      we.name = "end";
-      we.format = "tsn:";
-      we.data = d2h_col(o_end_.p, n, stream_, &st_.d2h_bytes);
-      w.children = {ws, we};
-      const int wi = std::min<int>(std::max<int>(cfg.window_index, 0), (int)cols.size());
-      cols.insert(cols.begin() + wi, w);
-      for (int g = 0; g < n_aggs_; ++g) {
-        OutColumn c;
-        c.name = "agg" + std::to_string(g);
-        c.format = agg_format_[g];
-        c.data = d2h_col(o_agg_[g].p, n, stream_, &st_.d2h_bytes);
-        cols.push_back(c);
-      }
-      OutColumn t;
-      t.name = "_timestamp";
-      t.format = "tsn:";
-      t.data = d2h_col(o_ts_.p, n, stream_, &st_.d2h_bytes);
-      cols.push_back(t);
+      const int wi = std::min<int>(std::max<int>(cfg.window_index, 0), plan_.keyed ? 1 : 0);
+      export_window_batch(out_host, n, stream_, &st_.d2h_bytes, plan_.keyed ? o_key_.p : nullptr, key_format_, o_agg_,
+                          plan_.agg_format, o_start_.p, o_end_.p, wi, o_ts_.p);
       AB_CUDA(cudaStreamSynchronize(stream_));
-      out_host->arrays.emplace_back();
-      out_host->schemas.emplace_back();
-      export_batch(cols, n, &out_host->arrays.back(), &out_host->schemas.back());
     } else {
       ArroyoB200DeviceBatch d{};
       d.n_rows = n;
       std::vector<uint64_t> cols;
-      if (keyed_) cols.push_back((uint64_t)o_key_.p);
+      if (plan_.keyed) cols.push_back((uint64_t)o_key_.p);
       const int wi = std::min<int>(std::max<int>(cfg.window_index, 0), (int)cols.size());
       cols.insert(cols.begin() + wi, (uint64_t)o_end_.p);
       cols.insert(cols.begin() + wi, (uint64_t)o_start_.p);
-      for (int g = 0; g < n_aggs_; ++g) cols.push_back((uint64_t)o_agg_[g].p);
+      for (int g = 0; g < plan_.n_aggs; ++g) cols.push_back((uint64_t)o_agg_[g].p);
       cols.push_back((uint64_t)o_ts_.p);
       int c = 0;
       for (uint64_t v : cols) d.cols[c++] = v;

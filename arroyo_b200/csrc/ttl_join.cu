@@ -127,12 +127,7 @@ __global__ void tj_gather_ts_kernel(const int* __restrict__ il, const int* __res
   for (; i < n; i += stride) dst[i] = max(lts[il[i]], rts[ir[i]]);
 }
 
-struct TSide {
-  int n_cols = 0, ts_col = 0, key_col = 0, n_routing = 0;
-  std::vector<int> payload;
-  std::vector<std::string> formats;
-  std::string key_format;  // the key's format once a batch has shown it
-  std::vector<DevBuf> cols;
+struct TSide : JoinSide {
   DevBuf next, tab;
   int64_t n = 0, cap = 0;
   uint32_t tab_cap = 0;
@@ -162,16 +157,12 @@ class TtlJoinOp final : public OpBase {
   void handle_checkpoint(int64_t, BatchesPriv*) override { flush(); }
   void on_close(int, BatchesPriv*) override { flush(); }
   void flush() override {
-    AB_CUDA(cudaSetDevice(device_));
+    set_device();
     AB_CUDA(cudaStreamSynchronize(stream_));
   }
   void stats(ArroyoB200Stats* out) override { *out = st_; }
 
  private:
-  int device_ = 0;
-  cudaStream_t stream_ = nullptr;
-  bool own_stream_ = false;
-  int num_sms_ = 132;  // set from the device at creation
   TSide side_[2];
   DevBuf cnt_, off_, total_, sums_, pair_new_, pair_old_, out_ts_;
   std::vector<DevBuf> out_cols_;
@@ -188,45 +179,13 @@ TtlJoinOp::TtlJoinOp(const ArroyoB200OpConfig& c) {
   name = "JoinWithExpiration";
   AB_REQUIRE(c.join_type == ARROYO_B200_JOIN_INNER, ARROYO_B200_UNSUPPORTED,
              "JoinWithExpiration: only inner joins of append-only inputs are supported");
-  auto init_side = [&](TSide& s, int n_cols, int ts_col, int key_col, int n_routing) {
-    AB_REQUIRE(n_cols >= 2 && n_cols <= ARROYO_B200_MAX_COLS && ts_col >= 0 && ts_col < n_cols && key_col >= 0 &&
-                   key_col < n_cols && n_routing >= 0 && n_routing < n_cols && key_col >= n_routing && ts_col >= n_routing,
-               ARROYO_B200_INVALID_ARGUMENT, "bad join side columns");
-    s.n_cols = n_cols;
-    s.ts_col = ts_col;
-    s.key_col = key_col;
-    s.n_routing = n_routing;
-    for (int i = n_routing; i < n_cols; ++i)
-      if (i != ts_col) s.payload.push_back(i);
-    s.cols.resize(n_cols);
-    s.formats.assign(n_cols, "l");
-    s.formats[ts_col] = "tsn:";
-  };
-  init_side(side_[0], c.n_cols, c.timestamp_col, c.left_key_col, c.left_n_routing);
-  init_side(side_[1], c.right_n_cols, c.right_timestamp_col, c.right_key_col, c.right_n_routing);
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0)
-    throw Error(ARROYO_B200_FATAL, "no CUDA device available: libarroyo_b200 has no CPU fallback");
-  device_ = c.device;
-  AB_REQUIRE(device_ >= 0 && device_ < count, ARROYO_B200_INVALID_ARGUMENT, "bad device ordinal");
-  AB_CUDA(cudaSetDevice(device_));
-  cudaDeviceProp prop{};
-  AB_CUDA(cudaGetDeviceProperties(&prop, device_));
-  num_sms_ = prop.multiProcessorCount;
-  if (c.stream) {
-    stream_ = (cudaStream_t)c.stream;
-  } else {
-    AB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    own_stream_ = true;
-  }
+  init_join_side(side_[0], c.n_cols, c.timestamp_col, c.left_key_col, c.left_n_routing);
+  init_join_side(side_[1], c.right_n_cols, c.right_timestamp_col, c.right_key_col, c.right_n_routing);
+  open_device(c);
   total_.alloc(16);
 }
 
-TtlJoinOp::~TtlJoinOp() {
-  cudaSetDevice(device_);
-  cudaStreamSynchronize(stream_);
-  if (own_stream_ && stream_) cudaStreamDestroy(stream_);
-}
+TtlJoinOp::~TtlJoinOp() { drain_stream(); }
 
 void TtlJoinOp::reserve(TSide& s, int64_t extra) {
   if (s.n + extra <= s.cap) return;
@@ -264,7 +223,7 @@ void TtlJoinOp::ensure_table(TSide& s, uint64_t more_rows) {
 }
 
 void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* batch, const ArrowSchema* schema, BatchesPriv* out) {
-  AB_CUDA(cudaSetDevice(device_));
+  set_device();
   AB_REQUIRE(parts >= 2 && parts % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
   const int sd = (int)(index / (parts / 2));
   AB_REQUIRE(sd == 0 || sd == 1, ARROYO_B200_INVALID_ARGUMENT, "bad input index");
@@ -353,9 +312,7 @@ void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* b
       OutColumn col;
       col.name = (side == 0 ? "l" : "r") + std::to_string(c);
       col.format = z.formats[c];
-      void* h = PinnedPool::get().alloc((size_t)n_out * 8);
-      AB_CUDA(cudaMemcpyAsync(h, out_cols_[oc].p, (size_t)n_out * 8, cudaMemcpyDeviceToHost, stream_));
-      col.data = h;
+      col.data = d2h_pinned(out_cols_[oc].p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
       ocols.push_back(col);
       ++oc;
     }
@@ -369,11 +326,8 @@ void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* b
   OutColumn t;
   t.name = "_timestamp";
   t.format = "tsn:";
-  void* ht = PinnedPool::get().alloc((size_t)n_out * 8);
-  AB_CUDA(cudaMemcpyAsync(ht, out_ts_.p, (size_t)n_out * 8, cudaMemcpyDeviceToHost, stream_));
-  t.data = ht;
+  t.data = d2h_pinned(out_ts_.p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
   ocols.push_back(t);
-  st_.d2h_bytes += (uint64_t)n_out * 8 * (uint64_t)(n_oc + 1);
   AB_CUDA(cudaStreamSynchronize(stream_));
   st_.rows_out += (uint64_t)n_out;
   ++st_.windows_out;

@@ -25,14 +25,12 @@
 #include <algorithm>
 #include <climits>
 
+#include "agg_plan.h"
 #include "bdict.cuh"
 #include "op.h"
 
 namespace ab {
 namespace {
-
-constexpr int U_MAX_ACC = ARROYO_B200_MAX_AGGS + 1;
-enum : int { U_ROWS = 0, U_SUM = 1, U_SUM_F64 = 2, U_MIN = 3, U_MAX = 4 };
 
 struct UState {
   unsigned long long* cur;   // [n_acc][id_cap]; cur[0] = rows
@@ -44,14 +42,14 @@ struct UState {
   unsigned int* n_touched;
   unsigned long long id_cap;
   int n_acc;
-  int acc_kind[U_MAX_ACC];
-  int acc_val[U_MAX_ACC];
+  int acc_kind[MAX_ACC];
+  int acc_val[MAX_ACC];
 };
 
 struct UIngest {
   const long long* key;
   const long long* ts;
-  const long long* val[4];
+  const long long* val[MAX_VALS];
   long long n;
   int keyed;
   int n_vals;
@@ -60,7 +58,7 @@ struct UIngest {
   // deferred rows: [key, ts, values...] columns with room for every row of the launch, and their count
   long long* d_key;
   long long* d_ts;
-  long long* d_val[4];
+  long long* d_val[MAX_VALS];
   unsigned long long* deferred;
 };
 
@@ -86,15 +84,15 @@ __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__
     }
     atomicAdd(p.st.cur + id, 1ull);
 #pragma unroll
-    for (int a = 1; a < U_MAX_ACC; ++a) {
+    for (int a = 1; a < MAX_ACC; ++a) {
       if (a >= p.st.n_acc) break;
       const long long v = __ldcs(p.val[p.st.acc_val[a]] + i);
       unsigned long long* dst = p.st.cur + (unsigned long long)a * p.st.id_cap + id;
       switch (p.st.acc_kind[a]) {
-        case U_SUM: atomicAdd(dst, (unsigned long long)v); break;
-        case U_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), (double)v); break;
-        case U_MIN: atomicMin(reinterpret_cast<long long*>(dst), v); break;
-        case U_MAX: atomicMax(reinterpret_cast<long long*>(dst), v); break;
+        case ACC_SUM_I64: atomicAdd(dst, (unsigned long long)v); break;
+        case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), (double)v); break;
+        case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(dst), v); break;
+        case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(dst), v); break;
       }
     }
     atomicMax(p.st.cur_ts + id, __ldcs(p.ts + i));
@@ -117,18 +115,12 @@ struct UFlush {
   unsigned int* counts;  // [0] retractions, [1] appends
 };
 
-__device__ __forceinline__ unsigned long long finalise(int kind, unsigned long long acc, unsigned long long rows) {
-  if (kind == ARROYO_B200_AGG_COUNT_STAR) return rows;
-  if (kind == ARROYO_B200_AGG_AVG_I64) return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)acc) / (double)rows);
-  return acc;
-}
-
 __global__ void __launch_bounds__(256) upd_flush_kernel(const __grid_constant__ UFlush p) {
   unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
   const unsigned int stride = gridDim.x * blockDim.x;
   for (; i < p.n; i += stride) {
     const unsigned int id = p.st.list[i];
-    unsigned long long now[U_MAX_ACC], old[U_MAX_ACC];
+    unsigned long long now[MAX_ACC], old[MAX_ACC];
     bool changed = false;
     for (int a = 0; a < p.st.n_acc; ++a) {
       now[a] = p.st.cur[(unsigned long long)a * p.st.id_cap + id];
@@ -138,19 +130,19 @@ __global__ void __launch_bounds__(256) upd_flush_kernel(const __grid_constant__ 
     // "don't bother emitting updates that just retract / append the same values (excluding the timestamp)" (:655-664):
     // compared on the OUTPUT values, like the reference compares ScalarValues
     for (int g = 0; g < p.n_aggs; ++g)
-      changed = changed || finalise(p.agg_kind[g], now[p.agg_acc[g]], now[0]) != finalise(p.agg_kind[g], old[p.agg_acc[g]], old[0]);
+      changed = changed || agg_finalise(p.agg_kind[g], now[p.agg_acc[g]], now[0]) != agg_finalise(p.agg_kind[g], old[p.agg_acc[g]], old[0]);
     const long long now_ts = p.st.cur_ts[id], old_ts = p.st.prev_ts[id];
     const long long key = p.keyed ? p.id_keys[id] : 0;
     if (had && changed) {
       const unsigned int o = atomicAdd(p.counts + 0, 1u);
       if (p.keyed) p.o_key[o] = key;
-      for (int g = 0; g < p.n_aggs; ++g) p.o_agg[g][o] = finalise(p.agg_kind[g], old[p.agg_acc[g]], old[0]);
+      for (int g = 0; g < p.n_aggs; ++g) p.o_agg[g][o] = agg_finalise(p.agg_kind[g], old[p.agg_acc[g]], old[0]);
       p.o_ts[o] = old_ts;
     }
     if (!had || changed) {
       const unsigned int o = p.n + atomicAdd(p.counts + 1, 1u);
       if (p.keyed) p.o_key[o] = key;
-      for (int g = 0; g < p.n_aggs; ++g) p.o_agg[g][o] = finalise(p.agg_kind[g], now[p.agg_acc[g]], now[0]);
+      for (int g = 0; g < p.n_aggs; ++g) p.o_agg[g][o] = agg_finalise(p.agg_kind[g], now[p.agg_acc[g]], now[0]);
       p.o_ts[o] = now_ts;
     }
     for (int a = 0; a < p.st.n_acc; ++a) p.st.prev[(unsigned long long)a * p.st.id_cap + id] = now[a];
@@ -164,9 +156,7 @@ __global__ void upd_init_kernel(UState st, unsigned long long n) {
   const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
   for (; i < n; i += stride) {
     for (int a = 0; a < st.n_acc; ++a) {
-      unsigned long long v = 0;
-      if (st.acc_kind[a] == U_MIN) v = (unsigned long long)LLONG_MAX;
-      if (st.acc_kind[a] == U_MAX) v = (unsigned long long)LLONG_MIN;
+      const unsigned long long v = acc_identity(st.acc_kind[a]);
       st.cur[(unsigned long long)a * st.id_cap + i] = v;
       st.prev[(unsigned long long)a * st.id_cap + i] = a == 0 ? 0 : v;
     }
@@ -214,13 +204,13 @@ class UpdatingAggOp final : public OpBase {
   }
   void handle_tick(BatchesPriv* out) override { flush_to(out); }  // :994-1004
   void flush() override {
-    AB_CUDA(cudaSetDevice(device_));
+    set_device();
     AB_CUDA(cudaStreamSynchronize(stream_));
   }
   void stats(ArroyoB200Stats* out) override {
     st_.n_keys = 0;
-    if (keyed_) {
-      AB_CUDA(cudaSetDevice(device_));
+    if (plan_.keyed) {
+      set_device();
       drain_deferred();  // also reads the dictionary's count (ids from BD_ID_BASE on)
       // id 0 is the INT64_MIN key's: it has rows once that key arrived
       unsigned long long min_key_rows = 0;
@@ -232,17 +222,8 @@ class UpdatingAggOp final : public OpBase {
   }
 
  private:
-  int device_ = 0;
-  cudaStream_t stream_ = nullptr;
-  bool own_stream_ = false;
-  int num_sms_ = 132;  // set from the device at creation
-  bool keyed_ = false;
-  int key_col_ = 0, ts_col_ = 0;
-  int n_vals_ = 0, val_cols_[4];
-  int n_acc_ = 1, acc_kind_[U_MAX_ACC], acc_val_[U_MAX_ACC];
-  int n_aggs_ = 0, agg_kind_[ARROYO_B200_MAX_AGGS], agg_acc_[ARROYO_B200_MAX_AGGS];
+  AggPlan plan_;
   std::string key_format_ = "l";
-  std::vector<std::string> agg_format_;
   // dictionary + state
   uint64_t n_buckets_ = 1, id_cap_ = 0;
   uint32_t total_keys_ = 0;
@@ -251,7 +232,7 @@ class UpdatingAggOp final : public OpBase {
   DevBuf staging_;
   uint64_t staging_cap_ = 0;
   // deferred rows (key, ts, values): two sets, one re-ingested while the other takes the rows that defer again
-  DevBuf defer_[2][2 + 4];
+  DevBuf defer_[2][2 + MAX_VALS];
   uint64_t defer_cap_[2] = {0, 0};
   int defer_cur_ = 0;
   uint64_t out_cap_ = 0;
@@ -272,85 +253,21 @@ class UpdatingAggOp final : public OpBase {
 UpdatingAggOp::UpdatingAggOp(const ArroyoB200OpConfig& c) {
   cfg = c;
   name = "UpdatingAggregatingFunc";
-  AB_REQUIRE(c.n_key_cols == 0 || c.n_key_cols == 1, ARROYO_B200_UNSUPPORTED, "only 0 or 1 group-by key columns are supported");
-  keyed_ = c.n_key_cols == 1;
-  key_col_ = c.key_col;
-  ts_col_ = c.timestamp_col;
-  AB_REQUIRE(c.n_cols >= 1 && c.n_cols <= ARROYO_B200_MAX_COLS && ts_col_ >= 0 && ts_col_ < c.n_cols,
-             ARROYO_B200_INVALID_ARGUMENT, "bad column layout");
-  AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= ARROYO_B200_MAX_AGGS, ARROYO_B200_INVALID_ARGUMENT, "bad n_aggs");
   AB_REQUIRE(!(c.flags & ARROYO_B200_FLAG_UPDATING_INPUT), ARROYO_B200_UNSUPPORTED,
              "updating aggregate over an updating input (retractions) is not supported");
-  n_aggs_ = c.n_aggs;
-  acc_kind_[0] = U_ROWS;
-  acc_val_[0] = 0;
-  for (int g = 0; g < n_aggs_; ++g) {
-    const int kind = c.aggs[g].kind;
-    agg_kind_[g] = kind;
-    agg_acc_[g] = 0;
-    if (kind == ARROYO_B200_AGG_COUNT_STAR) {
-      agg_format_.push_back("l");
-      continue;
-    }
-    const int col = c.aggs[g].input_col;
-    AB_REQUIRE(col >= 0 && col < c.n_cols, ARROYO_B200_INVALID_ARGUMENT, "aggregate input column out of range");
-    int vs = -1;
-    for (int v = 0; v < n_vals_; ++v)
-      if (val_cols_[v] == col) vs = v;
-    if (vs < 0) {
-      AB_REQUIRE(n_vals_ < 4, ARROYO_B200_UNSUPPORTED, "more than 4 distinct aggregate input columns");
-      vs = n_vals_;
-      val_cols_[n_vals_++] = col;
-    }
-    int ak;
-    switch (kind) {
-      case ARROYO_B200_AGG_SUM_I64: ak = U_SUM; agg_format_.push_back("l"); break;
-      // AVG sums the inputs as f64, like the reference's accumulator (each value cast to f64, then added): an
-      // integer sum would wrap and average to garbage once the values pass 2^63 in total
-      case ARROYO_B200_AGG_AVG_I64: ak = U_SUM_F64; agg_format_.push_back("g"); break;
-      case ARROYO_B200_AGG_MIN_I64: ak = U_MIN; agg_format_.push_back("l"); break;
-      case ARROYO_B200_AGG_MAX_I64: ak = U_MAX; agg_format_.push_back("l"); break;
-      default: throw Error(ARROYO_B200_UNSUPPORTED, "unsupported aggregate kind");
-    }
-    int found = -1;
-    for (int a = 1; a < n_acc_; ++a)
-      if (acc_kind_[a] == ak && acc_val_[a] == vs) found = a;
-    if (found < 0) {
-      found = n_acc_;
-      acc_kind_[n_acc_] = ak;
-      acc_val_[n_acc_] = vs;
-      ++n_acc_;
-    }
-    agg_acc_[g] = found;
-  }
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0)
-    throw Error(ARROYO_B200_FATAL, "no CUDA device available: libarroyo_b200 has no CPU fallback");
-  device_ = c.device;
-  AB_REQUIRE(device_ >= 0 && device_ < count, ARROYO_B200_INVALID_ARGUMENT, "bad device ordinal");
-  AB_CUDA(cudaSetDevice(device_));
-  cudaDeviceProp prop{};
-  AB_CUDA(cudaGetDeviceProperties(&prop, device_));
-  num_sms_ = prop.multiProcessorCount;
-  if (c.stream) {
-    stream_ = (cudaStream_t)c.stream;
-  } else {
-    AB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    own_stream_ = true;
-  }
+  // AVG sums the inputs as f64, like the reference's accumulator (each value cast to f64, then added): an integer
+  // sum would wrap and average to garbage once the values pass 2^63 in total
+  plan_ = AggPlan(c, ACC_SUM_F64);
+  open_device(c);
   counters_.alloc(32);
   AB_CUDA(cudaMemsetAsync(counters_.p, 0, 32, stream_));
   n_total_.alloc(4);
   AB_CUDA(cudaMemsetAsync(n_total_.p, 0, 4, stream_));
-  alloc_state(keyed_ ? bd_buckets_for(c.expected_keys ? c.expected_keys : (1ull << 16)) : 1);
+  alloc_state(plan_.keyed ? bd_buckets_for(c.expected_keys ? c.expected_keys : (1ull << 16)) : 1);
   AB_CUDA(cudaStreamSynchronize(stream_));
 }
 
-UpdatingAggOp::~UpdatingAggOp() {
-  cudaSetDevice(device_);
-  cudaStreamSynchronize(stream_);
-  if (own_stream_ && stream_) cudaStreamDestroy(stream_);
-}
+UpdatingAggOp::~UpdatingAggOp() { drain_stream(); }
 
 BDict UpdatingAggOp::dict_view() const {
   BDict d{};
@@ -372,10 +289,10 @@ UState UpdatingAggOp::state_view() const {
   s.list = list_.as<unsigned int>();
   s.n_touched = counters_.as<unsigned int>();
   s.id_cap = id_cap_;
-  s.n_acc = n_acc_;
-  for (int a = 0; a < n_acc_; ++a) {
-    s.acc_kind[a] = acc_kind_[a];
-    s.acc_val[a] = acc_val_[a];
+  s.n_acc = plan_.n_acc;
+  for (int a = 0; a < plan_.n_acc; ++a) {
+    s.acc_kind[a] = plan_.acc_kind[a];
+    s.acc_val[a] = plan_.acc_val[a];
   }
   return s;
 }
@@ -389,13 +306,13 @@ void UpdatingAggOp::alloc_state(uint64_t n_buckets) {
   AB_CUDA(cudaGetLastError());
   bucket_nkeys_.alloc(n_buckets_ * 4);
   AB_CUDA(cudaMemsetAsync(bucket_nkeys_.p, 0, n_buckets_ * 4, stream_));
-  if (keyed_) {
+  if (plan_.keyed) {
     slots_.alloc(n_buckets_ * BD_KS * sizeof(BSlot));
     bd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(slots_.as<BSlot>(), n_buckets_ * BD_KS);
     AB_CUDA(cudaGetLastError());
   }
-  cur_.alloc((size_t)n_acc_ * id_cap_ * 8);
-  prev_.alloc((size_t)n_acc_ * id_cap_ * 8);
+  cur_.alloc((size_t)plan_.n_acc * id_cap_ * 8);
+  prev_.alloc((size_t)plan_.n_acc * id_cap_ * 8);
   cur_ts_.alloc(id_cap_ * 8);
   prev_ts_.alloc(id_cap_ * 8);
   touched_.alloc(id_cap_ * 4);
@@ -441,7 +358,7 @@ void UpdatingAggOp::grow() {
 void UpdatingAggOp::reserve_defer(int set, uint64_t rows) {
   if (rows <= defer_cap_[set]) return;
   defer_cap_[set] = std::max<uint64_t>(rows, defer_cap_[set] * 2);
-  for (int c = 0; c < 2 + n_vals_; ++c) defer_[set][c].alloc(defer_cap_[set] * 8);
+  for (int c = 0; c < 2 + plan_.n_vals; ++c) defer_[set][c].alloc(defer_cap_[set] * 8);
 }
 
 // Re-ingests the rows the last launch deferred (their bucket was out of ids), doubling the bucket count before each
@@ -469,8 +386,8 @@ void UpdatingAggOp::drain_deferred() {
       const int full = defer_cur_;
       defer_cur_ ^= 1;
       AB_CUDA(cudaMemsetAsync(d_count, 0, 8, stream_));
-      const long long* vals[4] = {nullptr, nullptr, nullptr, nullptr};
-      for (int v = 0; v < n_vals_; ++v) vals[v] = defer_[full][2 + v].as<long long>();
+      const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
+      for (int v = 0; v < plan_.n_vals; ++v) vals[v] = defer_[full][2 + v].as<long long>();
       ingest(defer_[full][0].as<long long>(), defer_[full][1].as<long long>(), vals, (int64_t)n);
     }
   } catch (...) {
@@ -482,7 +399,7 @@ void UpdatingAggOp::drain_deferred() {
 
 // every row of the batch may bring a new key: keep the mean bucket fill at or under the target
 void UpdatingAggOp::ensure_room(uint64_t new_rows) {
-  if (!keyed_) return;
+  if (!plan_.keyed) return;
   drain_deferred();
   while ((uint64_t)total_keys_ + new_rows > n_buckets_ * (uint64_t)BD_MEAN) grow();
 }
@@ -492,17 +409,17 @@ void UpdatingAggOp::ingest(const long long* key, const long long* ts, const long
   UIngest p{};
   p.key = key;
   p.ts = ts;
-  for (int v = 0; v < n_vals_; ++v) p.val[v] = vals[v];
+  for (int v = 0; v < plan_.n_vals; ++v) p.val[v] = vals[v];
   p.n = n;
-  p.keyed = keyed_ ? 1 : 0;
-  p.n_vals = n_vals_;
+  p.keyed = plan_.keyed ? 1 : 0;
+  p.n_vals = plan_.n_vals;
   p.dict = dict_view();
   p.st = state_view();
-  if (keyed_) {  // every row of the launch may defer (all rows of a key whose bucket is full do)
+  if (plan_.keyed) {  // every row of the launch may defer (all rows of a key whose bucket is full do)
     reserve_defer(defer_cur_, (uint64_t)n);
     p.d_key = defer_[defer_cur_][0].as<long long>();
     p.d_ts = defer_[defer_cur_][1].as<long long>();
-    for (int v = 0; v < n_vals_; ++v) p.d_val[v] = defer_[defer_cur_][2 + v].as<long long>();
+    for (int v = 0; v < plan_.n_vals; ++v) p.d_val[v] = defer_[defer_cur_][2 + v].as<long long>();
   }
   p.deferred = reinterpret_cast<unsigned long long*>((char*)counters_.p + 16);
   const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms_ * 8);
@@ -513,34 +430,34 @@ void UpdatingAggOp::ingest(const long long* key, const long long* ts, const long
 }
 
 void UpdatingAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const ArrowSchema* schema) {
-  AB_CUDA(cudaSetDevice(device_));
+  set_device();
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
-  require_aggregate_input_types(cols, keyed_ ? key_col_ : -1, val_cols_, n_vals_);
-  if (keyed_) key_format_ = cols[key_col_].format;
+  require_aggregate_input_types(cols, plan_.keyed ? plan_.key_col : -1, plan_.val_cols, plan_.n_vals);
+  if (plan_.keyed) key_format_ = cols[plan_.key_col].format;
   st_.rows_in += (uint64_t)n;
   if (n == 0) {
     if (batch->release) batch->release(batch);
     return;
   }
   ensure_room((uint64_t)n);
-  const int n_used = 2 + n_vals_;
+  const int n_used = 2 + plan_.n_vals;
   if ((uint64_t)n > staging_cap_) {
     AB_CUDA(cudaStreamSynchronize(stream_));
     staging_cap_ = std::max<uint64_t>((uint64_t)n, staging_cap_ * 2);
     staging_.alloc((size_t)n_used * staging_cap_ * 8);
   }
   long long* base = staging_.as<long long>();
-  const long long* vals[4] = {nullptr, nullptr, nullptr, nullptr};
-  if (keyed_) AB_CUDA(cudaMemcpyAsync(base, cols[key_col_].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  AB_CUDA(cudaMemcpyAsync(base + staging_cap_, cols[ts_col_].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  for (int v = 0; v < n_vals_; ++v) {
-    AB_CUDA(cudaMemcpyAsync(base + (size_t)(2 + v) * staging_cap_, cols[val_cols_[v]].data, (size_t)n * 8, cudaMemcpyHostToDevice,
+  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
+  if (plan_.keyed) AB_CUDA(cudaMemcpyAsync(base, cols[plan_.key_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
+  AB_CUDA(cudaMemcpyAsync(base + staging_cap_, cols[plan_.ts_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
+  for (int v = 0; v < plan_.n_vals; ++v) {
+    AB_CUDA(cudaMemcpyAsync(base + (size_t)(2 + v) * staging_cap_, cols[plan_.val_cols[v]].data, (size_t)n * 8, cudaMemcpyHostToDevice,
                             stream_));
     vals[v] = base + (size_t)(2 + v) * staging_cap_;
   }
-  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((keyed_ ? 1 : 0) + 1 + n_vals_);
+  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((plan_.keyed ? 1 : 0) + 1 + plan_.n_vals);
   ingest(base, base + staging_cap_, vals, n);
   // the staging buffer is reused by the next batch: the copies and the kernel must have consumed the host batch
   AB_CUDA(cudaStreamSynchronize(stream_));
@@ -549,14 +466,14 @@ void UpdatingAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const A
 }
 
 void UpdatingAggOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols, int32_t n_cols, int64_t n_rows) {
-  AB_CUDA(cudaSetDevice(device_));
+  set_device();
   AB_REQUIRE(n_cols == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
   if (n_rows <= 0) return;
   st_.rows_in += (uint64_t)n_rows;
   ensure_room((uint64_t)n_rows);
-  const long long* vals[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (int v = 0; v < n_vals_; ++v) vals[v] = (const long long*)cols[val_cols_[v]];
-  ingest(keyed_ ? (const long long*)cols[key_col_] : nullptr, (const long long*)cols[ts_col_], vals, n_rows);
+  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
+  for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)cols[plan_.val_cols[v]];
+  ingest(plan_.keyed ? (const long long*)cols[plan_.key_col] : nullptr, (const long long*)cols[plan_.ts_col], vals, n_rows);
 }
 
 static void* d2h_part(const void* dev, size_t off_rows, int64_t n, void* host, size_t host_off_rows, cudaStream_t s) {
@@ -567,8 +484,8 @@ static void* d2h_part(const void* dev, size_t off_rows, int64_t n, void* host, s
 
 // flush (:637-738): one batch [key?, aggregates..., _timestamp, is_retract], or nothing when no key changed
 void UpdatingAggOp::flush_to(BatchesPriv* out) {
-  AB_CUDA(cudaSetDevice(device_));
-  if (keyed_) drain_deferred();
+  set_device();
+  if (plan_.keyed) drain_deferred();
   struct {
     unsigned int touched, retracts, appends, pad;
   } h{};
@@ -580,17 +497,17 @@ void UpdatingAggOp::flush_to(BatchesPriv* out) {
     out_cap_ = std::max<uint64_t>(2ull * n, 1024);
     o_key_.alloc(out_cap_ * 8);
     o_ts_.alloc(out_cap_ * 8);
-    for (int g = 0; g < n_aggs_; ++g) o_agg_[g].alloc(out_cap_ * 8);
+    for (int g = 0; g < plan_.n_aggs; ++g) o_agg_[g].alloc(out_cap_ * 8);
   }
   UFlush p{};
   p.st = state_view();
   p.id_keys = id_keys_.as<long long>();
   p.n = n;
-  p.keyed = keyed_ ? 1 : 0;
-  p.n_aggs = n_aggs_;
-  for (int g = 0; g < n_aggs_; ++g) {
-    p.agg_kind[g] = agg_kind_[g];
-    p.agg_acc[g] = agg_acc_[g];
+  p.keyed = plan_.keyed ? 1 : 0;
+  p.n_aggs = plan_.n_aggs;
+  for (int g = 0; g < plan_.n_aggs; ++g) {
+    p.agg_kind[g] = plan_.agg_kind[g];
+    p.agg_acc[g] = plan_.agg_acc[g];
     p.o_agg[g] = o_agg_[g].as<unsigned long long>();
   }
   p.o_key = o_key_.as<long long>();
@@ -618,8 +535,8 @@ void UpdatingAggOp::flush_to(BatchesPriv* out) {
     c.data = host;
     cols.push_back(c);
   };
-  if (keyed_) column("key", key_format_, o_key_.p);
-  for (int g = 0; g < n_aggs_; ++g) column(("agg" + std::to_string(g)).c_str(), agg_format_[g], o_agg_[g].p);
+  if (plan_.keyed) column("key", key_format_, o_key_.p);
+  for (int g = 0; g < plan_.n_aggs; ++g) column(("agg" + std::to_string(g)).c_str(), plan_.agg_format[g], o_agg_[g].p);
   column("_timestamp", "tsn:", o_ts_.p);
   {
     OutColumn r;

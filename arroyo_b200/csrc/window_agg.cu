@@ -33,6 +33,7 @@
 #include <memory>
 #include <set>
 
+#include "agg_plan.h"
 #include "bdict.cuh"
 #include "op.h"
 #include "planner.h"
@@ -40,8 +41,6 @@
 namespace ab {
 namespace {
 
-constexpr int MAX_VALS = 4;
-constexpr int MAX_ACC = ARROYO_B200_MAX_AGGS + 1;
 constexpr int MAX_SEGS = 512;
 constexpr int MAX_RING = 4096;
 constexpr int RING_INLINE = 64;
@@ -51,8 +50,6 @@ constexpr long long FREE_BIN = LLONG_MIN;
 constexpr int THREADS = 256;
 constexpr int PAIRS = 2;
 constexpr int TILE = THREADS * PAIRS * 2;  // rows per tile
-
-enum AccKind : int { ACC_ROWS = 0, ACC_SUM_I64 = 1, ACC_SUM_F64 = 2, ACC_MIN_I64 = 3, ACC_MAX_I64 = 4 };
 
 struct Counters {
   unsigned long long late_rows;
@@ -125,12 +122,7 @@ __global__ void pane_init_kernel(const __grid_constant__ InitParams p) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (; i < p.n; i += stride) {
-    for (int a = 0; a < p.n_acc; ++a) {
-      unsigned long long v = 0;
-      if (p.acc_kind[a] == ACC_MIN_I64) v = (unsigned long long)LLONG_MAX;
-      if (p.acc_kind[a] == ACC_MAX_I64) v = (unsigned long long)LLONG_MIN;
-      p.pane[a * p.id_cap + i] = v;
-    }
+    for (int a = 0; a < p.n_acc; ++a) p.pane[a * p.id_cap + i] = acc_identity(p.acc_kind[a]);
   }
 }
 
@@ -720,9 +712,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) emit_kernel(const __grid_constan
 #pragma unroll
         for (int a = 0; a < NACC; ++a)
           {
-            unsigned long long ident = 0;
-            if (p.acc_kind[a] == ACC_MIN_I64) ident = (unsigned long long)LLONG_MAX;
-            if (p.acc_kind[a] == ACC_MAX_I64) ident = (unsigned long long)LLONG_MIN;
+            const unsigned long long ident = acc_identity(p.acc_kind[a]);
             acc0[a] = ident;
             acc1[a] = ident;
           }
@@ -857,16 +847,7 @@ class WindowAggOp final : public OpBase {
   // config-derived
   bool sliding_;
   int64_t width_, slide_;  // slide_ == width_ for tumbling
-  bool keyed_;
-  int key_col_, ts_col_;
-  int n_vals_ = 0;
-  int val_cols_[MAX_VALS];
-  int n_acc_ = 1;
-  int acc_kind_[MAX_ACC];
-  int acc_val_[MAX_ACC];
-  int n_aggs_;
-  int agg_kind_[ARROYO_B200_MAX_AGGS];
-  int agg_acc_[ARROYO_B200_MAX_AGGS];
+  AggPlan plan_;
   bool invertible_ = true;
   // AVG(Int64) from the exact integer sum instead of a separate f64 RED per row (one scattered access
   // less per row).  Valid while no per-key sum can overflow i64: every guarded value is < 2^31 in
@@ -879,12 +860,6 @@ class WindowAggOp final : public OpBase {
   bool running_mode_ = false;
   bool profile_;
   std::string key_format_ = "l";
-  std::vector<std::string> agg_format_;
-
-  int device_;
-  cudaStream_t stream_ = nullptr;
-  bool own_stream_ = false;
-  int num_sms_ = 132;  // set from the device at creation
 
   // dictionary (bdict.cuh): n_buckets_ buckets of BD_KS slots; ids = BD_ID_BASE + bucket * BD_CAPB + index
   uint64_t id_cap_ = 0;
@@ -1016,7 +991,6 @@ class WindowAggOp final : public OpBase {
   size_t emit_events_used_ = 0;
 
   // helpers
-  void set_device() { AB_CUDA(cudaSetDevice(device_)); }
   void alloc_dictionary(uint64_t n_buckets);
   void preallocate();
   void grow_ids();
@@ -1060,89 +1034,24 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
   if (sliding_)
     AB_REQUIRE(width_ % slide_ == 0, ARROYO_B200_INVALID_ARGUMENT,
                "hop width must be a multiple of the slide (arroyo-planner/src/lib.rs:640-655)");
-  AB_REQUIRE(c.n_key_cols == 0 || c.n_key_cols == 1, ARROYO_B200_UNSUPPORTED,
-             "only 0 or 1 group-by key columns are supported");
-  keyed_ = c.n_key_cols == 1;
-  key_col_ = c.key_col;
-  ts_col_ = c.timestamp_col;
-  AB_REQUIRE(c.n_cols >= 1 && c.n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad n_cols");
-  AB_REQUIRE(ts_col_ >= 0 && ts_col_ < c.n_cols, ARROYO_B200_INVALID_ARGUMENT, "bad timestamp_col");
-  AB_REQUIRE(!keyed_ || (key_col_ >= 0 && key_col_ < c.n_cols), ARROYO_B200_INVALID_ARGUMENT, "bad key_col");
-  AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= ARROYO_B200_MAX_AGGS, ARROYO_B200_INVALID_ARGUMENT, "bad n_aggs");
-  n_aggs_ = c.n_aggs;
-  avg_exact_ = !(c.flags & ARROYO_B200_FLAG_AVG_F64);
-  acc_kind_[0] = ACC_ROWS;
-  acc_val_[0] = 0;
-  // Exact-sum AVG shares the integer sum of its column, and promote_avg later adds one f64 accumulator per AVG
-  // column.  A plan without room for those starts in f64 AVG mode (as with FLAG_AVG_F64), where every aggregate
-  // takes at most one accumulator: every accepted plan fits MAX_ACC and no promotion can fail mid-stream.
-  if (avg_exact_) {
-    std::set<std::pair<int, int>> exact_accs;  // (kind, column), AVG counted as SUM
-    std::set<int> avg_cols;
-    for (int g = 0; g < n_aggs_; ++g) {
-      const int kind = c.aggs[g].kind;
-      if (kind == ARROYO_B200_AGG_COUNT_STAR) continue;
-      exact_accs.emplace(kind == ARROYO_B200_AGG_AVG_I64 ? ARROYO_B200_AGG_SUM_I64 : kind, c.aggs[g].input_col);
-      if (kind == ARROYO_B200_AGG_AVG_I64) avg_cols.insert(c.aggs[g].input_col);
-    }
-    avg_exact_ = 1 + exact_accs.size() + avg_cols.size() <= (size_t)MAX_ACC;
-  }
-  for (int g = 0; g < n_aggs_; ++g) {
-    int kind = c.aggs[g].kind;
-    agg_kind_[g] = kind;
-    agg_acc_[g] = 0;
-    if (kind == ARROYO_B200_AGG_COUNT_STAR) {
-      agg_format_.push_back("l");
-      continue;
-    }
-    int col = c.aggs[g].input_col;
-    AB_REQUIRE(col >= 0 && col < c.n_cols, ARROYO_B200_INVALID_ARGUMENT, "aggregate input column out of range");
-    int vs = -1;
-    for (int v = 0; v < n_vals_; ++v)
-      if (val_cols_[v] == col) vs = v;
-    if (vs < 0) {
-      AB_REQUIRE(n_vals_ < MAX_VALS, ARROYO_B200_UNSUPPORTED, "more than 4 distinct aggregate input columns");
-      vs = n_vals_;
-      val_cols_[n_vals_++] = col;
-    }
-    int ak;
-    switch (kind) {
-      case ARROYO_B200_AGG_SUM_I64: ak = ACC_SUM_I64; agg_format_.push_back("l"); break;
-      case ARROYO_B200_AGG_AVG_I64:
-        // exact mode: AVG shares the wrapping integer sum and is finalised as (double)sum / count
-        ak = avg_exact_ ? ACC_SUM_I64 : ACC_SUM_F64;
-        if (avg_exact_) guard_vals_ |= 1u << vs;
-        agg_format_.push_back("g");
-        break;
-      case ARROYO_B200_AGG_MIN_I64: ak = ACC_MIN_I64; agg_format_.push_back("l"); invertible_ = false; break;
-      case ARROYO_B200_AGG_MAX_I64: ak = ACC_MAX_I64; agg_format_.push_back("l"); invertible_ = false; break;
-      default:
-        throw Error(ARROYO_B200_UNSUPPORTED, "unsupported aggregate kind");
-    }
-    // share accumulators between identical (kind, column) pairs
-    int found = -1;
-    for (int a = 1; a < n_acc_; ++a)
-      if (acc_kind_[a] == ak && acc_val_[a] == vs) found = a;
-    if (found < 0) {
-      found = n_acc_;
-      acc_kind_[n_acc_] = ak;
-      acc_val_[n_acc_] = vs;
-      ++n_acc_;
-    }
-    agg_acc_[g] = found;
-  }
+  // Exact-sum AVG shares the integer sum of its column (and is finalised as (double)sum / count), and promote_avg
+  // later adds one f64 accumulator per AVG column.  A plan without room for those starts in f64 AVG mode (as with
+  // FLAG_AVG_F64), where every aggregate takes at most one accumulator: every accepted plan fits MAX_ACC and no
+  // promotion can fail mid-stream.
+  plan_ = AggPlan(c, ACC_SUM_I64);
+  std::set<int> avg_slots;
+  for (int g = 0; g < plan_.n_aggs; ++g)
+    if (plan_.agg_kind[g] == ARROYO_B200_AGG_AVG_I64) avg_slots.insert(plan_.acc_val[plan_.agg_acc[g]]);
+  avg_exact_ = !(c.flags & ARROYO_B200_FLAG_AVG_F64) && plan_.n_acc + avg_slots.size() <= (size_t)MAX_ACC;
+  if (!avg_exact_) plan_ = AggPlan(c, ACC_SUM_F64);
+  if (avg_exact_)
+    for (int v : avg_slots) guard_vals_ |= 1u << v;
+  for (int g = 0; g < plan_.n_aggs; ++g)
+    if (plan_.agg_kind[g] == ARROYO_B200_AGG_MIN_I64 || plan_.agg_kind[g] == ARROYO_B200_AGG_MAX_I64) invertible_ = false;
   if (c.partial_count_col_plus1 > 0) {
     const int col = c.partial_count_col_plus1 - 1;
     AB_REQUIRE(col < c.n_cols, ARROYO_B200_INVALID_ARGUMENT, "partial count column out of range");
-    int vs = -1;
-    for (int v = 0; v < n_vals_; ++v)
-      if (val_cols_[v] == col) vs = v;
-    if (vs < 0) {
-      AB_REQUIRE(n_vals_ < MAX_VALS, ARROYO_B200_UNSUPPORTED, "more than 4 distinct aggregate input columns");
-      vs = n_vals_;
-      val_cols_[n_vals_++] = col;
-    }
-    rows_slot_ = vs;
+    rows_slot_ = plan_.value_slot(col);
     // partial sums are not bounded by 2^31: exactness of the integer AVG path rests on the upstream
     // (raw-row) stage's guard and on the window row bound checked at emission
     guard_vals_ = 0;
@@ -1153,25 +1062,10 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
   // have left the window (measured: 1e-5 relative after a 2^61 value passed through), so those
   // configurations re-merge the panes of each window like the reference does.
   bool has_f64 = false;
-  for (int a = 1; a < n_acc_; ++a) has_f64 = has_f64 || acc_kind_[a] == ACC_SUM_F64;
+  for (int a = 1; a < plan_.n_acc; ++a) has_f64 = has_f64 || plan_.acc_kind[a] == ACC_SUM_F64;
   running_mode_ = sliding_ && invertible_ && !has_f64 && !(c.flags & ARROYO_B200_FLAG_REMERGE_ONLY) && width_ > slide_;
 
-  int count = 0;
-  cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count <= 0)
-    throw Error(ARROYO_B200_FATAL, "no CUDA device available: libarroyo_b200 has no CPU fallback");
-  device_ = c.device;
-  AB_REQUIRE(device_ >= 0 && device_ < count, ARROYO_B200_INVALID_ARGUMENT, "bad device ordinal");
-  set_device();
-  cudaDeviceProp prop{};
-  AB_CUDA(cudaGetDeviceProperties(&prop, device_));
-  num_sms_ = prop.multiProcessorCount;
-  if (c.stream) {
-    stream_ = (cudaStream_t)c.stream;
-  } else {
-    AB_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-    own_stream_ = true;
-  }
+  open_device(c);
 
   if (sliding_) sliding_planner_.reset(new SlidingPlanner(width_, slide_));
   else tumbling_.reset(new TumblingPlanner(width_));
@@ -1187,7 +1081,7 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
 
   // one bucket per ~BD_MEAN expected keys (the bucket count doubles when a bucket runs out of ids)
   uint64_t want = c.expected_keys ? c.expected_keys : (1ull << 16);
-  alloc_dictionary(keyed_ ? bd_buckets_for(want) : 1);
+  alloc_dictionary(plan_.keyed ? bd_buckets_for(want) : 1);
   {
     const char* e = getenv("ARROYO_B200_NO_TWO_PASS");
     two_pass_enabled_ = !(e && atoi(e) != 0) && !(c.flags & ARROYO_B200_FLAG_NO_TWO_PASS);
@@ -1202,7 +1096,7 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
     while (ring_ < need && ring_ < MAX_RING) ring_ <<= 1;
   }
 
-  const int n_used = 2 + n_vals_;
+  const int n_used = 2 + plan_.n_vals;
   for (int i = 0; i < NCHUNK; ++i) {
     AB_CUDA(cudaEventCreateWithFlags(&chunk_free_[i], cudaEventDisableTiming));
     if (i == 0) {
@@ -1240,7 +1134,7 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
 // cudaMalloc inside process_batch / handle_watermark serialises the device and showed up as milliseconds per
 // step in short runs (the driver's 5-warm-up / 20-step scaling runs timed little else).
 void WindowAggOp::preallocate() {
-  const size_t block_bytes = (size_t)n_acc_ * id_cap_ * sizeof(unsigned long long);
+  const size_t block_bytes = (size_t)plan_.n_acc * id_cap_ * sizeof(unsigned long long);
   size_t want = (sliding_ ? (size_t)(width_ / slide_) : 1) + 4 + (running_mode_ ? 1 : 0);
   const size_t budget = (size_t)4 << 30;
   want = std::min<size_t>(std::min<size_t>(want, 64), std::max<size_t>(budget / std::max<size_t>(block_bytes, 1), 4));
@@ -1250,7 +1144,7 @@ void WindowAggOp::preallocate() {
     init_block(blk, id_cap_);
     free_panes_.emplace_back(blk, 0);  // already holds the identity: nothing to reset when it is acquired
   }
-  for (int c = 0; c < 2 + n_vals_; ++c) defer_[0][c].alloc(defer_cap_ * 8);
+  for (int c = 0; c < 2 + plan_.n_vals; ++c) defer_[0][c].alloc(defer_cap_ * 8);
   out_set(0, id_cap_);
   out_set(1, id_cap_);
 }
@@ -1294,7 +1188,6 @@ WindowAggOp::~WindowAggOp() {
     cudaEventDestroy(emit_done_);
     cudaEventDestroy(out_done_);
   }
-  if (own_stream_ && stream_) cudaStreamDestroy(stream_);
 }
 
 void WindowAggOp::alloc_dictionary(uint64_t n_buckets) {
@@ -1307,7 +1200,7 @@ void WindowAggOp::alloc_dictionary(uint64_t n_buckets) {
   AB_CUDA(cudaGetLastError());
   bucket_nkeys_.alloc(n_buckets_ * sizeof(unsigned int));
   AB_CUDA(cudaMemsetAsync(bucket_nkeys_.p, 0, n_buckets_ * sizeof(unsigned int), stream_));
-  if (keyed_) {
+  if (plan_.keyed) {
     slots_.alloc(n_buckets_ * BD_KS * sizeof(BSlot));
     bd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(slots_.as<BSlot>(), n_buckets_ * BD_KS);
     AB_CUDA(cudaGetLastError());
@@ -1353,8 +1246,8 @@ void WindowAggOp::init_block(unsigned long long* blk, uint64_t n_ids) {
   ip.pane = blk;
   ip.id_cap = id_cap_;
   ip.n = n_ids;
-  ip.n_acc = n_acc_;
-  for (int a = 0; a < n_acc_; ++a) ip.acc_kind[a] = acc_kind_[a];
+  ip.n_acc = plan_.n_acc;
+  for (int a = 0; a < plan_.n_acc; ++a) ip.acc_kind[a] = plan_.acc_kind[a];
   int blocks = (int)std::min<uint64_t>((n_ids + 255) / 256, (uint64_t)num_sms_ * 8);
   pane_init_kernel<<<blocks, 256, 0, stream_>>>(ip);
   AB_CUDA(cudaGetLastError());
@@ -1368,7 +1261,7 @@ unsigned long long* WindowAggOp::acquire_block() {
     init_block(pr.first, pr.second);
     return pr.first;
   }
-  pane_storage_.emplace_back((size_t)n_acc_ * id_cap_ * sizeof(unsigned long long));
+  pane_storage_.emplace_back((size_t)plan_.n_acc * id_cap_ * sizeof(unsigned long long));
   auto* blk = pane_storage_.back().as<unsigned long long>();
   init_block(blk, id_cap_);
   return blk;
@@ -1395,7 +1288,7 @@ __global__ void permute_block_kernel(const unsigned long long* __restrict__ old_
 // Doubles the bucket count: every key is re-inserted into the new dictionary (its id changes), and every live pane
 // block is permuted with the old -> new id map.
 void WindowAggOp::grow_ids() {
-  AB_REQUIRE(keyed_, ARROYO_B200_RUNTIME, "grow_ids on an unkeyed aggregate");
+  AB_REQUIRE(plan_.keyed, ARROYO_B200_RUNTIME, "grow_ids on an unkeyed aggregate");
   const uint64_t old_cap = id_cap_;
   const uint32_t old_ids = n_keys_host_;
   BDict old_d = dict_view();
@@ -1417,12 +1310,12 @@ void WindowAggOp::grow_ids() {
   std::vector<DevBuf> new_storage;
   auto migrate = [&](unsigned long long* old_blk) -> unsigned long long* {
     if (!old_blk) return nullptr;
-    new_storage.emplace_back((size_t)n_acc_ * new_cap * sizeof(unsigned long long));
+    new_storage.emplace_back((size_t)plan_.n_acc * new_cap * sizeof(unsigned long long));
     auto* nb = new_storage.back().as<unsigned long long>();
     init_block(nb, new_cap);
     const int grid = (int)std::min<uint64_t>((old_ids + 255) / 256, (uint64_t)num_sms_ * 8);
     permute_block_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_blk, nb, map.as<uint32_t>(), old_ids, old_cap, new_cap,
-                                                               n_acc_);
+                                                               plan_.n_acc);
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
     return nb;
@@ -1455,14 +1348,14 @@ __global__ void i64_to_f64_kernel(const unsigned long long* __restrict__ src, un
   for (; i < n; i += stride) dst[i] = (unsigned long long)__double_as_longlong((double)(long long)src[i]);
 }
 
-// Re-creates every live block with the current n_acc_; accumulators [0, old_n_acc) are copied, and each
+// Re-creates every live block with the current plan_.n_acc; accumulators [0, old_n_acc) are copied, and each
 // (new index, source index) pair in f64_from is filled with the f64 image of the source integer sum.
 void WindowAggOp::relayout_blocks(int old_n_acc, const std::vector<std::pair<int, int>>& f64_from) {
   std::vector<DevBuf> new_storage;
   const uint32_t n_valid = (uint32_t)std::min<uint64_t>(n_keys_host_, id_cap_);
   auto migrate = [&](unsigned long long* old_blk) -> unsigned long long* {
     if (!old_blk) return nullptr;
-    new_storage.emplace_back((size_t)n_acc_ * id_cap_ * sizeof(unsigned long long));
+    new_storage.emplace_back((size_t)plan_.n_acc * id_cap_ * sizeof(unsigned long long));
     auto* nb = new_storage.back().as<unsigned long long>();
     init_block(nb, id_cap_);
     for (int a = 0; a < old_n_acc; ++a)
@@ -1496,27 +1389,27 @@ void WindowAggOp::relayout_blocks(int old_n_acc, const std::vector<std::pair<int
 void WindowAggOp::promote_avg() {
   if (!avg_exact_) return;
   AB_REQUIRE(in_flight_.empty(), ARROYO_B200_RUNTIME, "promote with launches in flight");
-  const int old_n_acc = n_acc_;
+  const int old_n_acc = plan_.n_acc;
   // the constructor leaves room for these; checked before any state changes so a failure leaves the operator whole
   std::set<int> avg_srcs;
-  for (int g = 0; g < n_aggs_; ++g)
-    if (agg_kind_[g] == ARROYO_B200_AGG_AVG_I64) avg_srcs.insert(agg_acc_[g]);
+  for (int g = 0; g < plan_.n_aggs; ++g)
+    if (plan_.agg_kind[g] == ARROYO_B200_AGG_AVG_I64) avg_srcs.insert(plan_.agg_acc[g]);
   AB_REQUIRE(old_n_acc + (int)avg_srcs.size() <= MAX_ACC, ARROYO_B200_RUNTIME, "too many accumulators after AVG promotion");
   std::vector<std::pair<int, int>> f64_from;
-  for (int g = 0; g < n_aggs_; ++g) {
-    if (agg_kind_[g] != ARROYO_B200_AGG_AVG_I64) continue;
-    const int src = agg_acc_[g];
+  for (int g = 0; g < plan_.n_aggs; ++g) {
+    if (plan_.agg_kind[g] != ARROYO_B200_AGG_AVG_I64) continue;
+    const int src = plan_.agg_acc[g];
     int found = -1;
     for (auto& pr : f64_from)
       if (pr.second == src) found = pr.first;
     if (found < 0) {
-      found = n_acc_;
-      acc_kind_[n_acc_] = ACC_SUM_F64;
-      acc_val_[n_acc_] = acc_val_[src];
-      ++n_acc_;
+      found = plan_.n_acc;
+      plan_.acc_kind[plan_.n_acc] = ACC_SUM_F64;
+      plan_.acc_val[plan_.n_acc] = plan_.acc_val[src];
+      ++plan_.n_acc;
       f64_from.emplace_back(found, src);
     }
-    agg_acc_[g] = found;
+    plan_.agg_acc[g] = found;
   }
   avg_exact_ = false;
   // f64 accumulators are not exactly invertible: leave running mode (see the constructor)
@@ -1683,8 +1576,8 @@ void WindowAggOp::add_segment(const long long* key, const long long* ts, const l
   if (n <= 0) return;
   if (!segs_.empty()) {
     Segment& l = segs_.back();
-    bool contig = l.ts + l.n == ts && (!keyed_ || l.key + l.n == key);
-    for (int v = 0; v < n_vals_; ++v) contig = contig && (l.val[v] + l.n == vals[v]);
+    bool contig = l.ts + l.n == ts && (!plan_.keyed || l.key + l.n == key);
+    for (int v = 0; v < plan_.n_vals; ++v) contig = contig && (l.val[v] + l.n == vals[v]);
     if (contig) {
       l.n += n;
       pending_rows_ += n;
@@ -1695,7 +1588,7 @@ void WindowAggOp::add_segment(const long long* key, const long long* ts, const l
   Segment s{};
   s.key = key;
   s.ts = ts;
-  for (int v = 0; v < n_vals_; ++v) s.val[v] = vals[v];
+  for (int v = 0; v < plan_.n_vals; ++v) s.val[v] = vals[v];
   s.n = n;
   segs_.push_back(s);
   pending_rows_ += n;
@@ -1714,14 +1607,14 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
   int64_t n = 0;
   std::vector<InColumn> cols = import_batch(batch, schema, &n);
   AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
-  require_aggregate_input_types(cols, keyed_ ? key_col_ : -1, val_cols_, n_vals_);
-  if (keyed_) key_format_ = cols[key_col_].format;
+  require_aggregate_input_types(cols, plan_.keyed ? plan_.key_col : -1, plan_.val_cols, plan_.n_vals);
+  if (plan_.keyed) key_format_ = cols[plan_.key_col].format;
   poll_releases(false);
   st_.rows_in += (uint64_t)n;
   if (n > 0 && panes_.empty() && max_bin_seen_ == LLONG_MIN) {
     // residency hint only (no semantics): make the first row's pane resident so a cold start does
     // not have to go through the deferred path
-    int64_t b0 = bin_start((int64_t)cols[ts_col_].data[0], slide_);
+    int64_t b0 = bin_start((int64_t)cols[plan_.ts_col].data[0], slide_);
     if (b0 >= late_bin_) {
       ensure_pane(b0);
       max_bin_seen_ = b0;
@@ -1744,28 +1637,28 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
       if (at.type != cudaMemoryTypeHost || at.devicePointer == nullptr) pinned = false;
       else devp[c] = (const uint64_t*)at.devicePointer;
     };
-    if (keyed_) probe(key_col_);
-    probe(ts_col_);
-    for (int v = 0; v < n_vals_; ++v) probe(val_cols_[v]);
+    if (plan_.keyed) probe(plan_.key_col);
+    probe(plan_.ts_col);
+    for (int v = 0; v < plan_.n_vals; ++v) probe(plan_.val_cols[v]);
     if (pinned) {
       int64_t done = 0;
       while (done < n) {
         int64_t take = std::min<int64_t>(n - done, launch_rows_ - pending_rows_);
         const long long* vals[MAX_VALS];
-        for (int v = 0; v < n_vals_; ++v) vals[v] = (const long long*)devp[val_cols_[v]] + done;
-        add_segment(keyed_ ? (const long long*)devp[key_col_] + done : nullptr, (const long long*)devp[ts_col_] + done,
+        for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)devp[plan_.val_cols[v]] + done;
+        add_segment(plan_.keyed ? (const long long*)devp[plan_.key_col] + done : nullptr, (const long long*)devp[plan_.ts_col] + done,
                     vals, take);
         done += take;
         if (done < n && pending_rows_ >= launch_rows_) launch_pending();
       }
-      st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((keyed_ ? 1 : 0) + 1 + n_vals_);
+      st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((plan_.keyed ? 1 : 0) + 1 + plan_.n_vals);
       zero_copy_inputs_.push_back(*batch);
       batch->release = nullptr;
       if (pending_rows_ >= launch_rows_) launch_pending();
       return;
     }
   }
-  const int n_used = 2 + n_vals_;
+  const int n_used = 2 + plan_.n_vals;
   int64_t done = 0;
   while (done < n) {
     if (!chunk_[cur_chunk_].p) chunk_[cur_chunk_].alloc((size_t)n_used * chunk_rows_ * 8);
@@ -1780,14 +1673,14 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
     long long* d_key = base + 0 * chunk_rows_ + cur_rows_;
     long long* d_ts = base + 1 * chunk_rows_ + cur_rows_;
     const long long* d_vals[MAX_VALS];
-    if (keyed_) queue_copy(d_key, cols[key_col_].data + done, (size_t)take * 8);
-    queue_copy(d_ts, cols[ts_col_].data + done, (size_t)take * 8);
-    for (int v = 0; v < n_vals_; ++v) {
+    if (plan_.keyed) queue_copy(d_key, cols[plan_.key_col].data + done, (size_t)take * 8);
+    queue_copy(d_ts, cols[plan_.ts_col].data + done, (size_t)take * 8);
+    for (int v = 0; v < plan_.n_vals; ++v) {
       long long* dv = base + (size_t)(2 + v) * chunk_rows_ + cur_rows_;
-      queue_copy(dv, cols[val_cols_[v]].data + done, (size_t)take * 8);
+      queue_copy(dv, cols[plan_.val_cols[v]].data + done, (size_t)take * 8);
       d_vals[v] = dv;
     }
-    st_.h2d_bytes += (uint64_t)take * 8 * (uint64_t)((keyed_ ? 1 : 0) + 1 + n_vals_);
+    st_.h2d_bytes += (uint64_t)take * 8 * (uint64_t)((plan_.keyed ? 1 : 0) + 1 + plan_.n_vals);
     add_segment(d_key, d_ts, d_vals, take);
     pending_uses_chunk_ = true;
     cur_rows_ += take;
@@ -1812,8 +1705,8 @@ void WindowAggOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols,
   while (done < n_rows) {
     int64_t take = std::min<int64_t>(n_rows - done, launch_rows_ - pending_rows_);
     const long long* vals[MAX_VALS];
-    for (int v = 0; v < n_vals_; ++v) vals[v] = (const long long*)cols[val_cols_[v]] + done;
-    add_segment(keyed_ ? (const long long*)cols[key_col_] + done : nullptr, (const long long*)cols[ts_col_] + done, vals,
+    for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)cols[plan_.val_cols[v]] + done;
+    add_segment(plan_.keyed ? (const long long*)cols[plan_.key_col] + done : nullptr, (const long long*)cols[plan_.ts_col] + done, vals,
                 take);
     done += take;
     if (pending_rows_ >= launch_rows_) launch_pending();
@@ -1825,8 +1718,8 @@ void WindowAggOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols,
 // the per-bucket set-up and the dictionary fits the partition kernel's histograms.  Everything else -- and every row
 // the two passes hand back -- runs through the one-pass kernel.
 bool WindowAggOp::two_pass_eligible(uint64_t rows) const {
-  if (!two_pass_enabled_ || !keyed_ || rows_slot_ >= 0 || n_vals_ > 1 || n_acc_ > 2) return false;
-  if (n_acc_ == 2 && acc_kind_[1] != ACC_SUM_I64) return false;
+  if (!two_pass_enabled_ || !plan_.keyed || rows_slot_ >= 0 || plan_.n_vals > 1 || plan_.n_acc > 2) return false;
+  if (plan_.n_acc == 2 && plan_.acc_kind[1] != ACC_SUM_I64) return false;
   if (n_buckets_ > (uint64_t)P1_NR) return false;
   if (max_bin_seen_ == LLONG_MIN) return false;  // no pane known yet: the first launch finds out where the stream is
   if (two_pass_pause_ > 0) {
@@ -1901,7 +1794,7 @@ void WindowAggOp::launch_two_pass(IngestParams& p, uint64_t rows, long long tile
   }
   const uint32_t n_work = tp.tail_first * tp.slices + ((uint32_t)n_buckets_ - tp.tail_first) * tp.tail_slices;
   const int grid2 = (int)std::max<uint32_t>(1, std::min<uint32_t>(n_work, max_blocks));
-  if (n_vals_ == 0) {
+  if (plan_.n_vals == 0) {
     part_kernel<0, 0><<<grid1, P1_THREADS, P1_SMEM, stream_>>>(p, tp);
     AB_CUDA(cudaGetLastError());
     agg_kernel<0><<<grid2, P2_NW * 32, P2_SMEM, stream_>>>(p, tp);
@@ -1933,8 +1826,8 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
     hs[i] = segs_in[i];
     hs[i].tile_start = tiles;
     uintptr_t al = (uintptr_t)hs[i].ts;
-    if (keyed_) al |= (uintptr_t)hs[i].key;
-    for (int v = 0; v < n_vals_; ++v) al |= (uintptr_t)hs[i].val[v];
+    if (plan_.keyed) al |= (uintptr_t)hs[i].key;
+    for (int v = 0; v < plan_.n_vals; ++v) al |= (uintptr_t)hs[i].val[v];
     hs[i].vec_ok = (al & 15) == 0;
     tiles += (hs[i].n + TILE - 1) / TILE;
     rows += (uint64_t)hs[i].n;
@@ -1942,13 +1835,13 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
   AB_CUDA(cudaMemcpyAsync(d_segs_[li].p, hs, segs_in.size() * sizeof(Segment), cudaMemcpyHostToDevice, stream_));
   if (ring_ > RING_INLINE) upload_ring();
   if (!defer_[defer_cur_][0].p) {
-    for (int c = 0; c < 2 + n_vals_; ++c) defer_[defer_cur_][c].alloc(defer_cap_ * 8);
+    for (int c = 0; c < 2 + plan_.n_vals; ++c) defer_[defer_cur_][c].alloc(defer_cap_ * 8);
   }
 
   IngestParams p{};
   p.segs = d_segs_[li].as<Segment>();
   p.n_segs = (int)segs_in.size();
-  p.keyed = keyed_ ? 1 : 0;
+  p.keyed = plan_.keyed ? 1 : 0;
   p.n_tiles = tiles;
   p.dict = dict_view();
   p.slide_div = FastDivU64::make((uint64_t)slide_);
@@ -1960,7 +1853,7 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
   p.combine = (cfg.flags & ARROYO_B200_FLAG_NO_COMBINE) ? 0 : 1;
   p.rows_slot = rows_slot_;
   p.ring_mask = ring_ - 1;
-  p.n_acc = n_acc_;
+  p.n_acc = plan_.n_acc;
   p.pane_bins = d_pane_bins_.as<long long>();
   p.pane_ptrs = d_pane_ptrs_.as<unsigned long long*>();
   p.id_cap = id_cap_;
@@ -1970,15 +1863,15 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
       p.ring_bins[i] = h_pane_bins_[i];
       p.ring_ptrs[i] = h_pane_ptrs_[i];
     }
-  for (int a = 0; a < n_acc_; ++a) {
-    p.acc_kind[a] = acc_kind_[a];
-    p.acc_val[a] = acc_val_[a];
+  for (int a = 0; a < plan_.n_acc; ++a) {
+    p.acc_kind[a] = plan_.acc_kind[a];
+    p.acc_val[a] = plan_.acc_val[a];
   }
   p.counters = d_counters();
   p.slot_rows = d_slot_rows();
   p.d_key = defer_[defer_cur_][0].as<long long>();
   p.d_ts = defer_[defer_cur_][1].as<long long>();
-  for (int v = 0; v < n_vals_; ++v) p.d_val[v] = defer_[defer_cur_][2 + v].as<long long>();
+  for (int v = 0; v < plan_.n_vals; ++v) p.d_val[v] = defer_[defer_cur_][2 + v].as<long long>();
   p.defer_cap = defer_cap_;
 
   int grid = (int)std::min<long long>(tiles, (long long)num_sms_ * 8);
@@ -1998,22 +1891,22 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
   }
   // straight-line specialisations for the common accumulator signatures, generic otherwise
   int sig = GENERIC_SIG;
-  if (n_vals_ <= 1 && n_acc_ <= 4) {
+  if (plan_.n_vals <= 1 && plan_.n_acc <= 4) {
     int k[3] = {0, 0, 0};
-    for (int a = 1; a < n_acc_; ++a) k[a - 1] = acc_kind_[a];
+    for (int a = 1; a < plan_.n_acc; ++a) k[a - 1] = plan_.acc_kind[a];
     sig = sig_of(k[0], k[1], k[2]);
   }
 #define AB_LAUNCH(NV, SIG) ingest_kernel<NV, SIG><<<grid, THREADS, 0, stream_>>>(p)
   if (two_pass) {
     // launched above
-  } else if (n_vals_ == 0) AB_LAUNCH(0, 0);
-  else if (n_vals_ == 1 && sig == sig_of(ACC_SUM_I64)) AB_LAUNCH(1, sig_of(ACC_SUM_I64));
-  else if (n_vals_ == 1 && sig == sig_of(ACC_SUM_F64)) AB_LAUNCH(1, sig_of(ACC_SUM_F64));
-  else if (n_vals_ == 1 && sig == sig_of(ACC_SUM_I64, ACC_SUM_F64)) AB_LAUNCH(1, sig_of(ACC_SUM_I64, ACC_SUM_F64));
-  else if (n_vals_ == 1 && sig == sig_of(ACC_MIN_I64, ACC_MAX_I64)) AB_LAUNCH(1, sig_of(ACC_MIN_I64, ACC_MAX_I64));
-  else if (n_vals_ == 1) AB_LAUNCH(1, GENERIC_SIG);
-  else if (n_vals_ == 2) AB_LAUNCH(2, GENERIC_SIG);
-  else if (n_vals_ == 3) AB_LAUNCH(3, GENERIC_SIG);
+  } else if (plan_.n_vals == 0) AB_LAUNCH(0, 0);
+  else if (plan_.n_vals == 1 && sig == sig_of(ACC_SUM_I64)) AB_LAUNCH(1, sig_of(ACC_SUM_I64));
+  else if (plan_.n_vals == 1 && sig == sig_of(ACC_SUM_F64)) AB_LAUNCH(1, sig_of(ACC_SUM_F64));
+  else if (plan_.n_vals == 1 && sig == sig_of(ACC_SUM_I64, ACC_SUM_F64)) AB_LAUNCH(1, sig_of(ACC_SUM_I64, ACC_SUM_F64));
+  else if (plan_.n_vals == 1 && sig == sig_of(ACC_MIN_I64, ACC_MAX_I64)) AB_LAUNCH(1, sig_of(ACC_MIN_I64, ACC_MAX_I64));
+  else if (plan_.n_vals == 1) AB_LAUNCH(1, GENERIC_SIG);
+  else if (plan_.n_vals == 2) AB_LAUNCH(2, GENERIC_SIG);
+  else if (plan_.n_vals == 3) AB_LAUNCH(3, GENERIC_SIG);
   else AB_LAUNCH(4, GENERIC_SIG);
 #undef AB_LAUNCH
   AB_CUDA(cudaGetLastError());
@@ -2157,7 +2050,7 @@ void WindowAggOp::drain_deferred() {
     if (last_counters_.big_vals && avg_exact_) promote_avg();
     // dictionary pressure: a bucket ran out of ids (its rows were deferred), or the mean bucket fill is past the
     // point where that becomes likely: double the bucket count
-    if (keyed_ && (last_counters_.dict_full != dict_full_seen_ ||
+    if (plan_.keyed && (last_counters_.dict_full != dict_full_seen_ ||
                    (uint64_t)last_counters_.n_keys > n_buckets_ * (uint64_t)(BD_MEAN + BD_MEAN / 8))) {
       dict_full_seen_ = last_counters_.dict_full;
       grow_ids();
@@ -2172,7 +2065,7 @@ void WindowAggOp::drain_deferred() {
     Segment s{};
     s.key = defer_[full][0].as<long long>();
     s.ts = defer_[full][1].as<long long>();
-    for (int v = 0; v < n_vals_; ++v) s.val[v] = defer_[full][2 + v].as<long long>();
+    for (int v = 0; v < plan_.n_vals; ++v) s.val[v] = defer_[full][2 + v].as<long long>();
     s.n = (long long)n;
     // deferred rows were already counted (late rows among them are counted when re-ingested)
     launch_segments({s}, -1);
@@ -2241,7 +2134,7 @@ WindowAggOp::OutSet* WindowAggOp::out_set(size_t i, uint64_t cap) {
     os->wstart.alloc(c * 8);
     os->wend.alloc(c * 8);
     os->ts.alloc(c * 8);
-    for (int g = 0; g < n_aggs_; ++g) os->agg[g].alloc(c * 8);
+    for (int g = 0; g < plan_.n_aggs; ++g) os->agg[g].alloc(c * 8);
     os->cap = c;
     for (int a = 0; a < MAX_ACC; ++a) os->state[a].release();
   }
@@ -2268,21 +2161,21 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
   }
   p.panes = d_emit_panes_.as<const unsigned long long*>();
   p.n_panes = (int)blocks.size();
-  p.n_acc = n_acc_;
+  p.n_acc = plan_.n_acc;
   p.id_cap = id_cap_;
   p.n_ids = n_ids;
-  p.keyed = keyed_ ? 1 : 0;
-  for (int a = 0; a < n_acc_; ++a) p.acc_kind[a] = acc_kind_[a];
+  p.keyed = plan_.keyed ? 1 : 0;
+  for (int a = 0; a < plan_.n_acc; ++a) p.acc_kind[a] = plan_.acc_kind[a];
   std::vector<std::pair<unsigned long long*, unsigned long long*>> dup_cols;  // (src, dst): same output twice
   for (int a = 0; a < MAX_ACC; ++a) {
     p.out_raw[a] = nullptr;
     p.out_avg[a] = nullptr;
   }
   if (!partial) {
-    for (int g = 0; g < n_aggs_; ++g) {
+    for (int g = 0; g < plan_.n_aggs; ++g) {
       unsigned long long* col = os->agg[g].as<unsigned long long>();
-      const bool avg = agg_kind_[g] == ARROYO_B200_AGG_AVG_I64;
-      const int a = agg_kind_[g] == ARROYO_B200_AGG_COUNT_STAR ? 0 : agg_acc_[g];
+      const bool avg = plan_.agg_kind[g] == ARROYO_B200_AGG_AVG_I64;
+      const int a = plan_.agg_kind[g] == ARROYO_B200_AGG_COUNT_STAR ? 0 : plan_.agg_acc[g];
       unsigned long long*& slot = avg ? p.out_avg[a] : p.out_raw[a];
       if (slot) dup_cols.emplace_back(slot, col);
       else slot = col;
@@ -2309,7 +2202,7 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
   p.n_add = n_add;
   p.partial = partial ? 1 : 0;
   if (partial) {
-    for (int a = 0; a < n_acc_; ++a) {
+    for (int a = 0; a < plan_.n_acc; ++a) {
       if (!os->state[a].p) os->state[a].alloc(os->cap * 8);
       p.out_state[a] = os->state[a].as<unsigned long long>();
     }
@@ -2330,7 +2223,7 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
     if (use_running) emit_kernel<true, N><<<grid, EMIT_THREADS, 0, stream_>>>(p); \
     else emit_kernel<false, N><<<grid, EMIT_THREADS, 0, stream_>>>(p);            \
   } while (0)
-  switch (n_acc_) {
+  switch (plan_.n_acc) {
     case 1: AB_EMIT(1); break;
     case 2: AB_EMIT(2); break;
     case 3: AB_EMIT(3); break;
@@ -2372,13 +2265,6 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
   return n_out;
 }
 
-static void* d2h_column(const void* dev, int64_t n, cudaStream_t s, uint64_t* bytes) {
-  void* h = PinnedPool::get().alloc((size_t)std::max<int64_t>(n, 1) * 8);
-  if (n > 0) AB_CUDA(cudaMemcpyAsync(h, dev, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-  *bytes += (uint64_t)n * 8;
-  return h;
-}
-
 // Output batch in the operator's out_schema order: aggregate output columns [key?, aggs...] with the
 // window struct inserted at window_index, then _timestamp (planner extension/aggregate.rs:306-389).
 void WindowAggOp::export_window(OutSet* os, int64_t n, BatchesPriv* out_host) {
@@ -2389,45 +2275,11 @@ void WindowAggOp::export_window(OutSet* os, int64_t n, BatchesPriv* out_host) {
     AB_CUDA(cudaStreamWaitEvent(out_stream_, emit_done_, 0));
     cs = out_stream_;
   }
-  std::vector<OutColumn> cols;
-  if (keyed_) {
-    OutColumn k;
-    k.name = "key";
-    k.format = key_format_;
-    k.data = d2h_column(os->key.p, n, cs, &st_.d2h_bytes);
-    cols.push_back(k);
-  }
-  for (int g = 0; g < n_aggs_; ++g) {
-    OutColumn a;
-    a.name = "agg" + std::to_string(g);
-    a.format = agg_format_[g];
-    a.data = d2h_column(os->agg[g].p, n, cs, &st_.d2h_bytes);
-    cols.push_back(a);
-  }
-  if (cfg.final_projection) {
-    OutColumn w;
-    w.name = "window";
-    w.format = "+s";
-    OutColumn ws, we;
-    ws.name = "start";
-    ws.format = "tsn:";
-    ws.data = d2h_column(os->wstart.p, n, cs, &st_.d2h_bytes);
-    we.name = "end";
-    we.format = "tsn:";
-    we.data = d2h_column(os->wend.p, n, cs, &st_.d2h_bytes);
-    w.children = {ws, we};
-    int wi = std::min<int>(std::max<int>(cfg.window_index, 0), (int)cols.size());
-    cols.insert(cols.begin() + wi, w);
-  }
-  OutColumn t;
-  t.name = "_timestamp";
-  t.format = "tsn:";
-  t.data = d2h_column(os->ts.p, n, cs, &st_.d2h_bytes);
-  cols.push_back(t);
+  // the window struct is part of the final projection only; its position counts [key?, aggs...]
+  const int wi = std::min<int>(std::max<int>(cfg.window_index, 0), (plan_.keyed ? 1 : 0) + plan_.n_aggs);
+  export_window_batch(out_host, n, cs, &st_.d2h_bytes, plan_.keyed ? os->key.p : nullptr, key_format_, os->agg,
+                      plan_.agg_format, cfg.final_projection ? os->wstart.p : nullptr, os->wend.p, wi, os->ts.p);
   if (!async_out_) AB_CUDA(cudaStreamSynchronize(stream_));
-  out_host->arrays.emplace_back();
-  out_host->schemas.emplace_back();
-  export_batch(cols, n, &out_host->arrays.back(), &out_host->schemas.back());
 }
 
 // Partial-state batch in `partial_schema`: [key?, state cols..., _timestamp = pane start]
@@ -2435,37 +2287,37 @@ void WindowAggOp::export_window(OutSet* os, int64_t n, BatchesPriv* out_host) {
 void WindowAggOp::export_partial(OutSet* os, int64_t n, BatchesPriv* out) {
   std::vector<OutColumn> cols;
   std::vector<size_t> fix_f64;  // AVG state kept as an exact integer sum: the partial schema wants Float64
-  if (keyed_) {
+  if (plan_.keyed) {
     OutColumn k;
     k.name = "key";
     k.format = key_format_;
-    k.data = d2h_column(os->key.p, n, stream_, &st_.d2h_bytes);
+    k.data = d2h_pinned(os->key.p, (size_t)n * 8, stream_, &st_.d2h_bytes);
     cols.push_back(k);
   }
-  for (int g = 0; g < n_aggs_; ++g) {
+  for (int g = 0; g < plan_.n_aggs; ++g) {
     auto add = [&](const char* nm, const char* fmt, const void* dev) {
       OutColumn c;
       c.name = std::string("agg") + std::to_string(g) + nm;
       c.format = fmt;
-      c.data = d2h_column(dev, n, stream_, &st_.d2h_bytes);
+      c.data = d2h_pinned(dev, (size_t)n * 8, stream_, &st_.d2h_bytes);
       cols.push_back(c);
     };
-    switch (agg_kind_[g]) {
+    switch (plan_.agg_kind[g]) {
       case ARROYO_B200_AGG_COUNT_STAR: add("[count]", "l", os->state[0].p); break;
-      case ARROYO_B200_AGG_SUM_I64: add("[sum]", "l", os->state[agg_acc_[g]].p); break;
+      case ARROYO_B200_AGG_SUM_I64: add("[sum]", "l", os->state[plan_.agg_acc[g]].p); break;
       case ARROYO_B200_AGG_AVG_I64:
         add("[count]", "L", os->state[0].p);
-        add("[sum]", "g", os->state[agg_acc_[g]].p);
-        if (acc_kind_[agg_acc_[g]] == ACC_SUM_I64) fix_f64.push_back(cols.size() - 1);
+        add("[sum]", "g", os->state[plan_.agg_acc[g]].p);
+        if (plan_.acc_kind[plan_.agg_acc[g]] == ACC_SUM_I64) fix_f64.push_back(cols.size() - 1);
         break;
-      case ARROYO_B200_AGG_MIN_I64: add("[min]", agg_format_[g].c_str(), os->state[agg_acc_[g]].p); break;
-      case ARROYO_B200_AGG_MAX_I64: add("[max]", agg_format_[g].c_str(), os->state[agg_acc_[g]].p); break;
+      case ARROYO_B200_AGG_MIN_I64: add("[min]", plan_.agg_format[g].c_str(), os->state[plan_.agg_acc[g]].p); break;
+      case ARROYO_B200_AGG_MAX_I64: add("[max]", plan_.agg_format[g].c_str(), os->state[plan_.agg_acc[g]].p); break;
     }
   }
   OutColumn t;
   t.name = "_timestamp";
   t.format = "tsn:";
-  t.data = d2h_column(os->ts.p, n, stream_, &st_.d2h_bytes);
+  t.data = d2h_pinned(os->ts.p, (size_t)n * 8, stream_, &st_.d2h_bytes);
   cols.push_back(t);
   AB_CUDA(cudaStreamSynchronize(stream_));
   for (size_t ci : fix_f64) {
@@ -2552,8 +2404,8 @@ void WindowAggOp::emit_window(int64_t a, int64_t b, size_t out_index, BatchesPri
     d.n_rows = n;
     int c = 0;
     std::vector<uint64_t> cols;
-    if (keyed_) cols.push_back((uint64_t)os->key.p);
-    for (int g = 0; g < n_aggs_; ++g) cols.push_back((uint64_t)os->agg[g].p);
+    if (plan_.keyed) cols.push_back((uint64_t)os->key.p);
+    for (int g = 0; g < plan_.n_aggs; ++g) cols.push_back((uint64_t)os->agg[g].p);
     if (cfg.final_projection) {
       int wi = std::min<int>(std::max<int>(cfg.window_index, 0), (int)cols.size());
       cols.insert(cols.begin() + wi, (uint64_t)os->wend.p);
@@ -2745,8 +2597,8 @@ void WindowAggOp::handle_checkpoint(int64_t wm, BatchesPriv* out) {
     fp.frozen = p.frozen;
     fp.id_cap = id_cap_;
     fp.n_ids = n_keys_host_;
-    fp.n_acc = n_acc_;
-    for (int a = 0; a < n_acc_; ++a) fp.acc_kind[a] = acc_kind_[a];
+    fp.n_acc = plan_.n_acc;
+    for (int a = 0; a < plan_.n_acc; ++a) fp.acc_kind[a] = plan_.acc_kind[a];
     int grid = (int)std::min<uint32_t>((n_keys_host_ + 255) / 256, (uint32_t)num_sms_ * 8);
     fold_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(fp);
     AB_CUDA(cudaGetLastError());
@@ -2779,8 +2631,8 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
   if (sliding_) sliding_planner_->restore_begin(has_wm, watermark);
   // expected partial layout
   int n_state_cols = 0;
-  for (int g = 0; g < n_aggs_; ++g) n_state_cols += agg_kind_[g] == ARROYO_B200_AGG_AVG_I64 ? 2 : 1;
-  const int expect_cols = (keyed_ ? 1 : 0) + n_state_cols + 1;
+  for (int g = 0; g < plan_.n_aggs; ++g) n_state_cols += plan_.agg_kind[g] == ARROYO_B200_AGG_AVG_I64 ? 2 : 1;
+  const int expect_cols = (plan_.keyed ? 1 : 0) + n_state_cols + 1;
   std::vector<DevBuf> keep;
   for (int64_t bi = 0; bi < n; ++bi) {
     int64_t rows = 0;
@@ -2788,7 +2640,7 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
     AB_REQUIRE((int)cols.size() == expect_cols, ARROYO_B200_INVALID_ARGUMENT,
                "state batch does not match the partial schema");
     if (rows == 0) continue;
-    if (keyed_) key_format_ = cols[0].format;
+    if (plan_.keyed) key_format_ = cols[0].format;
     const int64_t ts = (int64_t)cols.back().data[0];
     const int64_t bin = bin_start(ts, slide_);
     ensure_pane(bin);
@@ -2803,20 +2655,20 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
     // upload columns
     PartialParams pp{};
     pp.n = rows;
-    pp.keyed = keyed_ ? 1 : 0;
-    pp.n_acc = n_acc_;
-    for (int a = 0; a < n_acc_; ++a) pp.acc_kind[a] = acc_kind_[a];
+    pp.keyed = plan_.keyed ? 1 : 0;
+    pp.n_acc = plan_.n_acc;
+    for (int a = 0; a < plan_.n_acc; ++a) pp.acc_kind[a] = plan_.acc_kind[a];
     auto up = [&](const uint64_t* h) -> const unsigned long long* {
       keep.emplace_back((size_t)rows * 8);
       AB_CUDA(cudaMemcpyAsync(keep.back().p, h, (size_t)rows * 8, cudaMemcpyHostToDevice, stream_));
       return keep.back().as<unsigned long long>();
     };
     int ci = 0;
-    if (keyed_) pp.key = (const long long*)up(cols[ci++].data);
+    if (plan_.keyed) pp.key = (const long long*)up(cols[ci++].data);
     for (int a = 0; a < MAX_ACC; ++a) pp.state[a] = nullptr;
     std::vector<std::pair<int, int>> avg_sum_cols;  // (agg, column of its f64 sum)
-    for (int g = 0; g < n_aggs_; ++g) {
-      switch (agg_kind_[g]) {
+    for (int g = 0; g < plan_.n_aggs; ++g) {
+      switch (plan_.agg_kind[g]) {
         case ARROYO_B200_AGG_COUNT_STAR: {
           const unsigned long long* c = up(cols[ci++].data);
           if (!pp.state[0]) pp.state[0] = c;
@@ -2829,14 +2681,14 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
           break;
         }
         default:
-          pp.state[agg_acc_[g]] = up(cols[ci++].data);
+          pp.state[plan_.agg_acc[g]] = up(cols[ci++].data);
           break;
       }
     }
     std::vector<long long> conv;
     for (auto& pr : avg_sum_cols) {
-      const int acc = agg_acc_[pr.first];
-      if (acc_kind_[acc] == ACC_SUM_F64) {
+      const int acc = plan_.agg_acc[pr.first];
+      if (plan_.acc_kind[acc] == ACC_SUM_F64) {
         pp.state[acc] = up(cols[pr.second].data);
       } else if (!pp.state[acc]) {
         // exact-sum AVG without a SUM over the same column: the checkpoint only has the f64 image of the sum
@@ -2860,7 +2712,7 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
       pp.state[0] = keep.back().as<unsigned long long>();
     }
     // room for every key of the batch at the target bucket fill (most of them are usually known already)
-    while (keyed_ && (uint64_t)total_keys_host_ + (uint64_t)rows > n_buckets_ * (uint64_t)BD_MEAN) {
+    while (plan_.keyed && (uint64_t)total_keys_host_ + (uint64_t)rows > n_buckets_ * (uint64_t)BD_MEAN) {
       AB_CUDA(cudaStreamSynchronize(stream_));
       grow_ids();
     }
@@ -2888,7 +2740,7 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
 void WindowAggOp::stats(ArroyoB200Stats* out) {
   set_device();
   resolve_deferred();  // an outstanding emission's windows are counted once their row counts are in
-  st_.n_keys = keyed_ ? total_keys_host_ : 0;
+  st_.n_keys = plan_.keyed ? total_keys_host_ : 0;
   st_.rows_late = last_counters_.late_rows;
   *out = st_;
 }

@@ -75,6 +75,14 @@ def test_bad_config_is_rejected_before_touching_cuda():
     cfg.kind = ffi.TUMBLING_AGGREGATE
     cfg.width_ns = 0  # instant window: outside the supported subset
     assert lib.arroyo_b200_op_create(C.byref(cfg), C.byref(h), err, 256) == ffi.UNSUPPORTED
+    # a group-by key column outside the input, for each aggregating operator
+    cfg.width_ns = cfg.slide_ns = cfg.gap_ns = 10 * 10**9
+    cfg.n_key_cols = 1
+    cfg.key_col = 2
+    for kind in (ffi.TUMBLING_AGGREGATE, ffi.SESSION_AGGREGATE, ffi.UPDATING_AGGREGATE):
+        cfg.kind = kind
+        st = lib.arroyo_b200_op_create(C.byref(cfg), C.byref(h), err, 256)
+        assert st == ffi.INVALID_ARGUMENT and b"key_col" in err.value and not h, (kind, st, err.value)
 
 
 def test_bin_start_fast_division_matches_modulo():
