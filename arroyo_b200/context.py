@@ -69,6 +69,22 @@ class StateTable:
                     yield t, b
 
 
+class KeyValueTable:
+    """The slice of UncachedKeyValueView (arroyo-state/src/tables/expiring_time_key_map.rs:1073-1110) the updating
+    aggregate uses: `insert_batch` appends a batch of rows, `get_all` yields every batch written so far, in no
+    particular order and without de-duplication (a key may have rows in several batches; its `_generation` column
+    tells which is the latest)."""
+
+    def __init__(self):
+        self.batches: list = []
+
+    def insert_batch(self, batch):
+        self.batches.append(batch)
+
+    def get_all(self):
+        yield from self.batches
+
+
 class OperatorContext:
     def __init__(self, n_inputs: int = 1, task_index: int = 0, parallelism: int = 1):
         self.watermarks = WatermarkHolder(n_inputs)
@@ -86,6 +102,12 @@ class OperatorContext:
         if name not in self.tables:
             self.tables[name] = StateTable(retention)
         return self.tables[name]
+
+    def key_value_table(self, name: str) -> KeyValueTable:
+        """get_uncached_key_value_view(name)."""
+        if not hasattr(self, "key_value_tables"):
+            self.key_value_tables = {}
+        return self.key_value_tables.setdefault(name, KeyValueTable())
 
     def global_table(self, name: str) -> dict:
         """GlobalKeyedView (arroyo-state/src/tables/global_keyed_map.rs): one value per subtask, all of them

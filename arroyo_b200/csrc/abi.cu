@@ -406,6 +406,23 @@ int32_t arroyo_b200_op_handle_checkpoint(ArroyoB200Op* op, int64_t watermark_ns,
   });
 }
 
+int32_t arroyo_b200_op_checkpoint_state(ArroyoB200Op* op, ArroyoB200Batches* state_out) {
+  if (state_out) memset(state_out, 0, sizeof *state_out);
+  return guarded(op, [&](OpBase* o) {
+    AB_REQUIRE(state_out != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null out");
+    auto* priv = new BatchesPriv();
+    try {
+      o->checkpoint_state(priv);
+    } catch (...) {
+      ArroyoB200Batches tmp{};
+      batches_finish(priv, &tmp);
+      batches_release(&tmp);
+      throw;
+    }
+    batches_finish(priv, state_out);
+  });
+}
+
 int32_t arroyo_b200_op_on_close(ArroyoB200Op* op, int32_t end_of_data, ArroyoB200Batches* out) {
   if (out) memset(out, 0, sizeof *out);
   return guarded(op, [&](OpBase* o) {

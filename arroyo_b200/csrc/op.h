@@ -35,6 +35,8 @@ class OpBase {
   virtual void handle_checkpoint(int64_t watermark, BatchesPriv* out) = 0;
   virtual void on_close(int end_of_data, BatchesPriv* out) = 0;
   virtual void handle_tick(BatchesPriv* /*out*/) {}
+  // the key-value state table the updating aggregate writes at a checkpoint; every other operator has none
+  virtual void checkpoint_state(BatchesPriv* /*out*/) {}
   virtual void flush() = 0;
   // enqueue whatever input is still being batched on the host side; does not wait
   virtual void submit() {}

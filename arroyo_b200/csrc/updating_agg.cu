@@ -14,7 +14,16 @@
 //           (drain_deferred);
 //   flush   one thread per touched key: compares the accumulators with their values at the previous flush (kept per
 //           id: "the values it had before"), writes the retraction row (old values, old timestamp) and the append row
-//           (new values), and rolls the snapshot forward.
+//           (new values), and rolls the snapshot forward.  It also marks the id "flushed since the last state
+//           export" (one byte store per key);
+//   state   checkpoint_state writes table "a" (checkpoint_sliding :272-340, insert_batch :619-635): one row per marked
+//           id, compacted from the snapshot, [key?, per aggregate its accumulator state, _timestamp, _generation].
+//           The reference writes at every flush; writing at a checkpoint the keys flushed since the last export leaves
+//           the same latest row per key.  Every export carries one generation, one above the last;
+//   restore on_start (initialize :446-503) reads table "a" back: the keys go into the dictionary (growing it when a
+//           bucket runs out of ids), the row with the largest (_generation, position) wins per key and seeds both the
+//           live accumulators and the previous-flush snapshot, so the first flush retracts what the uninterrupted run
+//           would have retracted.
 // Output rows: [key?, aggregates..., _timestamp, is_retract] -- retractions first, then appends (a key's retraction
 // must precede its append; the order between keys is unspecified in the reference too: it iterates a HashMap).
 // The shim wraps `is_retract` into the `_updating_meta` struct together with the row id its metadata expression
@@ -38,6 +47,7 @@ struct UState {
   long long* cur_ts;         // max(_timestamp)
   long long* prev_ts;
   unsigned int* touched;     // per id: in the touched list
+  unsigned char* flushed;    // per id: flushed since the last state export
   unsigned int* list;        // touched ids
   unsigned int* n_touched;
   unsigned long long id_cap;
@@ -148,6 +158,101 @@ __global__ void __launch_bounds__(256) upd_flush_kernel(const __grid_constant__ 
     for (int a = 0; a < p.st.n_acc; ++a) p.st.prev[(unsigned long long)a * p.st.id_cap + id] = now[a];
     p.st.prev_ts[id] = now_ts;
     p.st.touched[id] = 0;
+#ifndef AB_UPDATING_NO_FLUSH_MARK  // measurement knob (tools/updating_state_rates.py): the flush without its store
+    p.st.flushed[id] = 1;
+#endif
+  }
+}
+
+// State export: every id flushed since the last export leaves as one row of its previous-flush snapshot (the values
+// the last flush emitted), compacted with one atomic per warp.
+struct UExport {
+  UState st;
+  const long long* id_keys;
+  unsigned long long n_ids;  // ids to scan: [0, n_ids)
+  long long* o_key;
+  unsigned long long* o_acc[MAX_ACC];
+  long long* o_ts;
+  unsigned int* count;
+};
+
+__global__ void __launch_bounds__(256) upd_export_kernel(const __grid_constant__ UExport p) {
+  unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  const unsigned int lane = threadIdx.x & 31;
+  for (; i < p.n_ids; i += stride) {
+    const bool mine = p.st.flushed[i] != 0;
+    const unsigned int active = __activemask();
+    const unsigned int mask = __ballot_sync(active, mine);
+    if (!mask) continue;
+    const int leader = __ffs(active) - 1;
+    unsigned int base = 0;
+    if ((int)lane == leader) base = atomicAdd(p.count, (unsigned int)__popc(mask));
+    base = __shfl_sync(active, base, leader);
+    if (!mine) continue;
+    const unsigned int o = base + __popc(mask & ((1u << lane) - 1u));
+    p.st.flushed[i] = 0;
+    p.o_key[o] = p.id_keys[i];
+    for (int a = 0; a < p.st.n_acc; ++a) p.o_acc[a][o] = p.st.prev[(unsigned long long)a * p.st.id_cap + i];
+    p.o_ts[o] = p.st.prev_ts[i];
+  }
+}
+
+// Restore: rows of table "a" in batch order, one thread per row.
+struct URestore {
+  UState st;
+  BDict dict;
+  const long long* key;
+  const unsigned long long* gen;
+  const unsigned long long* val[MAX_ACC];  // per accumulator; val[0] null: every row counts one
+  const long long* ts;
+  unsigned int* ids;              // per row
+  unsigned long long* best_gen;   // per id
+  long long* best_pos;            // per id, -1: no row
+  unsigned long long* overflow;   // rows whose bucket is out of ids
+  long long n;
+  int keyed;
+};
+
+__global__ void __launch_bounds__(256) upd_restore_insert_kernel(const __grid_constant__ URestore p) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < p.n; i += stride) {
+    const uint32_t id = p.keyed ? bd_lookup_or_insert(p.dict, p.key[i]) : 0u;
+    p.ids[i] = id;
+    if (id >= ID_OVERFLOW) atomicAdd(p.overflow, 1ull);
+  }
+}
+
+// the largest generation per id, then the last row of that generation
+__global__ void __launch_bounds__(256) upd_restore_gen_kernel(const __grid_constant__ URestore p) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < p.n; i += stride) atomicMax(p.best_gen + p.ids[i], p.gen[i]);
+}
+__global__ void __launch_bounds__(256) upd_restore_pos_kernel(const __grid_constant__ URestore p) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < p.n; i += stride) {
+    const unsigned int id = p.ids[i];
+    if (p.gen[i] == p.best_gen[id]) atomicMax(p.best_pos + id, i);
+  }
+}
+
+// the winning row seeds the live accumulators and the previous-flush snapshot alike
+__global__ void __launch_bounds__(256) upd_restore_seed_kernel(const __grid_constant__ URestore p) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < p.n; i += stride) {
+    const unsigned int id = p.ids[i];
+    if (p.best_pos[id] != i) continue;
+    for (int a = 0; a < p.st.n_acc; ++a) {
+      const unsigned long long v = p.val[a] ? p.val[a][i] : 1ull;
+      p.st.cur[(unsigned long long)a * p.st.id_cap + id] = v;
+      p.st.prev[(unsigned long long)a * p.st.id_cap + id] = v;
+    }
+    p.st.cur_ts[id] = p.ts[i];
+    p.st.prev_ts[id] = p.ts[i];
   }
 }
 
@@ -163,6 +268,7 @@ __global__ void upd_init_kernel(UState st, unsigned long long n) {
     st.cur_ts[i] = LLONG_MIN;
     st.prev_ts[i] = LLONG_MIN;
     st.touched[i] = 0;
+    st.flushed[i] = 0;
   }
 }
 
@@ -180,6 +286,7 @@ __global__ void upd_permute_kernel(UState o, UState n, const uint32_t* __restric
     n.cur_ts[m] = o.cur_ts[i];
     n.prev_ts[m] = o.prev_ts[i];
     n.touched[m] = o.touched[i];
+    n.flushed[m] = o.flushed[i];
   }
 }
 __global__ void upd_remap_list_kernel(unsigned int* list, unsigned int n, const uint32_t* __restrict__ map) {
@@ -191,9 +298,7 @@ class UpdatingAggOp final : public OpBase {
  public:
   explicit UpdatingAggOp(const ArroyoB200OpConfig& c);
   ~UpdatingAggOp() override;
-  void on_start(ArrowArray*, ArrowSchema*, int64_t n, int64_t, int64_t) override {
-    AB_REQUIRE(n == 0, ARROYO_B200_UNSUPPORTED, "updating aggregate: state restore (tables 'a' / 'b') is not implemented");
-  }
+  void on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t, int64_t) override;
   void process_batch(uint32_t, uint32_t, ArrowArray* batch, const ArrowSchema* schema) override;
   void process_device_batch(uint32_t, uint32_t, const uint64_t* cols, int32_t n_cols, int64_t n_rows) override;
   // watermarks pass through an updating aggregate untouched (it emits on ticks, incremental_aggregator.rs:990-1004)
@@ -203,6 +308,7 @@ class UpdatingAggOp final : public OpBase {
     if (end_of_data && out) flush_to(out);
   }
   void handle_tick(BatchesPriv* out) override { flush_to(out); }  // :994-1004
+  void checkpoint_state(BatchesPriv* out) override;
   void flush() override {
     set_device();
     AB_CUDA(cudaStreamSynchronize(stream_));
@@ -228,7 +334,7 @@ class UpdatingAggOp final : public OpBase {
   uint64_t n_buckets_ = 1, id_cap_ = 0;
   uint32_t total_keys_ = 0;
   DevBuf slots_, bucket_nkeys_, id_keys_, n_total_;
-  DevBuf cur_, prev_, cur_ts_, prev_ts_, touched_, list_, counters_;  // counters_: [n_touched, retractions, appends, pad] u32 + deferred u64
+  DevBuf cur_, prev_, cur_ts_, prev_ts_, touched_, flushed_, list_, counters_;  // counters_: [n_touched, retractions, appends, pad] u32 + deferred u64
   DevBuf staging_;
   uint64_t staging_cap_ = 0;
   // deferred rows (key, ts, values): two sets, one re-ingested while the other takes the rows that defer again
@@ -237,7 +343,22 @@ class UpdatingAggOp final : public OpBase {
   int defer_cur_ = 0;
   uint64_t out_cap_ = 0;
   DevBuf o_key_, o_ts_, o_agg_[ARROYO_B200_MAX_AGGS];
+  // state export: keys flushed since the last export (an upper bound: a key flushed twice counts twice), the
+  // generation the next export writes, and the export's output buffers
+  uint64_t unexported_ = 0, generation_ = 0, state_cap_ = 0;
+  bool restored_ = false;
+  DevBuf s_key_, s_ts_, s_acc_[MAX_ACC];
   ArroyoB200Stats st_{};
+
+  // One column of table "a" after the key: its Arrow format and what it holds.
+  enum StateRole { S_ROWS, S_ACC, S_TS, S_GEN };
+  struct StateCol {
+    const char* format;
+    int role;
+    int acc;         // S_ACC: the accumulator
+    bool count_star;  // S_ROWS: the COUNT(*) aggregate's own column
+  };
+  std::vector<StateCol> state_layout() const;
 
   BDict dict_view() const;
   UState state_view() const;
@@ -286,6 +407,7 @@ UState UpdatingAggOp::state_view() const {
   s.cur_ts = cur_ts_.as<long long>();
   s.prev_ts = prev_ts_.as<long long>();
   s.touched = touched_.as<unsigned int>();
+  s.flushed = flushed_.as<unsigned char>();
   s.list = list_.as<unsigned int>();
   s.n_touched = counters_.as<unsigned int>();
   s.id_cap = id_cap_;
@@ -316,6 +438,7 @@ void UpdatingAggOp::alloc_state(uint64_t n_buckets) {
   cur_ts_.alloc(id_cap_ * 8);
   prev_ts_.alloc(id_cap_ * 8);
   touched_.alloc(id_cap_ * 4);
+  flushed_.alloc(id_cap_);
   list_.alloc(id_cap_ * 4);
   upd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(state_view(), id_cap_);
   AB_CUDA(cudaGetLastError());
@@ -333,7 +456,7 @@ void UpdatingAggOp::grow() {
   const uint64_t old_cap = id_cap_;
   DevBuf k_slots = std::move(slots_), k_nk = std::move(bucket_nkeys_), k_keys = std::move(id_keys_), k_cur = std::move(cur_),
          k_prev = std::move(prev_), k_cts = std::move(cur_ts_), k_pts = std::move(prev_ts_), k_t = std::move(touched_),
-         k_list = std::move(list_);
+         k_f = std::move(flushed_), k_list = std::move(list_);
   unsigned int h_touched = 0;
   AB_CUDA(cudaMemcpyAsync(&h_touched, counters_.p, 4, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaMemsetAsync(n_total_.p, 0, 4, stream_));
@@ -493,6 +616,7 @@ void UpdatingAggOp::flush_to(BatchesPriv* out) {
   AB_CUDA(cudaStreamSynchronize(stream_));
   const unsigned int n = h.touched;
   if (n == 0 || !out) return;
+  unexported_ += n;
   if (2ull * n > out_cap_) {
     out_cap_ = std::max<uint64_t>(2ull * n, 1024);
     o_key_.alloc(out_cap_ * 8);
@@ -554,6 +678,228 @@ void UpdatingAggOp::flush_to(BatchesPriv* out) {
   out->arrays.emplace_back();
   out->schemas.emplace_back();
   export_batch(cols, total, &out->arrays.back(), &out->schemas.back());
+}
+
+
+// Table "a" after the key column (sliding_state_schema, :1083-1160): per aggregate in plan order the state of its
+// sliding accumulator -- count(*) [count: Int64], sum [sum: Int64, count: UInt64], avg [count: UInt64, sum: Float64],
+// min [min: Int64], max [max: Int64] -- then the trailing max(_timestamp) aggregate's state as `_timestamp` and the
+// generation.  Every count column holds the key's row count.
+std::vector<UpdatingAggOp::StateCol> UpdatingAggOp::state_layout() const {
+  std::vector<StateCol> l;
+  for (int g = 0; g < plan_.n_aggs; ++g) {
+    const int acc = plan_.agg_acc[g];
+    switch (plan_.agg_kind[g]) {
+      case ARROYO_B200_AGG_COUNT_STAR: l.push_back({"l", S_ROWS, 0, true}); break;
+      case ARROYO_B200_AGG_SUM_I64:
+        l.push_back({"l", S_ACC, acc, false});
+        l.push_back({"L", S_ROWS, 0, false});
+        break;
+      case ARROYO_B200_AGG_AVG_I64:
+        l.push_back({"L", S_ROWS, 0, false});
+        l.push_back({"g", S_ACC, acc, false});
+        break;
+      default: l.push_back({"l", S_ACC, acc, false}); break;  // min / max
+    }
+  }
+  l.push_back({"tsn:", S_TS, 0, false});
+  l.push_back({"L", S_GEN, 0, false});
+  return l;
+}
+
+// checkpoint_sliding (:272-340): one batch of table "a" with the keys flushed since the last call, or nothing.
+void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
+  set_device();
+  if (unexported_ == 0) return;
+  const uint64_t n_ids = plan_.keyed ? BD_ID_BASE + n_buckets_ * BD_CAPB : 1;
+  const uint64_t cap = std::min<uint64_t>(unexported_, n_ids);
+  if (cap > state_cap_) {
+    state_cap_ = std::max<uint64_t>(cap, 1024);
+    s_key_.alloc(state_cap_ * 8);
+    s_ts_.alloc(state_cap_ * 8);
+    for (int a = 0; a < plan_.n_acc; ++a) s_acc_[a].alloc(state_cap_ * 8);
+  }
+  unsigned int* count = reinterpret_cast<unsigned int*>((char*)counters_.p + 24);
+  AB_CUDA(cudaMemsetAsync(count, 0, 4, stream_));
+  UExport p{};
+  p.st = state_view();
+  p.id_keys = id_keys_.as<long long>();
+  p.n_ids = n_ids;
+  p.o_key = s_key_.as<long long>();
+  for (int a = 0; a < plan_.n_acc; ++a) p.o_acc[a] = s_acc_[a].as<unsigned long long>();
+  p.o_ts = s_ts_.as<long long>();
+  p.count = count;
+  const int grid = (int)std::min<uint64_t>((n_ids + 255) / 256, (uint64_t)num_sms_ * 8);
+  upd_export_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  unsigned int rows = 0;
+  AB_CUDA(cudaMemcpyAsync(&rows, count, 4, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  unexported_ = 0;
+  if (rows == 0) return;
+  std::vector<OutColumn> cols;
+  auto column = [&](const std::string& name, const std::string& format, const void* dev) {
+    OutColumn c;
+    c.name = name;
+    c.format = format;
+    c.data = d2h_pinned(dev, (size_t)rows * 8, stream_, &st_.d2h_bytes);
+    cols.push_back(c);
+  };
+  if (plan_.keyed) column("key", key_format_, s_key_.p);
+  const std::vector<StateCol> layout = state_layout();
+  for (size_t j = 0; j < layout.size(); ++j) {
+    const StateCol& sc = layout[j];
+    const std::string name = "state" + std::to_string(j);
+    if (sc.role == S_GEN) {
+      OutColumn c;
+      c.name = "_generation";
+      c.format = sc.format;
+      uint64_t* g = (uint64_t*)PinnedPool::get().alloc((size_t)rows * 8);
+      std::fill(g, g + rows, (uint64_t)generation_);
+      c.data = g;
+      cols.push_back(c);
+    } else if (sc.role == S_TS) {
+      column("_timestamp", sc.format, s_ts_.p);
+    } else {
+      column(name, sc.format, s_acc_[sc.role == S_ROWS ? 0 : sc.acc].p);
+    }
+  }
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  ++generation_;
+  out->arrays.emplace_back();
+  out->schemas.emplace_back();
+  export_batch(cols, rows, &out->arrays.back(), &out->schemas.back());
+}
+
+// initialize (:446-503): the batches of table "a", in any order and with any number of rows per key.
+void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t, int64_t) {
+  if (n <= 0) return;
+  AB_REQUIRE(state != nullptr && schemas != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null state batches");
+  AB_REQUIRE(st_.rows_in == 0 && !restored_, ARROYO_B200_INVALID_ARGUMENT,
+             "updating aggregate: restore into an operator that already holds rows or restored state");
+  // every batch is checked before anything changes
+  const std::vector<StateCol> layout = state_layout();
+  const int kc = plan_.keyed ? 1 : 0;
+  std::vector<std::vector<InColumn>> batches((size_t)n);
+  std::vector<int64_t> rows((size_t)n, 0);
+  int64_t total = 0;
+  for (int64_t b = 0; b < n; ++b) {
+    try {
+      batches[b] = import_batch(&state[b], &schemas[b], &rows[b]);
+    } catch (const Error& e) {
+      throw Error(ARROYO_B200_INVALID_ARGUMENT, std::string("state batch: ") + e.what());
+    }
+    const std::vector<InColumn>& cols = batches[b];
+    AB_REQUIRE(cols.size() == (size_t)kc + layout.size(), ARROYO_B200_INVALID_ARGUMENT,
+               "state batch does not have the columns of table 'a' for this plan");
+    if (plan_.keyed) {
+      const std::string& f = cols[0].format;
+      AB_REQUIRE(f == "l" || f == "L" || f.compare(0, 4, "tsn:") == 0, ARROYO_B200_INVALID_ARGUMENT,
+                 "state batch: key of type '" + f + "' (supported: l, L, tsn:)");
+    }
+    for (size_t j = 0; j < layout.size(); ++j) {
+      const std::string& f = cols[kc + j].format;
+      const std::string want = layout[j].format;
+      const bool ok = want == "tsn:" ? f.compare(0, 4, "tsn:") == 0 : f == want;
+      AB_REQUIRE(ok, ARROYO_B200_INVALID_ARGUMENT,
+                 "state batch: column " + std::to_string(kc + j) + " has type '" + f + "', table 'a' has '" + want + "'");
+    }
+    total += rows[b];
+  }
+  if (total == 0) return;
+  // which column seeds each accumulator: the row count from COUNT(*), else from a SUM's or AVG's count, else 1
+  int rows_col = -1, ts_col = -1, gen_col = -1, acc_col[MAX_ACC];
+  for (int a = 0; a < MAX_ACC; ++a) acc_col[a] = -1;
+  for (size_t j = 0; j < layout.size(); ++j) {
+    const StateCol& sc = layout[j];
+    const int c = kc + (int)j;
+    if (sc.role == S_ROWS && (rows_col < 0 || (sc.count_star && !layout[rows_col - kc].count_star))) rows_col = c;
+    if (sc.role == S_ACC && acc_col[sc.acc] < 0) acc_col[sc.acc] = c;
+    if (sc.role == S_TS) ts_col = c;
+    if (sc.role == S_GEN) gen_col = c;
+  }
+  acc_col[0] = rows_col;
+  set_device();
+  if (plan_.keyed) {
+    key_format_ = batches[0][0].format;
+    const uint64_t b = bd_buckets_for((uint64_t)total);  // the dictionary holds every restored key without growing
+    if (b > n_buckets_) alloc_state(b);
+  }
+  // the columns of every batch, concatenated in batch order: a row's position is its index
+  auto upload = [&](int c, DevBuf& dst) {
+    dst.alloc((size_t)total * 8);
+    int64_t off = 0;
+    for (int64_t b = 0; b < n; ++b) {
+      if (rows[b])
+        AB_CUDA(cudaMemcpyAsync((char*)dst.p + off * 8, batches[b][c].data, (size_t)rows[b] * 8, cudaMemcpyHostToDevice,
+                                stream_));
+      off += rows[b];
+    }
+    st_.h2d_bytes += (uint64_t)total * 8;
+  };
+  DevBuf d_key, d_gen, d_ts, d_val[MAX_ACC];
+  if (plan_.keyed) upload(0, d_key);
+  upload(gen_col, d_gen);
+  upload(ts_col, d_ts);
+  URestore p{};
+  for (int a = 0; a < plan_.n_acc; ++a) {
+    if (acc_col[a] < 0) continue;
+    upload(acc_col[a], d_val[a]);
+    p.val[a] = d_val[a].as<unsigned long long>();
+  }
+  uint64_t max_gen = 0;
+  for (int64_t b = 0; b < n; ++b)
+    for (int64_t i = 0; i < rows[b]; ++i) max_gen = std::max<uint64_t>(max_gen, batches[b][gen_col].data[i]);
+  DevBuf ids((size_t)total * 4), overflow(8);
+  p.key = d_key.as<long long>();
+  p.gen = d_gen.as<unsigned long long>();
+  p.ts = d_ts.as<long long>();
+  p.ids = ids.as<unsigned int>();
+  p.overflow = overflow.as<unsigned long long>();
+  p.n = total;
+  p.keyed = plan_.keyed ? 1 : 0;
+  const int grid = std::max(1, (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms_ * 8));
+  // keys whose bucket is out of ids: the dictionary doubles and every row looks its key up again (placed keys keep
+  // theirs).  A dictionary sized for few rows has few buckets, each covering a wide hash range, so crowded keys may
+  // need several doublings to split: below the default size (2^16 keys) it doubles freely; from there on,
+  // RESTORE_STALLS doublings in a row that place none of the rest give up
+  constexpr int RESTORE_STALLS = 4;
+  const uint64_t free_buckets = bd_buckets_for(1ull << 16);
+  for (uint64_t left = UINT64_MAX, stalls = 0;;) {
+    p.dict = dict_view();
+    AB_CUDA(cudaMemsetAsync(overflow.p, 0, 8, stream_));
+    upd_restore_insert_kernel<<<grid, 256, 0, stream_>>>(p);
+    AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
+    unsigned long long over = 0;
+    AB_CUDA(cudaMemcpyAsync(&over, overflow.p, 8, cudaMemcpyDeviceToHost, stream_));
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    if (over == 0) break;
+    stalls = over < left || n_buckets_ < free_buckets ? 0 : stalls + 1;
+    left = over;
+    AB_REQUIRE(stalls < RESTORE_STALLS, ARROYO_B200_RUNTIME,
+               "updating aggregate: restored keys whose dictionary bucket is out of ids still do not fit after the "
+               "dictionary grew");
+    grow();
+  }
+  p.st = state_view();
+  DevBuf best_gen(id_cap_ * 8), best_pos(id_cap_ * 8);
+  AB_CUDA(cudaMemsetAsync(best_gen.p, 0, id_cap_ * 8, stream_));
+  AB_CUDA(cudaMemsetAsync(best_pos.p, 0xFF, id_cap_ * 8, stream_));  // -1
+  p.best_gen = best_gen.as<unsigned long long>();
+  p.best_pos = best_pos.as<long long>();
+  upd_restore_gen_kernel<<<grid, 256, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  upd_restore_pos_kernel<<<grid, 256, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  upd_restore_seed_kernel<<<grid, 256, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  st_.kernel_launches += 3;
+  AB_CUDA(cudaMemcpyAsync(&total_keys_, n_total_.p, 4, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  generation_ = max_gen + 1;
+  restored_ = true;
 }
 
 }  // namespace

@@ -524,7 +524,10 @@ class UpdatingAggregatingFunc(_NativeOperator):
     """arroyo-worker/src/arrow/incremental_aggregator.rs (`IncrementalAggregatingFunc`): the non-windowed GROUP BY.
     Change rows leave on ticks (`tick_interval` = flush interval, :990-1004), at checkpoints (:951-961) and at end of
     data (:1006-1018): [key cols..., aggregates..., _timestamp, _is_retract].  `config`: anything with `key_names`
-    and `aggs` (oracle.updating_oracle.UpdatingAggConfig has the shape).  Append-only inputs only."""
+    and `aggs` (oracle.updating_oracle.UpdatingAggConfig has the shape).  Append-only inputs only.
+
+    State: a checkpoint also writes the accumulators of the keys flushed since the last checkpoint to the key-value
+    table "a" (`state_names()` columns, :619-635), and `on_start` restores them from it (:446-503)."""
     kind = ffi.UPDATING_AGGREGATE
     IS_RETRACT = "_is_retract"
 
@@ -545,7 +548,36 @@ class UpdatingAggregatingFunc(_NativeOperator):
             self._key_type = schema.field(self.config.key_names[0]).type
 
     def tables(self):
-        return {"a": 0, "b": 0}  # accumulator state / batch state (:963-988): restore is not implemented
+        # accumulator state / batch state (:963-988); "b" (count(distinct ...)) stays empty: such plans are refused
+        return {"a": 0, "b": 0}
+
+    def state_names(self) -> List[str]:
+        """Columns of table "a": keys, each aggregate's accumulator state, `_timestamp`, `_generation`."""
+        names = list(self.config.key_names)
+        fields = {"count": ["count"], "sum": ["sum", "count"], "avg": ["count", "sum"], "min": ["min"], "max": ["max"]}
+        for a in self.config.aggs:
+            names += [f"{a.name}[{f}]" for f in fields[a.kind]]
+        return names + [TIMESTAMP, "_generation"]
+
+    def on_start(self, ctx: OperatorContext):
+        batches = list(ctx.key_value_table("a").get_all())
+        if not batches:
+            return
+        if not self.created:
+            raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "restore needs input_schema at construction")
+        n = len(batches)
+        arrs = (ffi.ArrowArray * n)()
+        schs = (ffi.ArrowSchema * n)()
+        for i, b in enumerate(batches):
+            b._export_to_c(C.addressof(arrs[i]), C.addressof(schs[i]))
+        try:
+            st = self._lib.arroyo_b200_op_on_start(self._h, arrs, schs, n, ffi.INT64_MIN, ffi.INT64_MIN)
+        finally:
+            # the library copies the state during the call: the exported structs stay ours
+            for s in list(arrs) + list(schs):
+                if s.release:
+                    C.CFUNCTYPE(None, C.c_void_p)(s.release)(C.addressof(s))
+        _check(self._lib, self._h, st)
 
     def _build(self, names: List[str]):
         c = self.config
@@ -596,14 +628,19 @@ class UpdatingAggregatingFunc(_NativeOperator):
     def handle_watermark(self, watermark, ctx: OperatorContext, collector: Collector):
         return watermark
 
-    def _emit(self, out, collector: Collector):
-        names = self.output_names()
+    def _typed(self, out, names) -> List[pa.RecordBatch]:
+        res = []
         for b in import_batches(self._lib, out):
             cols = b.columns
             # device batches carry no Arrow types: the key column leaves with the input schema's key type
             if self._key_type is not None and cols[0].type != self._key_type:
                 cols = [cols[0].view(self._key_type)] + cols[1:]
-            collector.collect(pa.RecordBatch.from_arrays(cols, names=names))
+            res.append(pa.RecordBatch.from_arrays(cols, names=names))
+        return res
+
+    def _emit(self, out, collector: Collector):
+        for b in self._typed(out, self.output_names()):
+            collector.collect(b)
 
     def handle_tick(self, tick, ctx: OperatorContext, collector: Collector):
         if not self.created:
@@ -618,6 +655,16 @@ class UpdatingAggregatingFunc(_NativeOperator):
         out = ffi.Batches()
         _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_checkpoint(self._h, ffi.INT64_MIN, C.byref(out)))
         self._emit(out, collector)
+        if ctx is not None:  # then the state of the keys flushed since the last checkpoint (:951-961)
+            self.checkpoint_state(ctx.key_value_table("a"))
+
+    def checkpoint_state(self, table):
+        """arroyo_b200_op_checkpoint_state: inserts the state rows of the keys flushed since the last call into
+        `table` (a KeyValueTable)."""
+        out = ffi.Batches()
+        _check(self._lib, self._h, self._lib.arroyo_b200_op_checkpoint_state(self._h, C.byref(out)))
+        for b in self._typed(out, self.state_names()):
+            table.insert_batch(b)
 
     def on_close(self, final_message, ctx: OperatorContext, collector: Collector):
         if not self.created:

@@ -271,7 +271,16 @@ const char* arroyo_b200_op_name(const ArroyoB200Op* op);
  * ExpiringTimeKeyView::all_batches_for_watermark, arroyo-state/src/tables/expiring_time_key_map.rs:858-872;
  * sliding_aggregating_window.rs:556-595, tumbling :228-248).  `n == 0` = fresh start.
  * `watermark_ns` = ctx.last_present_watermark() or INT64_MIN when there is none.
- * `table_min_time_ns` = ExpiringTimeKeyView::get_min_time() or INT64_MIN. */
+ * `table_min_time_ns` = ExpiringTimeKeyView::get_min_time() or INT64_MIN.
+ * Updating aggregate (incremental_aggregator.rs:446-503): `state` holds every batch of table "a"
+ * (UncachedKeyValueView::get_all, in any order, not de-duplicated), in the layout
+ * arroyo_b200_op_checkpoint_state writes; both time arguments are ignored.  Per key the row with the
+ * largest `_generation` wins, a tie going to the later row (batch order, then row order); it seeds the
+ * accumulators and the values the next flush retracts.  The dictionary is sized from the row count and
+ * grows when a bucket runs out of ids; keys that still cannot be placed => ARROYO_B200_RUNTIME.
+ * ARROYO_B200_INVALID_ARGUMENT, with nothing changed: a column count or type that is not the plan's
+ * layout, or an operator that has already taken rows or been restored.  Restored rows do not count in
+ * `rows_in`; their keys count in `n_keys`. */
 int32_t arroyo_b200_op_on_start(ArroyoB200Op* op, struct ArrowArray* state, struct ArrowSchema* schemas,
                                 int64_t n, int64_t watermark_ns, int64_t table_min_time_ns);
 
@@ -366,6 +375,17 @@ int32_t arroyo_b200_op_handle_watermark_device_poll(ArroyoB200Op* op, ArroyoB200
  * ExpiringTimeKeyView::insert(pane_start, batch) and flushes.  `watermark_ns` = ctx.watermark()
  * if it is an event time, else INT64_MIN. */
 int32_t arroyo_b200_op_handle_checkpoint(ArroyoB200Op* op, int64_t watermark_ns, ArroyoB200Batches* state_out);
+
+/* The updating aggregate's accumulator table "a" (incremental_aggregator.rs:619-635, checkpoint_sliding
+ * :272-340): one batch with the latest state of every key flushed since the previous call, or no batch.
+ * The shim calls it after handle_checkpoint and inserts the batches with
+ * UncachedKeyValueView::insert_batch.  Columns: [key (the input key's type), per aggregate in plan
+ * order: count(*) -> count Int64; sum -> sum Int64 (wrapping), count UInt64; avg -> count UInt64,
+ * sum Float64; min -> min Int64; max -> max Int64; then _timestamp Timestamp(ns) = max(_timestamp),
+ * _generation UInt64].  The unkeyed plan has no key column.  Every row of one call carries the same
+ * generation, larger than any the operator wrote or restored before.  State rows count in no statistic
+ * but `d2h_bytes`.  Every other operator kind returns no batches. */
+int32_t arroyo_b200_op_checkpoint_state(ArroyoB200Op* op, ArroyoB200Batches* state_out);
 
 /* ArrowOperator::on_close(final_message, ctx, collector) (operator.rs:1247-1256). */
 int32_t arroyo_b200_op_on_close(ArroyoB200Op* op, int32_t end_of_data, ArroyoB200Batches* out);
