@@ -2,6 +2,7 @@
 // reference interfaces each one replaces).  Nothing unwinds across this boundary.
 #include <algorithm>
 #include <chrono>
+#include <memory>
 #include <new>
 
 #include "op.h"
@@ -43,6 +44,39 @@ int32_t guarded(ArroyoB200Op* op, F&& f) {
   } catch (...) {
     op->impl->last_error = "unknown C++ exception";
     return ARROYO_B200_RUNTIME;
+  }
+}
+
+// An entry point that hands back an ArroyoB200Batches: `out` starts zeroed, and `f(o, priv)` emits into a fresh
+// BatchesPriv that `out` takes when the call succeeds and that is thrown away when it fails.  A null `out` is refused
+// unless `null_out_ok` (on_close), which throws the batches away too.  `timer`: the handle's wall-time counter the
+// call adds to, or null.
+template <class F>
+int32_t emit_batches(ArroyoB200Op* op, ArroyoB200Batches* out, F&& f, double ArroyoB200Op::*timer = nullptr,
+                     bool null_out_ok = false) {
+  if (out) memset(out, 0, sizeof *out);
+  if (!op) return ARROYO_B200_INVALID_ARGUMENT;
+  double untimed = 0;
+  WallTimer wt(timer ? op->*timer : untimed);
+  return guarded(op, [&](OpBase* o) {
+    AB_REQUIRE(out != nullptr || null_out_ok, ARROYO_B200_INVALID_ARGUMENT, "null out");
+    std::unique_ptr<BatchesPriv, void (*)(BatchesPriv*)> priv(new BatchesPriv(), discard);
+    f(o, priv.get());
+    if (out) batches_finish(priv.release(), out);
+  });
+}
+
+// Begins an emission into a fresh `pending_out`.  When that fails, the copies it enqueued are waited for and its
+// batches thrown away: nothing half-emitted stays pending.
+void begin_emission(OpBase* o, int64_t watermark_ns) {
+  o->pending_out = new BatchesPriv();
+  try {
+    o->begin_watermark(watermark_ns);
+  } catch (...) {
+    o->poll_watermark(true);
+    discard(o->pending_out);
+    o->pending_out = nullptr;
+    throw;
   }
 }
 
@@ -140,9 +174,7 @@ void arroyo_b200_op_destroy(ArroyoB200Op* op) {
     if (op->impl && op->impl->pending_out) {
       // an emission that was begun and never collected: wait for its copies, give the buffers back
       op->impl->poll_watermark(true);
-      ArroyoB200Batches tmp{};
-      batches_finish(op->impl->pending_out, &tmp);
-      batches_release(&tmp);
+      discard(op->impl->pending_out);
       op->impl->pending_out = nullptr;
     }
     delete op->impl;
@@ -175,22 +207,9 @@ int32_t arroyo_b200_op_process_batch(ArroyoB200Op* op, uint32_t input_index, uin
 
 int32_t arroyo_b200_op_process_batch_emit(ArroyoB200Op* op, uint32_t input_index, uint32_t in_partitions,
                                           struct ArrowArray* batch, const struct ArrowSchema* schema, ArroyoB200Batches* out) {
-  if (out) memset(out, 0, sizeof *out);
-  if (!op) return ARROYO_B200_INVALID_ARGUMENT;
-  WallTimer wt(op->host_process_ms);
-  return guarded(op, [&](OpBase* o) {
-    AB_REQUIRE(out != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null out");
-    auto* priv = new BatchesPriv();
-    try {
-      o->process_batch_emit(input_index, in_partitions, batch, schema, priv);
-    } catch (...) {
-      ArroyoB200Batches tmp{};
-      batches_finish(priv, &tmp);
-      batches_release(&tmp);
-      throw;
-    }
-    batches_finish(priv, out);
-  });
+  return emit_batches(
+      op, out, [&](OpBase* o, BatchesPriv* b) { o->process_batch_emit(input_index, in_partitions, batch, schema, b); },
+      &ArroyoB200Op::host_process_ms);
 }
 
 int32_t arroyo_b200_op_process_device_batch(ArroyoB200Op* op, uint32_t input_index, uint32_t in_partitions,
@@ -215,39 +234,13 @@ int32_t arroyo_b200_op_process_device_batches(ArroyoB200Op* op, uint32_t input_i
 }
 
 int32_t arroyo_b200_op_handle_watermark(ArroyoB200Op* op, int64_t watermark_ns, ArroyoB200Batches* out) {
-  if (out) memset(out, 0, sizeof *out);
-  if (!op) return ARROYO_B200_INVALID_ARGUMENT;
-  WallTimer wt(op->host_watermark_ms);
-  return guarded(op, [&](OpBase* o) {
-    AB_REQUIRE(out != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null out");
-    auto* priv = new BatchesPriv();
-    try {
-      o->handle_watermark(watermark_ns, priv, nullptr);
-    } catch (...) {
-      ArroyoB200Batches tmp{};
-      batches_finish(priv, &tmp);
-      batches_release(&tmp);
-      throw;
-    }
-    batches_finish(priv, out);
-  });
+  return emit_batches(
+      op, out, [&](OpBase* o, BatchesPriv* b) { o->handle_watermark(watermark_ns, b, nullptr); },
+      &ArroyoB200Op::host_watermark_ms);
 }
 
 int32_t arroyo_b200_op_handle_tick(ArroyoB200Op* op, ArroyoB200Batches* out) {
-  if (out) memset(out, 0, sizeof *out);
-  return guarded(op, [&](OpBase* o) {
-    AB_REQUIRE(out != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null out");
-    auto* priv = new BatchesPriv();
-    try {
-      o->handle_tick(priv);
-    } catch (...) {
-      ArroyoB200Batches tmp{};
-      batches_finish(priv, &tmp);
-      batches_release(&tmp);
-      throw;
-    }
-    batches_finish(priv, out);
-  });
+  return emit_batches(op, out, [&](OpBase* o, BatchesPriv* b) { o->handle_tick(b); });
 }
 
 int32_t arroyo_b200_op_handle_watermark_begin(ArroyoB200Op* op, int64_t watermark_ns) {
@@ -256,17 +249,7 @@ int32_t arroyo_b200_op_handle_watermark_begin(ArroyoB200Op* op, int64_t watermar
   return guarded(op, [&](OpBase* o) {
     AB_REQUIRE(o->pending_out == nullptr, ARROYO_B200_INVALID_ARGUMENT,
                "the previous emission has not been collected (handle_watermark_poll)");
-    o->pending_out = new BatchesPriv();
-    try {
-      o->begin_watermark(watermark_ns);
-    } catch (...) {
-      o->poll_watermark(true);
-      ArroyoB200Batches tmp{};
-      batches_finish(o->pending_out, &tmp);
-      batches_release(&tmp);
-      o->pending_out = nullptr;
-      throw;
-    }
+    begin_emission(o, watermark_ns);
   });
 }
 
@@ -320,32 +303,16 @@ int32_t arroyo_b200_op_run_batches(ArroyoB200Op* op, struct ArrowArray* batches,
       }
       if (async_emit) {
         collect(true);  // windows leave in order: the previous emission first
-        o->pending_out = new BatchesPriv();
-        try {
-          o->begin_watermark(wm);
-        } catch (...) {
-          // same clean-up as arroyo_b200_op_handle_watermark_begin: nothing half-emitted stays pending
-          o->poll_watermark(true);
-          ArroyoB200Batches tmp{};
-          batches_finish(o->pending_out, &tmp);
-          batches_release(&tmp);
-          o->pending_out = nullptr;
-          throw;
-        }
+        begin_emission(o, wm);
       } else {
         o->handle_watermark(wm, acc, nullptr);
       }
     }
     if (async_emit) collect(false);
   });
-  if (out) {
-    batches_finish(acc, out);
-  } else {
-    // null `out` was rejected above: drop whatever was accumulated instead of writing through it
-    ArroyoB200Batches tmp{};
-    batches_finish(acc, &tmp);
-    batches_release(&tmp);
-  }
+  // a null `out` was rejected above: whatever was accumulated is dropped instead of written through it
+  if (out) batches_finish(acc, out);
+  else discard(acc);
   return st;
 }
 
@@ -390,59 +357,15 @@ int32_t arroyo_b200_op_handle_watermark_device_poll(ArroyoB200Op* op, ArroyoB200
 }
 
 int32_t arroyo_b200_op_handle_checkpoint(ArroyoB200Op* op, int64_t watermark_ns, ArroyoB200Batches* state_out) {
-  if (state_out) memset(state_out, 0, sizeof *state_out);
-  return guarded(op, [&](OpBase* o) {
-    AB_REQUIRE(state_out != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null out");
-    auto* priv = new BatchesPriv();
-    try {
-      o->handle_checkpoint(watermark_ns, priv);
-    } catch (...) {
-      ArroyoB200Batches tmp{};
-      batches_finish(priv, &tmp);
-      batches_release(&tmp);
-      throw;
-    }
-    batches_finish(priv, state_out);
-  });
+  return emit_batches(op, state_out, [&](OpBase* o, BatchesPriv* b) { o->handle_checkpoint(watermark_ns, b); });
 }
 
 int32_t arroyo_b200_op_checkpoint_state(ArroyoB200Op* op, ArroyoB200Batches* state_out) {
-  if (state_out) memset(state_out, 0, sizeof *state_out);
-  return guarded(op, [&](OpBase* o) {
-    AB_REQUIRE(state_out != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null out");
-    auto* priv = new BatchesPriv();
-    try {
-      o->checkpoint_state(priv);
-    } catch (...) {
-      ArroyoB200Batches tmp{};
-      batches_finish(priv, &tmp);
-      batches_release(&tmp);
-      throw;
-    }
-    batches_finish(priv, state_out);
-  });
+  return emit_batches(op, state_out, [&](OpBase* o, BatchesPriv* b) { o->checkpoint_state(b); });
 }
 
 int32_t arroyo_b200_op_on_close(ArroyoB200Op* op, int32_t end_of_data, ArroyoB200Batches* out) {
-  if (out) memset(out, 0, sizeof *out);
-  return guarded(op, [&](OpBase* o) {
-    auto* priv = new BatchesPriv();
-    try {
-      o->on_close(end_of_data, priv);
-    } catch (...) {
-      ArroyoB200Batches tmp{};
-      batches_finish(priv, &tmp);
-      batches_release(&tmp);
-      throw;
-    }
-    if (out) {
-      batches_finish(priv, out);
-    } else {
-      ArroyoB200Batches tmp{};
-      batches_finish(priv, &tmp);
-      batches_release(&tmp);
-    }
-  });
+  return emit_batches(op, out, [&](OpBase* o, BatchesPriv* b) { o->on_close(end_of_data, b); }, nullptr, true);
 }
 
 int32_t arroyo_b200_op_flush(ArroyoB200Op* op) {

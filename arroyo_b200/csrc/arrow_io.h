@@ -288,18 +288,66 @@ inline void export_window_batch(BatchesPriv* out, int64_t n, cudaStream_t s, uin
   export_batch(cols, n, &out->arrays.back(), &out->schemas.back());
 }
 
-inline void batches_release(ArroyoB200Batches* b) {
-  if (!b || !b->private_data) return;
-  auto* p = (BatchesPriv*)b->private_data;
+// Releases every batch of `p`, and `p` itself: batches that never reach the caller.
+inline void discard(BatchesPriv* p) {
   for (auto& a : p->arrays)
     if (a.release) a.release(&a);
   for (auto& s : p->schemas)
     if (s.release) s.release(&s);
   delete p;
+}
+
+inline void batches_release(ArroyoB200Batches* b) {
+  if (!b || !b->private_data) return;
+  discard((BatchesPriv*)b->private_data);
   b->n_batches = 0;
   b->arrays = nullptr;
   b->schemas = nullptr;
   b->private_data = nullptr;
 }
+
+// Host input batches the library has taken and holds until the stream has passed the copies that read them.  The
+// owner drains its stream before this is destroyed, which releases whatever is still held.
+class HeldInputs {
+ public:
+  HeldInputs() = default;
+  HeldInputs(const HeldInputs&) = delete;
+  HeldInputs& operator=(const HeldInputs&) = delete;
+  ~HeldInputs() {
+    for (auto& h : held_) {
+      if (h.second.release) h.second.release(&h.second);
+      cudaEventDestroy(h.first);
+    }
+  }
+
+  // Takes `batch` (its `release` is set to NULL) until `s` has passed the work enqueued on it so far.
+  void hold(ArrowArray* batch, cudaStream_t s) {
+    cudaEvent_t ev;
+    AB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    AB_CUDA(cudaEventRecord(ev, s));
+    held_.emplace_back(ev, *batch);
+    batch->release = nullptr;
+  }
+
+  // Releases, in the order they were taken, the batches whose copies have completed; with `wait`, all of them.
+  void release(bool wait) {
+    while (!held_.empty()) {
+      auto& h = held_.front();
+      if (wait) {
+        AB_CUDA(cudaEventSynchronize(h.first));
+      } else {
+        const cudaError_t e = cudaEventQuery(h.first);
+        if (e == cudaErrorNotReady) break;
+        AB_CUDA(e);
+      }
+      if (h.second.release) h.second.release(&h.second);
+      cudaEventDestroy(h.first);
+      held_.erase(held_.begin());
+    }
+  }
+
+ private:
+  std::vector<std::pair<cudaEvent_t, ArrowArray>> held_;
+};
 
 }  // namespace ab

@@ -234,7 +234,7 @@ class InstantJoinOp final : public OpBase {
   void flush() override {
     set_device();
     AB_CUDA(cudaStreamSynchronize(stream_));
-    release_inputs();
+    inputs_.release(true);
   }
   void stats(ArroyoB200Stats* out) override { *out = st_; }
 
@@ -249,10 +249,9 @@ class InstantJoinOp final : public OpBase {
   std::vector<DevBuf> out_cols_;
   std::vector<DevBuf> out_valid_;
   DevBuf out_ts_;
-  std::vector<std::pair<cudaEvent_t, ArrowArray>> pending_;
+  HeldInputs inputs_;  // host batches whose copies to the side columns may still run
   ArroyoB200Stats st_{};
 
-  void release_inputs();
   void reserve(Side& s, int64_t extra);
   void append(Side& s, const uint64_t* const* cols, int64_t n, bool host);
   int grid_for(int64_t n) const { return (int)std::max<int64_t>(1, std::min<int64_t>((n + JT - 1) / JT, (int64_t)num_sms_ * 8)); }
@@ -273,22 +272,7 @@ InstantJoinOp::InstantJoinOp(const ArroyoB200OpConfig& c) {
   h_scalars_.alloc(8 * sizeof(unsigned long long));
 }
 
-InstantJoinOp::~InstantJoinOp() {
-  drain_stream();
-  for (auto& p : pending_) {
-    if (p.second.release) p.second.release(&p.second);
-    cudaEventDestroy(p.first);
-  }
-}
-
-void InstantJoinOp::release_inputs() {
-  for (auto& p : pending_) {
-    cudaEventSynchronize(p.first);
-    if (p.second.release) p.second.release(&p.second);
-    cudaEventDestroy(p.first);
-  }
-  pending_.clear();
-}
+InstantJoinOp::~InstantJoinOp() { drain_stream(); }
 
 void InstantJoinOp::reserve(Side& s, int64_t extra) {
   if (s.n + extra <= s.cap) return;
@@ -333,11 +317,7 @@ void InstantJoinOp::process_batch(uint32_t index, uint32_t in_partitions, ArrowA
   const uint64_t* ptrs[ARROYO_B200_MAX_COLS];
   for (int c = 0; c < s.n_cols; ++c) ptrs[c] = cols[c].data;
   append(s, ptrs, n, true);
-  cudaEvent_t ev;
-  AB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-  AB_CUDA(cudaEventRecord(ev, stream_));
-  pending_.emplace_back(ev, *batch);
-  batch->release = nullptr;
+  inputs_.hold(batch, stream_);
 }
 
 void InstantJoinOp::process_device_batch(uint32_t index, uint32_t in_partitions, const uint64_t* cols, int32_t n_cols,
@@ -409,7 +389,7 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
   }
   AB_CUDA(cudaMemcpyAsync(h_scalars_.p, sc, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
-  release_inputs();
+  inputs_.release(true);
   const unsigned long long* hs = h_scalars_.as<unsigned long long>();
   const int64_t nl = (int64_t)hs[0], nr = (int64_t)hs[1];
   const int64_t min_ts = std::min<int64_t>((int64_t)hs[2], (int64_t)hs[3]);

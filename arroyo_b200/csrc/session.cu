@@ -693,13 +693,12 @@ class SessionOp final : public OpBase {
   uint32_t seq_ = 0;
   bool has_wm_ = false;
   int64_t wm_ = 0;
-  DevBuf staging_;
-  uint64_t staging_cap_ = 0;
+  AggStaging staging_;
   DevBuf scan_sums_;
   // output
   uint64_t out_cap_ = 0;
   DevBuf o_key_, o_start_, o_end_, o_ts_, o_agg_[ARROYO_B200_MAX_AGGS];
-  std::vector<std::pair<cudaEvent_t, ArrowArray>> pending_;
+  HeldInputs inputs_;  // host batches whose copies to staging_ may still run
   ArroyoB200Stats st_{};
   DevBuf late_, earliest_;
   uint64_t compact_min_ = 1u << 16;  // pools smaller than this are never compacted (ARROYO_B200_SESSION_COMPACT_MIN)
@@ -717,11 +716,10 @@ class SessionOp final : public OpBase {
     AB_CUDA(cudaStreamSynchronize(stream_));
   }
   void check_err();
-  void prep(const long long* key, const long long* ts, const long long* const* vals, int64_t n);
+  void prep(const AggCols& d, int64_t n);
   void apply_pending();
   void sort_big_keys(const GroupParams& g, uint64_t n);
   void maybe_compact();
-  void release_inputs(bool wait);
 };
 
 SessionOp::SessionOp(const ArroyoB200OpConfig& c) {
@@ -749,13 +747,7 @@ SessionOp::SessionOp(const ArroyoB200OpConfig& c) {
   AB_CUDA(cudaStreamSynchronize(stream_));
 }
 
-SessionOp::~SessionOp() {
-  drain_stream();
-  for (auto& p : pending_) {
-    if (p.second.release) p.second.release(&p.second);
-    cudaEventDestroy(p.first);
-  }
-}
+SessionOp::~SessionOp() { drain_stream(); }
 
 void SessionOp::alloc_keys(uint64_t cap) {
   id_cap_ = cap;
@@ -937,23 +929,8 @@ void SessionOp::check_err() {
   throw Error(ARROYO_B200_RUNTIME, "session operator pool / output capacity exceeded");
 }
 
-void SessionOp::release_inputs(bool wait) {
-  while (!pending_.empty()) {
-    auto& p = pending_.front();
-    if (wait) AB_CUDA(cudaEventSynchronize(p.first));
-    else {
-      cudaError_t e = cudaEventQuery(p.first);
-      if (e == cudaErrorNotReady) break;
-      AB_CUDA(e);
-    }
-    if (p.second.release) p.second.release(&p.second);
-    cudaEventDestroy(p.first);
-    pending_.erase(pending_.begin());
-  }
-}
-
 // one input batch -> launch arena
-void SessionOp::prep(const long long* key, const long long* ts, const long long* const* vals, int64_t n) {
+void SessionOp::prep(const AggCols& d, int64_t n) {
   if (n <= 0) return;
   // a launch never mixes rows that arrived under different watermarks, and is cut at 4 Mi rows
   if (arena_rows_bound_ + (uint64_t)n > (1ull << 22) && arena_rows_bound_ > 0) apply_pending();
@@ -961,9 +938,9 @@ void SessionOp::prep(const long long* key, const long long* ts, const long long*
   ensure_arena(arena_rows_bound_ + (uint64_t)n);
   if (plan_.keyed) grow_keys((uint64_t)n);
   PrepParams p{};
-  p.key = key;
-  p.ts = ts;
-  for (int v = 0; v < plan_.n_vals; ++v) p.val[v] = vals[v];
+  p.key = d.key;
+  p.ts = d.ts;
+  for (int v = 0; v < plan_.n_vals; ++v) p.val[v] = d.val[v];
   p.n = n;
   p.seq = seq_++;
   p.has_wm = has_wm_ ? 1 : 0;
@@ -996,50 +973,23 @@ void SessionOp::prep(const long long* key, const long long* ts, const long long*
 
 void SessionOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const ArrowSchema* schema) {
   set_device();
-  int64_t n = 0;
-  std::vector<InColumn> cols = import_batch(batch, schema, &n);
-  AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
-  require_aggregate_input_types(cols, plan_.keyed ? plan_.key_col : -1, plan_.val_cols, plan_.n_vals);
-  if (plan_.keyed) key_format_ = cols[plan_.key_col].format;
-  release_inputs(false);
-  st_.rows_in += (uint64_t)n;
+  AggCols d;
+  const int64_t n = staging_.stage(plan_, batch, schema, stream_, &st_, &key_format_, &d);
+  inputs_.release(false);
   if (n == 0) {
     if (batch->release) batch->release(batch);
     return;
   }
-  // stage the used columns (the staging buffer is reused in stream order)
-  const int n_used = 2 + plan_.n_vals;
-  if ((uint64_t)n > staging_cap_) {
-    AB_CUDA(cudaStreamSynchronize(stream_));
-    staging_cap_ = std::max<uint64_t>((uint64_t)n, staging_cap_ * 2);
-    staging_.alloc((size_t)n_used * staging_cap_ * 8);
-  }
-  long long* base = staging_.as<long long>();
-  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
-  if (plan_.keyed) AB_CUDA(cudaMemcpyAsync(base, cols[plan_.key_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  AB_CUDA(cudaMemcpyAsync(base + staging_cap_, cols[plan_.ts_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  for (int v = 0; v < plan_.n_vals; ++v) {
-    AB_CUDA(cudaMemcpyAsync(base + (size_t)(2 + v) * staging_cap_, cols[plan_.val_cols[v]].data, (size_t)n * 8,
-                            cudaMemcpyHostToDevice, stream_));
-    vals[v] = base + (size_t)(2 + v) * staging_cap_;
-  }
-  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((plan_.keyed ? 1 : 0) + 1 + plan_.n_vals);
-  cudaEvent_t ev;
-  AB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-  AB_CUDA(cudaEventRecord(ev, stream_));
-  pending_.emplace_back(ev, *batch);
-  batch->release = nullptr;
-  prep(base, base + staging_cap_, vals, n);
+  inputs_.hold(batch, stream_);
+  prep(d, n);
 }
 
 void SessionOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols, int32_t n_cols, int64_t n_rows) {
   set_device();
-  AB_REQUIRE(n_cols == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
+  const AggCols d = plan_.columns(cols, n_cols);
   if (n_rows <= 0) return;
   st_.rows_in += (uint64_t)n_rows;
-  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
-  for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)cols[plan_.val_cols[v]];
-  prep(plan_.keyed ? (const long long*)cols[plan_.key_col] : nullptr, (const long long*)cols[plan_.ts_col], vals, n_rows);
+  prep(d, n_rows);
 }
 
 // group the arena by key and run the per-key state machines over the new runs
@@ -1172,7 +1122,7 @@ void SessionOp::flush() {
   set_device();
   apply_pending();
   AB_CUDA(cudaStreamSynchronize(stream_));
-  release_inputs(true);
+  inputs_.release(true);
 }
 
 // handle_checkpoint (session_aggregating_window.rs:907-925): table "s" (the raw input batches) is written by the
@@ -1215,8 +1165,12 @@ void SessionOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int
     unsigned long long late = 0;
     AB_CUDA(cudaMemcpyAsync(&late, late_.p, 8, cudaMemcpyDeviceToHost, stream_));
     for (int64_t i = 0; i < n; ++i) {
-      process_batch(0, 1, &state[i], &schemas[i]);
+      AggCols d;
+      const int64_t rows = staging_.stage(plan_, &state[i], &schemas[i], stream_, &st_, &key_format_, &d);
+      prep(d, rows);
       apply_pending();  // every stored batch is its own input batch
+      AB_CUDA(cudaStreamSynchronize(stream_));
+      if (state[i].release) state[i].release(&state[i]);  // taken: its rows are in the operator's pools
     }
     st_.rows_in = rows_in;
     AB_CUDA(cudaMemcpyAsync(late_.p, &late, 8, cudaMemcpyHostToDevice, stream_));
@@ -1347,7 +1301,7 @@ void SessionOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vector<
     AB_CUDA(cudaStreamSynchronize(stream_));
     st_.rows_late = late;
   }
-  release_inputs(false);
+  inputs_.release(false);
   if (n > 0) {
     st_.rows_out += (uint64_t)n;
     ++st_.windows_out;

@@ -335,8 +335,7 @@ class UpdatingAggOp final : public OpBase {
   uint32_t total_keys_ = 0;
   DevBuf slots_, bucket_nkeys_, id_keys_, n_total_;
   DevBuf cur_, prev_, cur_ts_, prev_ts_, touched_, flushed_, list_, counters_;  // counters_: [n_touched, retractions, appends, pad] u32 + deferred u64
-  DevBuf staging_;
-  uint64_t staging_cap_ = 0;
+  AggStaging staging_;
   // deferred rows (key, ts, values): two sets, one re-ingested while the other takes the rows that defer again
   DevBuf defer_[2][2 + MAX_VALS];
   uint64_t defer_cap_[2] = {0, 0};
@@ -367,7 +366,7 @@ class UpdatingAggOp final : public OpBase {
   void reserve_defer(int set, uint64_t rows);
   void drain_deferred();
   void ensure_room(uint64_t new_rows);
-  void ingest(const long long* key, const long long* ts, const long long* const* vals, int64_t n);
+  void ingest(const AggCols& d, int64_t n);
   void flush_to(BatchesPriv* out);
 };
 
@@ -509,9 +508,11 @@ void UpdatingAggOp::drain_deferred() {
       const int full = defer_cur_;
       defer_cur_ ^= 1;
       AB_CUDA(cudaMemsetAsync(d_count, 0, 8, stream_));
-      const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
-      for (int v = 0; v < plan_.n_vals; ++v) vals[v] = defer_[full][2 + v].as<long long>();
-      ingest(defer_[full][0].as<long long>(), defer_[full][1].as<long long>(), vals, (int64_t)n);
+      AggCols d;
+      d.key = defer_[full][0].as<long long>();
+      d.ts = defer_[full][1].as<long long>();
+      for (int v = 0; v < plan_.n_vals; ++v) d.val[v] = defer_[full][2 + v].as<long long>();
+      ingest(d, (int64_t)n);
     }
   } catch (...) {
     cudaMemsetAsync(d_count, 0, 8, stream_);  // a failed drain must not fail every later call
@@ -527,12 +528,12 @@ void UpdatingAggOp::ensure_room(uint64_t new_rows) {
   while ((uint64_t)total_keys_ + new_rows > n_buckets_ * (uint64_t)BD_MEAN) grow();
 }
 
-void UpdatingAggOp::ingest(const long long* key, const long long* ts, const long long* const* vals, int64_t n) {
+void UpdatingAggOp::ingest(const AggCols& d, int64_t n) {
   if (n <= 0) return;
   UIngest p{};
-  p.key = key;
-  p.ts = ts;
-  for (int v = 0; v < plan_.n_vals; ++v) p.val[v] = vals[v];
+  p.key = d.key;
+  p.ts = d.ts;
+  for (int v = 0; v < plan_.n_vals; ++v) p.val[v] = d.val[v];
   p.n = n;
   p.keyed = plan_.keyed ? 1 : 0;
   p.n_vals = plan_.n_vals;
@@ -554,34 +555,15 @@ void UpdatingAggOp::ingest(const long long* key, const long long* ts, const long
 
 void UpdatingAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const ArrowSchema* schema) {
   set_device();
-  int64_t n = 0;
-  std::vector<InColumn> cols = import_batch(batch, schema, &n);
-  AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
-  require_aggregate_input_types(cols, plan_.keyed ? plan_.key_col : -1, plan_.val_cols, plan_.n_vals);
-  if (plan_.keyed) key_format_ = cols[plan_.key_col].format;
-  st_.rows_in += (uint64_t)n;
+  AggCols d;
+  const int64_t n = staging_.stage(plan_, batch, schema, stream_, &st_, &key_format_, &d);
   if (n == 0) {
     if (batch->release) batch->release(batch);
     return;
   }
+  // ensure_room synchronises the stream before it can fail: a refused batch is no longer being copied
   ensure_room((uint64_t)n);
-  const int n_used = 2 + plan_.n_vals;
-  if ((uint64_t)n > staging_cap_) {
-    AB_CUDA(cudaStreamSynchronize(stream_));
-    staging_cap_ = std::max<uint64_t>((uint64_t)n, staging_cap_ * 2);
-    staging_.alloc((size_t)n_used * staging_cap_ * 8);
-  }
-  long long* base = staging_.as<long long>();
-  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
-  if (plan_.keyed) AB_CUDA(cudaMemcpyAsync(base, cols[plan_.key_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  AB_CUDA(cudaMemcpyAsync(base + staging_cap_, cols[plan_.ts_col].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  for (int v = 0; v < plan_.n_vals; ++v) {
-    AB_CUDA(cudaMemcpyAsync(base + (size_t)(2 + v) * staging_cap_, cols[plan_.val_cols[v]].data, (size_t)n * 8, cudaMemcpyHostToDevice,
-                            stream_));
-    vals[v] = base + (size_t)(2 + v) * staging_cap_;
-  }
-  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((plan_.keyed ? 1 : 0) + 1 + plan_.n_vals);
-  ingest(base, base + staging_cap_, vals, n);
+  ingest(d, n);
   // the staging buffer is reused by the next batch: the copies and the kernel must have consumed the host batch
   AB_CUDA(cudaStreamSynchronize(stream_));
   if (batch->release) batch->release(batch);
@@ -590,13 +572,11 @@ void UpdatingAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const A
 
 void UpdatingAggOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols, int32_t n_cols, int64_t n_rows) {
   set_device();
-  AB_REQUIRE(n_cols == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
+  const AggCols d = plan_.columns(cols, n_cols);
   if (n_rows <= 0) return;
   st_.rows_in += (uint64_t)n_rows;
   ensure_room((uint64_t)n_rows);
-  const long long* vals[MAX_VALS] = {nullptr, nullptr, nullptr, nullptr};
-  for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)cols[plan_.val_cols[v]];
-  ingest(plan_.keyed ? (const long long*)cols[plan_.key_col] : nullptr, (const long long*)cols[plan_.ts_col], vals, n_rows);
+  ingest(d, n_rows);
 }
 
 static void* d2h_part(const void* dev, size_t off_rows, int64_t n, void* host, size_t host_off_rows, cudaStream_t s) {
@@ -772,7 +752,8 @@ void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
   export_batch(cols, rows, &out->arrays.back(), &out->schemas.back());
 }
 
-// initialize (:446-503): the batches of table "a", in any order and with any number of rows per key.
+// initialize (:446-503): the batches of table "a", in any order and with any number of rows per key.  A restore that
+// succeeds takes every batch once the copies have completed.
 void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t, int64_t) {
   if (n <= 0) return;
   AB_REQUIRE(state != nullptr && schemas != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null state batches");
@@ -807,7 +788,14 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
     }
     total += rows[b];
   }
-  if (total == 0) return;
+  auto take_all = [&]() {
+    for (int64_t b = 0; b < n; ++b)
+      if (state[b].release) state[b].release(&state[b]);
+  };
+  if (total == 0) {
+    take_all();
+    return;
+  }
   // which column seeds each accumulator: the row count from COUNT(*), else from a SUM's or AVG's count, else 1
   int rows_col = -1, ts_col = -1, gen_col = -1, acc_col[MAX_ACC];
   for (int a = 0; a < MAX_ACC; ++a) acc_col[a] = -1;
@@ -900,6 +888,7 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   AB_CUDA(cudaStreamSynchronize(stream_));
   generation_ = max_gen + 1;
   restored_ = true;
+  take_all();
 }
 
 }  // namespace

@@ -1698,16 +1698,15 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
 
 void WindowAggOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols, int32_t n_cols, int64_t n_rows) {
   set_device();
-  AB_REQUIRE(n_cols == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
+  const AggCols d = plan_.columns(cols, n_cols);
   if (n_rows <= 0) return;
   st_.rows_in += (uint64_t)n_rows;
   int64_t done = 0;
   while (done < n_rows) {
     int64_t take = std::min<int64_t>(n_rows - done, launch_rows_ - pending_rows_);
     const long long* vals[MAX_VALS];
-    for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)cols[plan_.val_cols[v]] + done;
-    add_segment(plan_.keyed ? (const long long*)cols[plan_.key_col] + done : nullptr, (const long long*)cols[plan_.ts_col] + done, vals,
-                take);
+    for (int v = 0; v < plan_.n_vals; ++v) vals[v] = d.val[v] + done;
+    add_segment(d.key ? d.key + done : nullptr, d.ts + done, vals, take);
     done += take;
     if (pending_rows_ >= launch_rows_) launch_pending();
   }
@@ -2639,7 +2638,10 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
     std::vector<InColumn> cols = import_batch(&state[bi], &schemas[bi], &rows);
     AB_REQUIRE((int)cols.size() == expect_cols, ARROYO_B200_INVALID_ARGUMENT,
                "state batch does not match the partial schema");
-    if (rows == 0) continue;
+    if (rows == 0) {
+      if (state[bi].release) state[bi].release(&state[bi]);
+      continue;
+    }
     if (plan_.keyed) key_format_ = cols[0].format;
     const int64_t ts = (int64_t)cols.back().data[0];
     const int64_t bin = bin_start(ts, slide_);

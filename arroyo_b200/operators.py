@@ -6,6 +6,7 @@ process_batch(batch, ctx, collector), handle_watermark(watermark, ctx, collector
 handle_checkpoint(barrier, ctx, collector), on_close(final_message, ctx, collector).
 Batches are pyarrow RecordBatches crossing the boundary through the Arrow C Data Interface."""
 import ctypes as C
+import functools
 from typing import List, Optional
 
 import pyarrow as pa
@@ -32,6 +33,31 @@ def export_batch(batch: pa.RecordBatch):
     arr, sch = ffi.ArrowArray(), ffi.ArrowSchema()
     batch._export_to_c(C.addressof(arr), C.addressof(sch))
     return arr, sch
+
+
+def _release(s):
+    """Releases an exported Arrow C struct unless its consumer already took it (`release` set to NULL)."""
+    if s.release:
+        C.CFUNCTYPE(None, C.c_void_p)(s.release)(C.addressof(s))
+
+
+def _agg_config(kind: int, c, names: List[str]) -> ffi.OpConfig:
+    """The OpConfig of an aggregate over input columns `names`: its key column and aggregates from `c`."""
+    cfg = ffi.OpConfig()
+    cfg.kind = kind
+    cfg.n_cols = len(names)
+    cfg.timestamp_col = names.index(TIMESTAMP)
+    if len(c.key_names) > 1:
+        raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, "more than one group-by key column")
+    cfg.n_key_cols = len(c.key_names)
+    cfg.key_col = names.index(c.key_names[0]) if c.key_names else 0
+    cfg.n_aggs = len(c.aggs)
+    for i, a in enumerate(c.aggs):
+        if a.kind not in _AGG_KINDS:
+            raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, f"aggregate {a.kind}")
+        cfg.aggs[i].kind = _AGG_KINDS[a.kind]
+        cfg.aggs[i].input_col = names.index(a.col) if a.col is not None else 0
+    return cfg
 
 
 class ExportedBatches:
@@ -137,6 +163,56 @@ class _NativeOperator:
         _check(self._lib, self._h, self._lib.arroyo_b200_op_stats(self._h, C.byref(s)))
         return s.as_dict()
 
+    def _process_batch(self, entry, index: int, parts: int, batch: pa.RecordBatch, out: Optional[ffi.Batches] = None):
+        """Hands `batch` to `entry` (arroyo_b200_op_process_batch, or arroyo_b200_op_process_batch_emit with `out`).
+        The library takes the array when the call succeeds; whatever it did not take is released here."""
+        arr, sch = export_batch(batch)
+        extra = () if out is None else (C.byref(out),)
+        try:
+            st = entry(self._h, index, parts, C.byref(arr), C.byref(sch), *extra)
+        finally:
+            _release(arr)
+            _release(sch)
+        _check(self._lib, self._h, st)
+
+    def _on_start(self, batches: List[pa.RecordBatch], wm: int, t: int):
+        """arroyo_b200_op_on_start with `batches` as the state, the restored watermark `wm` and the table time `t`
+        (ffi.INT64_MIN: none).  The library takes the batches it consumed; the rest are released here."""
+        n = len(batches)
+        arrs = (ffi.ArrowArray * max(n, 1))()
+        schs = (ffi.ArrowSchema * max(n, 1))()
+        for i, b in enumerate(batches):
+            b._export_to_c(C.addressof(arrs[i]), C.addressof(schs[i]))
+        try:
+            st = self._lib.arroyo_b200_op_on_start(self._h, arrs, schs, n, wm, t)
+        finally:
+            for s in list(arrs) + list(schs):
+                _release(s)
+        _check(self._lib, self._h, st)
+
+    def _collect(self, out: ffi.Batches, collector: Optional[Collector]):
+        """Imports the batches of `out` under `output_names()` into `collector` (None: they are dropped)."""
+        names = self.output_names()
+        for b in import_batches(self._lib, out):
+            if collector is not None:
+                collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+
+    def _device_windows(self, call, max_out: int, drain: bool = True):
+        """The windows of a device-resident emission, list of (n_rows, [device pointers]).  `call(out, max_out, n)`
+        hands out at most `max_out` of them; with `drain`, arroyo_b200_op_handle_watermark_device_poll collects the
+        ones the library queued beyond that."""
+        out = getattr(self, "_dev_out", None)
+        if out is None or len(out) < max_out:
+            out = self._dev_out = (ffi.DeviceBatch * max_out)()  # reused: building it costs more than the call
+        n = C.c_int64(0)
+        got = []
+        while True:
+            _check(self._lib, self._h, call(out, max_out, C.byref(n)))
+            got += [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
+            if not drain or n.value != max_out or max_out <= 0:
+                return got
+            call = functools.partial(self._lib.arroyo_b200_op_handle_watermark_device_poll, self._h)
+
 
 class _WindowAggregate(_NativeOperator):
     def __init__(self, config, input_schema: Optional[pa.Schema] = None, **kw):
@@ -149,24 +225,11 @@ class _WindowAggregate(_NativeOperator):
     # -- construction (OperatorConstructor::with_config) -------------------------------------
     def _build(self, names: List[str]):
         c = self.config
-        cfg = ffi.OpConfig()
-        cfg.kind = self.kind
-        cfg.width_ns = int(c.width)
-        cfg.slide_ns = int(getattr(c, "slide", 0) or 0)
-        cfg.n_cols = len(names)
-        cfg.timestamp_col = names.index(TIMESTAMP)
-        if len(c.key_names) > 1:
-            raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, "more than one group-by key column")
-        cfg.n_key_cols = len(c.key_names)
-        cfg.key_col = names.index(c.key_names[0]) if c.key_names else 0
         if len(c.aggs) > ffi.MAX_AGGS:
             raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, "too many aggregates")
-        cfg.n_aggs = len(c.aggs)
-        for i, a in enumerate(c.aggs):
-            if a.kind not in _AGG_KINDS:
-                raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, f"aggregate {a.kind}")
-            cfg.aggs[i].kind = _AGG_KINDS[a.kind]
-            cfg.aggs[i].input_col = names.index(a.col) if a.col is not None else 0
+        cfg = _agg_config(self.kind, c, names)
+        cfg.width_ns = int(c.width)
+        cfg.slide_ns = int(getattr(c, "slide", 0) or 0)
         pc = getattr(c, "partial_count_col", None)
         cfg.partial_count_col_plus1 = names.index(pc) + 1 if pc else 0
         cfg.final_projection = 1 if c.final_projection else 0
@@ -204,31 +267,13 @@ class _WindowAggregate(_NativeOperator):
             return
         if not self.created:
             raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "restore needs input_schema at construction")
-        n = len(batches)
-        arrs = (ffi.ArrowArray * max(n, 1))()
-        schs = (ffi.ArrowSchema * max(n, 1))()
-        for i, b in enumerate(batches):
-            b._export_to_c(C.addressof(arrs[i]), C.addressof(schs[i]))
         mt = table.get_min_time()
-        st = self._lib.arroyo_b200_op_on_start(
-            self._h, arrs, schs, n, ffi.INT64_MIN if wm is None else clamp_watermark(wm),
-            ffi.INT64_MIN if mt is None else mt)
-        _check(self._lib, self._h, st)
+        self._on_start(batches, ffi.INT64_MIN if wm is None else clamp_watermark(wm), ffi.INT64_MIN if mt is None else mt)
 
     def process_batch(self, batch: pa.RecordBatch, ctx: OperatorContext, collector: Collector):
         if not self.created:
             self._build(batch.schema.names)
-        arr, sch = export_batch(batch)
-        st = self._lib.arroyo_b200_op_process_batch(self._h, 0, 1, C.byref(arr), C.byref(sch))
-        if st != ffi.OK:
-            # on error the caller keeps ownership of the exported structs
-            for s in (arr, sch):
-                if s.release:
-                    C.CFUNCTYPE(None, C.c_void_p)(s.release)(C.addressof(s))
-        _check(self._lib, self._h, st)
-        # the schema struct stays ours
-        if sch.release:
-            C.CFUNCTYPE(None, C.c_void_p)(sch.release)(C.addressof(sch))
+        self._process_batch(self._lib.arroyo_b200_op_process_batch, 0, 1, batch)
 
     def process_device_batch(self, cols: List[int], n_rows: int):
         """`cols` = device pointers (ints), one per input column."""
@@ -247,11 +292,8 @@ class _WindowAggregate(_NativeOperator):
         if wm is None or not self.created:
             return None if self.kind == ffi.SLIDING_AGGREGATE and wm is None else watermark
         out = ffi.Batches()
-        st = self._lib.arroyo_b200_op_handle_watermark(self._h, clamp_watermark(wm), C.byref(out))
-        _check(self._lib, self._h, st)
-        names = self.output_names()
-        for b in import_batches(self._lib, out):
-            collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+        _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark(self._h, clamp_watermark(wm), C.byref(out)))
+        self._collect(out, collector)
         return watermark
 
     def handle_watermark_begin(self, watermark, ctx: OperatorContext) -> bool:
@@ -272,9 +314,7 @@ class _WindowAggregate(_NativeOperator):
         _check(self._lib, self._h, st)
         if not ready.value:
             return False
-        names = self.output_names()
-        for b in import_batches(self._lib, out):
-            collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+        self._collect(out, collector)
         return True
 
     def run_batches(self, exported: "ExportedBatches", watermarks, collector: Collector, first: int = 0,
@@ -292,30 +332,14 @@ class _WindowAggregate(_NativeOperator):
             self._h, C.addressof(exported.arrays) + first * step, C.addressof(exported.schema), count,
             C.cast(C.addressof(watermarks) + 8 * first, C.POINTER(C.c_int64)), 1 if async_emit else 0, C.byref(out),
             C.byref(taken))
-        names = self.output_names()
-        for b in import_batches(self._lib, out):
-            collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+        self._collect(out, collector)
         _check(self._lib, self._h, st)
 
     def handle_watermark_device(self, wm: int, max_out: int = 64):
         """Emission left on the device: list of (n_rows, [device pointers]).  The library hands out at most `max_out`
         windows per call and queues the rest; they are collected here with further polls."""
-        out = getattr(self, "_dev_out", None)
-        if out is None or len(out) < max_out:
-            out = self._dev_out = (ffi.DeviceBatch * max_out)()  # reused: building it costs more than the call
-        n = C.c_int64(0)
-        st = self._lib.arroyo_b200_op_handle_watermark_device(self._h, clamp_watermark(wm), out, max_out, C.byref(n))
-        _check(self._lib, self._h, st)
-        got = [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
-        return got + self._drain_device(max_out, n.value)
-
-    def _drain_device(self, max_out: int, n: int):
-        got = []
-        while n == max_out and max_out > 0:
-            more = self.handle_watermark_device_poll(max_out, drain=False)
-            got += more
-            n = len(more)
-        return got
+        return self._device_windows(
+            functools.partial(self._lib.arroyo_b200_op_handle_watermark_device, self._h, clamp_watermark(wm)), max_out)
 
     def handle_watermark_device_begin(self, wm: int):
         """First half of handle_watermark_device: the emission is enqueued, its row counts are not awaited."""
@@ -324,13 +348,8 @@ class _WindowAggregate(_NativeOperator):
     def handle_watermark_device_poll(self, max_out: int = 64, drain: bool = True):
         """Second half: the windows of the outstanding emission, list of (n_rows, [device pointers]).  With `drain`,
         polls until the library has no window queued (it hands out at most `max_out` per call)."""
-        out = getattr(self, "_dev_out", None)
-        if out is None or len(out) < max_out:
-            out = self._dev_out = (ffi.DeviceBatch * max_out)()
-        n = C.c_int64(0)
-        _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark_device_poll(self._h, out, max_out, C.byref(n)))
-        got = [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
-        return got + (self._drain_device(max_out, n.value) if drain else [])
+        return self._device_windows(
+            functools.partial(self._lib.arroyo_b200_op_handle_watermark_device_poll, self._h), max_out, drain)
 
     def handle_checkpoint(self, barrier, ctx: OperatorContext, collector: Collector):
         if not self.created:
@@ -387,23 +406,9 @@ class SessionAggregatingWindowFunc(_NativeOperator):
         return {"s": int(self.config.gap) * 100, "e": 0}
 
     def _build(self, names: List[str]):
-        c = self.config
-        cfg = ffi.OpConfig()
-        cfg.kind = self.kind
-        cfg.gap_ns = int(c.gap)
-        cfg.n_cols = len(names)
-        cfg.timestamp_col = names.index(TIMESTAMP)
-        if len(c.key_names) > 1:
-            raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, "more than one group-by key column")
-        cfg.n_key_cols = len(c.key_names)
-        cfg.key_col = names.index(c.key_names[0]) if c.key_names else 0
-        cfg.n_aggs = len(c.aggs)
-        for i, a in enumerate(c.aggs):
-            if a.kind not in _AGG_KINDS:
-                raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, f"aggregate {a.kind}")
-            cfg.aggs[i].kind = _AGG_KINDS[a.kind]
-            cfg.aggs[i].input_col = names.index(a.col) if a.col is not None else 0
-        cfg.window_index = int(c.window_index)
+        cfg = _agg_config(self.kind, self.config, names)
+        cfg.gap_ns = int(self.config.gap)
+        cfg.window_index = int(self.config.window_index)
         self._create(cfg)
 
     def output_names(self) -> List[str]:
@@ -412,15 +417,6 @@ class SessionAggregatingWindowFunc(_NativeOperator):
         names.insert(min(max(c.window_index, 0), len(names)), "window")
         return names + [a.name for a in c.aggs] + [TIMESTAMP]
 
-    def _send(self, batch: pa.RecordBatch):
-        arr, sch = export_batch(batch)
-        st = self._lib.arroyo_b200_op_process_batch(self._h, 0, 1, C.byref(arr), C.byref(sch))
-        if st != ffi.OK and arr.release:
-            C.CFUNCTYPE(None, C.c_void_p)(arr.release)(C.addressof(arr))
-        if sch.release:
-            C.CFUNCTYPE(None, C.c_void_p)(sch.release)(C.addressof(sch))
-        _check(self._lib, self._h, st)
-
     def _set_watermark(self, ctx: OperatorContext):
         """A new operator takes the last watermark before its first batch (on_start with nothing to restore): the
         library only learns watermarks from handle_watermark and on_start, and without one it would treat every row as
@@ -428,9 +424,7 @@ class SessionAggregatingWindowFunc(_NativeOperator):
         wm = ctx.last_present_watermark()
         if wm is None or not self.created:
             return
-        arrs, schs = (ffi.ArrowArray * 1)(), (ffi.ArrowSchema * 1)()
-        _check(self._lib, self._h, self._lib.arroyo_b200_op_on_start(self._h, arrs, schs, 0, clamp_watermark(wm),
-                                                                     ffi.INT64_MIN))
+        self._on_start([], clamp_watermark(wm), ffi.INT64_MIN)
 
     def process_batch(self, batch: pa.RecordBatch, ctx: OperatorContext, collector: Collector):
         if not self.created:
@@ -449,7 +443,7 @@ class SessionAggregatingWindowFunc(_NativeOperator):
             ts = kept.column(kept.schema.names.index(TIMESTAMP)).cast(pa.int64())
             import pyarrow.compute as pc
             ctx.table("s", int(self.config.gap) * 100).insert(int(pc.max(ts).as_py()), kept)
-        self._send(batch)
+        self._process_batch(self._lib.arroyo_b200_op_process_batch, 0, 1, batch)
 
     def process_device_batch(self, cols: List[int], n_rows: int):
         """Device-resident input (operator chaining): the rows never reach the host, so table "s" is not maintained
@@ -486,38 +480,21 @@ class SessionAggregatingWindowFunc(_NativeOperator):
             if not batches:
                 return
             self._build(batches[0].schema.names)
-        n = len(batches)
-        arrs = (ffi.ArrowArray * max(n, 1))()
-        schs = (ffi.ArrowSchema * max(n, 1))()
-        for i, b in enumerate(batches):
-            b._export_to_c(C.addressof(arrs[i]), C.addressof(schs[i]))
         wm = ctx.last_present_watermark()
-        st = self._lib.arroyo_b200_op_on_start(self._h, arrs, schs, n,
-                                               ffi.INT64_MIN if wm is None else clamp_watermark(wm), start_time)
-        _check(self._lib, self._h, st)
+        self._on_start(batches, ffi.INT64_MIN if wm is None else clamp_watermark(wm), start_time)
 
     def handle_watermark(self, watermark, ctx: OperatorContext, collector: Collector):
         wm = ctx.last_present_watermark()
         if wm is None or not self.created:
             return watermark
         out = ffi.Batches()
-        st = self._lib.arroyo_b200_op_handle_watermark(self._h, clamp_watermark(wm), C.byref(out))
-        _check(self._lib, self._h, st)
-        names = self.output_names()
-        for b in import_batches(self._lib, out):
-            collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+        _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark(self._h, clamp_watermark(wm), C.byref(out)))
+        self._collect(out, collector)
         return watermark
 
     def handle_watermark_device(self, wm: int, max_out: int = 4):
-        out = (ffi.DeviceBatch * max_out)()
-        n = C.c_int64(0)
-        st = self._lib.arroyo_b200_op_handle_watermark_device(self._h, clamp_watermark(wm), out, max_out, C.byref(n))
-        _check(self._lib, self._h, st)
-        got = [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
-        while n.value == max_out and max_out > 0:  # windows beyond max_out stay queued in the library
-            _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark_device_poll(self._h, out, max_out, C.byref(n)))
-            got += [(out[i].n_rows, [out[i].cols[c] for c in range(out[i].n_cols)]) for i in range(n.value)]
-        return got
+        return self._device_windows(
+            functools.partial(self._lib.arroyo_b200_op_handle_watermark_device, self._h, clamp_watermark(wm)), max_out)
 
 
 class UpdatingAggregatingFunc(_NativeOperator):
@@ -565,36 +542,10 @@ class UpdatingAggregatingFunc(_NativeOperator):
             return
         if not self.created:
             raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "restore needs input_schema at construction")
-        n = len(batches)
-        arrs = (ffi.ArrowArray * n)()
-        schs = (ffi.ArrowSchema * n)()
-        for i, b in enumerate(batches):
-            b._export_to_c(C.addressof(arrs[i]), C.addressof(schs[i]))
-        try:
-            st = self._lib.arroyo_b200_op_on_start(self._h, arrs, schs, n, ffi.INT64_MIN, ffi.INT64_MIN)
-        finally:
-            # the library copies the state during the call: the exported structs stay ours
-            for s in list(arrs) + list(schs):
-                if s.release:
-                    C.CFUNCTYPE(None, C.c_void_p)(s.release)(C.addressof(s))
-        _check(self._lib, self._h, st)
+        self._on_start(batches, ffi.INT64_MIN, ffi.INT64_MIN)
 
     def _build(self, names: List[str]):
-        c = self.config
-        cfg = ffi.OpConfig()
-        cfg.kind = self.kind
-        cfg.n_cols = len(names)
-        cfg.timestamp_col = names.index(TIMESTAMP)
-        if len(c.key_names) > 1:
-            raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, "more than one group-by key column")
-        cfg.n_key_cols = len(c.key_names)
-        cfg.key_col = names.index(c.key_names[0]) if c.key_names else 0
-        cfg.n_aggs = len(c.aggs)
-        for i, a in enumerate(c.aggs):
-            if a.kind not in _AGG_KINDS:
-                raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, f"aggregate {a.kind}")
-            cfg.aggs[i].kind = _AGG_KINDS[a.kind]
-            cfg.aggs[i].input_col = names.index(a.col) if a.col is not None else 0
+        cfg = _agg_config(self.kind, self.config, names)
         if self.updating_input:
             self._flags |= ffi.FLAG_UPDATING_INPUT
         self._create(cfg)
@@ -606,13 +557,7 @@ class UpdatingAggregatingFunc(_NativeOperator):
         if not self.created:
             self._build(batch.schema.names)
         self._note_key_type(batch.schema)
-        arr, sch = export_batch(batch)
-        st = self._lib.arroyo_b200_op_process_batch(self._h, 0, 1, C.byref(arr), C.byref(sch))
-        if st != ffi.OK and arr.release:
-            C.CFUNCTYPE(None, C.c_void_p)(arr.release)(C.addressof(arr))
-        if sch.release:
-            C.CFUNCTYPE(None, C.c_void_p)(sch.release)(C.addressof(sch))
-        _check(self._lib, self._h, st)
+        self._process_batch(self._lib.arroyo_b200_op_process_batch, 0, 1, batch)
 
     def process_device_batch(self, cols: List[int], n_rows: int):
         """`cols` = device pointers (ints), one per input column; needs `input_schema` at construction."""
@@ -732,13 +677,7 @@ class InstantJoin(_NativeOperator):
         return out + [TIMESTAMP]
 
     def _send(self, index, parts, batch):
-        arr, sch = export_batch(batch)
-        st = self._lib.arroyo_b200_op_process_batch(self._h, index, parts, C.byref(arr), C.byref(sch))
-        if st != ffi.OK and arr.release:
-            C.CFUNCTYPE(None, C.c_void_p)(arr.release)(C.addressof(arr))
-        if sch.release:
-            C.CFUNCTYPE(None, C.c_void_p)(sch.release)(C.addressof(sch))
-        _check(self._lib, self._h, st)
+        self._process_batch(self._lib.arroyo_b200_op_process_batch, index, parts, batch)
 
     def on_start(self, ctx: OperatorContext):
         """instant_join.rs:205-247: every batch of table "left" goes back through process_left, every batch of table
@@ -748,10 +687,7 @@ class InstantJoin(_NativeOperator):
         for side, name in enumerate(("left", "right")):
             replay.append([b for _, b in ctx.table(name, 0).all_batches_for_watermark(wm)])
         if self.created and wm is not None:
-            empty = (ffi.ArrowArray * 1)()
-            emptys = (ffi.ArrowSchema * 1)()
-            _check(self._lib, self._h, self._lib.arroyo_b200_op_on_start(self._h, empty, emptys, 0, clamp_watermark(wm),
-                                                                          ffi.INT64_MIN))
+            self._on_start([], clamp_watermark(wm), ffi.INT64_MIN)
         for side, batches in enumerate(replay):
             for b in batches:
                 self.process_batch_index(side, 2, b, ctx, None)
@@ -801,11 +737,8 @@ class InstantJoin(_NativeOperator):
             finally:
                 self.config.left_on, self.config.right_on = saved
         out = ffi.Batches()
-        st = self._lib.arroyo_b200_op_handle_watermark(self._h, clamp_watermark(wm), C.byref(out))
-        _check(self._lib, self._h, st)
-        names = self.output_names()
-        for b in import_batches(self._lib, out):
-            collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+        _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_watermark(self._h, clamp_watermark(wm), C.byref(out)))
+        self._collect(out, collector)
         return wm
 
 
@@ -827,18 +760,9 @@ class JoinWithExpiration(InstantJoin):
         return
 
     def _send(self, index, parts, batch, collector=None):
-        arr, sch = export_batch(batch)
         out = ffi.Batches()
-        st = self._lib.arroyo_b200_op_process_batch_emit(self._h, index, parts, C.byref(arr), C.byref(sch), C.byref(out))
-        if st != ffi.OK and arr.release:
-            C.CFUNCTYPE(None, C.c_void_p)(arr.release)(C.addressof(arr))
-        if sch.release:
-            C.CFUNCTYPE(None, C.c_void_p)(sch.release)(C.addressof(sch))
-        _check(self._lib, self._h, st)
-        names = self.output_names()
-        for b in import_batches(self._lib, out):
-            if collector is not None:
-                collector.collect(pa.RecordBatch.from_arrays(b.columns, names=names))
+        self._process_batch(self._lib.arroyo_b200_op_process_batch_emit, index, parts, batch, out)
+        self._collect(out, collector)
 
     def process_batch_index(self, index: int, in_partitions: int, batch: pa.RecordBatch, ctx: OperatorContext,
                             collector: Collector):

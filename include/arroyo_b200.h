@@ -272,6 +272,10 @@ const char* arroyo_b200_op_name(const ArroyoB200Op* op);
  * sliding_aggregating_window.rs:556-595, tumbling :228-248).  `n == 0` = fresh start.
  * `watermark_ns` = ctx.last_present_watermark() or INT64_MIN when there is none.
  * `table_min_time_ns` = ExpiringTimeKeyView::get_min_time() or INT64_MIN.
+ * Ownership follows the Arrow C Data convention, as in process_batch: the library takes a state
+ * batch by releasing it, which sets its `release` to NULL; a successful restore takes every array.
+ * Whatever still has a non-null `release` after the call, successful or not, belongs to the caller,
+ * and so do the schemas.
  * Updating aggregate (incremental_aggregator.rs:446-503): `state` holds every batch of table "a"
  * (UncachedKeyValueView::get_all, in any order, not de-duplicated), in the layout
  * arroyo_b200_op_checkpoint_state writes; both time arguments are ignored.  Per key the row with the
