@@ -1,4 +1,4 @@
-// The window aggregate's key dictionary: a *bucketed* open-addressing table.
+// The key dictionary of the window and updating aggregates: a *bucketed* open-addressing table.
 //
 //   bucket(key) = mulhi32(bd_hash(key) >> 32, n_buckets)           BD_KS 16-byte slots {key, idx} per bucket,
 //   slot0(key)  = (key * odd constant) >> 53                linear probing that wraps inside the bucket
@@ -11,10 +11,15 @@
 // dictionary is read-only; a bucket holds ~BD_MEAN keys (Poisson, sigma ~32: BD_CAPB is 8 sigma above the mean).
 // The direct kernel (one probe + REDs per row) uses the same table through bd_resolve.
 //
-// When a bucket runs out of ids or the table outgrows its mean fill, the host doubles n_buckets and rebuilds
-// (ids change; pane blocks are permuted with the old->new id map, window_agg.cu::grow_ids).
+// The updating aggregate (updating_agg.cu) uses the same table for its dense ids, without the two-pass ingest.
+//
+// BucketDict, at the end of this file, is the host side both operators share: it owns the device buffers, and when a
+// bucket runs out of ids or the table outgrows its mean fill it doubles n_buckets and rebuilds.  Ids change: each
+// operator moves its own per-id state with the old->new id map (the window's pane blocks, the updating aggregate's
+// accumulators).  BucketDict::place gives restored keys their ids before anything is merged.
 #pragma once
 
+#include <algorithm>
 #include <climits>
 
 #include "common.cuh"
@@ -183,5 +188,130 @@ static __global__ void bd_rehash_kernel(BDict old_d, BDict new_d, uint32_t old_i
     map[i] = nid;
   }
 }
+
+// Restore: the id of every row's key, inserted on first sight; ID_OVERFLOW (counted in *overflow) when the key's
+// bucket is out of ids.  keys == nullptr (an unkeyed plan): every row has id 0.
+static __global__ void __launch_bounds__(256) bd_place_kernel(const BDict d, const long long* keys, long long n, uint32_t* ids,
+                                                              unsigned long long* overflow) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) {
+    const uint32_t id = keys ? bd_lookup_or_insert(d, keys[i]) : 0u;
+    ids[i] = id;
+    if (id >= ID_OVERFLOW) atomicAdd(overflow, 1ull);
+  }
+}
+
+// What BucketDict::grow hands back: map[old id] = new id (ID_UNSET: the id held no key) for the old ids [0, old_ids),
+// and the old id capacity (the stride of the caller's per-id arrays before the growth).
+struct BdGrowth {
+  DevBuf map;
+  uint32_t old_ids;
+  uint64_t old_cap;
+};
+
+// The host side of one dictionary.  The key counter (BDict::n_total) stays where its operator reads it back with the
+// rest of its bookkeeping; the owner only takes its address.  An unkeyed plan keeps one bucket's id range and no slots.
+class BucketDict {
+ public:
+  // `launches` counts the kernels launched here (the operator's statistic)
+  void init(cudaStream_t stream, int num_sms, bool keyed, unsigned int* n_total, uint64_t* launches) {
+    stream_ = stream;
+    num_sms_ = num_sms;
+    keyed_ = keyed;
+    n_total_ = n_total;
+    launches_ = launches;
+  }
+  uint64_t n_buckets() const { return n_buckets_; }
+  uint64_t id_cap() const { return id_cap_; }
+  // the id range: every bucket's ids, used or not
+  uint32_t n_ids() const { return (uint32_t)(BD_ID_BASE + n_buckets_ * BD_CAPB); }
+  const long long* id_keys() const { return id_keys_.as<long long>(); }
+
+  // A dictionary of `n_buckets` empty buckets.  Ids are 32-bit with two values reserved: refused at 2^31.
+  void alloc(uint64_t n_buckets) {
+    AB_REQUIRE(bd_id_cap(n_buckets) < (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
+    n_buckets_ = n_buckets;
+    id_cap_ = bd_id_cap(n_buckets);
+    id_keys_.alloc(id_cap_ * sizeof(long long));
+    bd_fill_keys_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(id_keys_.as<long long>(), id_cap_);
+    AB_CUDA(cudaGetLastError());
+    nkeys_.alloc(n_buckets_ * sizeof(unsigned int));
+    AB_CUDA(cudaMemsetAsync(nkeys_.p, 0, n_buckets_ * sizeof(unsigned int), stream_));
+    if (keyed_) {
+      slots_.alloc(n_buckets_ * BD_KS * sizeof(BSlot));
+      bd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(slots_.as<BSlot>(), n_buckets_ * BD_KS);
+      AB_CUDA(cudaGetLastError());
+    }
+    *launches_ += keyed_ ? 2 : 1;
+  }
+
+  BDict view() const {
+    BDict d{};
+    d.slots = slots_.as<BSlot>();
+    d.nkeys = nkeys_.as<unsigned int>();
+    d.id_keys = id_keys_.as<long long>();
+    d.n_total = n_total_;
+    d.n_buckets = (uint32_t)n_buckets_;
+    return d;
+  }
+
+  // Doubles the bucket count and re-inserts every key: ids change, the key counter is recounted.  A bucket's keys split
+  // between the two buckets that replace it, so the rehash itself never runs out of ids.  Refused before anything
+  // moves: the dictionary stays usable.  Returns with the stream drained.
+  BdGrowth grow() {
+    AB_REQUIRE(keyed_, ARROYO_B200_RUNTIME, "growth of an unkeyed dictionary");
+    AB_REQUIRE(bd_id_cap(n_buckets_ * 2) < (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
+    BdGrowth g{DevBuf((size_t)id_cap_ * sizeof(uint32_t)), n_ids(), id_cap_};
+    const BDict old_d = view();
+    const DevBuf old_slots = std::move(slots_), old_nkeys = std::move(nkeys_), old_keys = std::move(id_keys_);
+    AB_CUDA(cudaMemsetAsync(n_total_, 0, sizeof(unsigned int), stream_));
+    alloc(n_buckets_ * 2);
+    bd_rehash_kernel<<<grid(g.old_ids), 256, 0, stream_>>>(old_d, view(), g.old_ids, g.map.as<uint32_t>());
+    AB_CUDA(cudaGetLastError());
+    ++*launches_;
+    AB_CUDA(cudaStreamSynchronize(stream_));  // the old buffers go when this returns
+    return g;
+  }
+
+  // Gives each of `n` restored keys (device memory) its id, ids[i], before the caller merges anything.  When a bucket
+  // runs out of ids, `grow_step()` -- grow() plus the move of the operator's own per-id state -- doubles the dictionary
+  // and every row looks its key up again (a placed key keeps its place, under a new id).  A dictionary sized for few
+  // rows has few buckets, each covering a wide hash range, so crowded keys may need several doublings to split: below
+  // the default size (2^16 keys) it doubles freely; from there on, RESTORE_STALLS doublings in a row that place none
+  // of the rest give up with RUNTIME.
+  template <class GrowStep>
+  void place(const long long* keys, long long n, uint32_t* ids, GrowStep grow_step) {
+    constexpr int RESTORE_STALLS = 4;
+    const uint64_t free_buckets = bd_buckets_for(1ull << 16);
+    DevBuf overflow(sizeof(unsigned long long));
+    for (uint64_t left = UINT64_MAX, stalls = 0;;) {
+      AB_CUDA(cudaMemsetAsync(overflow.p, 0, sizeof(unsigned long long), stream_));
+      bd_place_kernel<<<grid(n), 256, 0, stream_>>>(view(), keys, n, ids, overflow.as<unsigned long long>());
+      AB_CUDA(cudaGetLastError());
+      ++*launches_;
+      unsigned long long over = 0;
+      AB_CUDA(cudaMemcpyAsync(&over, overflow.p, sizeof over, cudaMemcpyDeviceToHost, stream_));
+      AB_CUDA(cudaStreamSynchronize(stream_));
+      if (over == 0) return;
+      stalls = over < left || n_buckets_ < free_buckets ? 0 : stalls + 1;
+      left = over;
+      AB_REQUIRE(stalls < RESTORE_STALLS, ARROYO_B200_RUNTIME,
+                 "restored keys whose dictionary bucket is out of ids still do not fit after the dictionary grew");
+      grow_step();
+    }
+  }
+
+ private:
+  cudaStream_t stream_ = nullptr;
+  int num_sms_ = 0;
+  bool keyed_ = false;
+  unsigned int* n_total_ = nullptr;
+  uint64_t* launches_ = nullptr;
+  uint64_t n_buckets_ = 0, id_cap_ = 0;
+  DevBuf slots_, nkeys_, id_keys_;
+
+  int grid(uint64_t items) const { return (int)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, (uint64_t)num_sms_ * 8)); }
+};
 
 }  // namespace ab

@@ -20,8 +20,8 @@
 //           id, compacted from the snapshot, [key?, per aggregate its accumulator state, _timestamp, _generation].
 //           The reference writes at every flush; writing at a checkpoint the keys flushed since the last export leaves
 //           the same latest row per key.  Every export carries one generation, one above the last;
-//   restore on_start (initialize :446-503) reads table "a" back: the keys go into the dictionary (growing it when a
-//           bucket runs out of ids), the row with the largest (_generation, position) wins per key and seeds both the
+//   restore on_start (initialize :446-503) reads table "a" back: the keys go into the dictionary (BucketDict::place,
+//           which grows it when a bucket runs out of ids), the row with the largest (_generation, position) wins per key and seeds both the
 //           live accumulators and the previous-flush snapshot, so the first flush retracts what the uninterrupted run
 //           would have retracted.
 // Output rows: [key?, aggregates..., _timestamp, is_retract] -- retractions first, then appends (a key's retraction
@@ -201,28 +201,14 @@ __global__ void __launch_bounds__(256) upd_export_kernel(const __grid_constant__
 // Restore: rows of table "a" in batch order, one thread per row.
 struct URestore {
   UState st;
-  BDict dict;
-  const long long* key;
   const unsigned long long* gen;
   const unsigned long long* val[MAX_ACC];  // per accumulator; val[0] null: every row counts one
   const long long* ts;
-  unsigned int* ids;              // per row
+  const unsigned int* ids;        // per row, from BucketDict::place
   unsigned long long* best_gen;   // per id
   long long* best_pos;            // per id, -1: no row
-  unsigned long long* overflow;   // rows whose bucket is out of ids
   long long n;
-  int keyed;
 };
-
-__global__ void __launch_bounds__(256) upd_restore_insert_kernel(const __grid_constant__ URestore p) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < p.n; i += stride) {
-    const uint32_t id = p.keyed ? bd_lookup_or_insert(p.dict, p.key[i]) : 0u;
-    p.ids[i] = id;
-    if (id >= ID_OVERFLOW) atomicAdd(p.overflow, 1ull);
-  }
-}
 
 // the largest generation per id, then the last row of that generation
 __global__ void __launch_bounds__(256) upd_restore_gen_kernel(const __grid_constant__ URestore p) {
@@ -330,10 +316,10 @@ class UpdatingAggOp final : public OpBase {
  private:
   AggPlan plan_;
   std::string key_format_ = "l";
-  // dictionary + state
-  uint64_t n_buckets_ = 1, id_cap_ = 0;
+  // dictionary (its key counter in n_total_) + per-id state
+  BucketDict dict_;
   uint32_t total_keys_ = 0;
-  DevBuf slots_, bucket_nkeys_, id_keys_, n_total_;
+  DevBuf n_total_;
   DevBuf cur_, prev_, cur_ts_, prev_ts_, touched_, flushed_, list_, counters_;  // counters_: [n_touched, retractions, appends, pad] u32 + deferred u64
   AggStaging staging_;
   // deferred rows (key, ts, values): two sets, one re-ingested while the other takes the rows that defer again
@@ -359,9 +345,8 @@ class UpdatingAggOp final : public OpBase {
   };
   std::vector<StateCol> state_layout() const;
 
-  BDict dict_view() const;
   UState state_view() const;
-  void alloc_state(uint64_t n_buckets);
+  void alloc_state();
   void grow();
   void reserve_defer(int set, uint64_t rows);
   void drain_deferred();
@@ -383,21 +368,13 @@ UpdatingAggOp::UpdatingAggOp(const ArroyoB200OpConfig& c) {
   AB_CUDA(cudaMemsetAsync(counters_.p, 0, 32, stream_));
   n_total_.alloc(4);
   AB_CUDA(cudaMemsetAsync(n_total_.p, 0, 4, stream_));
-  alloc_state(plan_.keyed ? bd_buckets_for(c.expected_keys ? c.expected_keys : (1ull << 16)) : 1);
+  dict_.init(stream_, num_sms_, plan_.keyed, n_total_.as<unsigned int>(), &st_.kernel_launches);
+  dict_.alloc(plan_.keyed ? bd_buckets_for(c.expected_keys ? c.expected_keys : (1ull << 16)) : 1);
+  alloc_state();
   AB_CUDA(cudaStreamSynchronize(stream_));
 }
 
 UpdatingAggOp::~UpdatingAggOp() { drain_stream(); }
-
-BDict UpdatingAggOp::dict_view() const {
-  BDict d{};
-  d.slots = slots_.as<BSlot>();
-  d.nkeys = bucket_nkeys_.as<unsigned int>();
-  d.id_keys = id_keys_.as<long long>();
-  d.n_total = n_total_.as<unsigned int>();
-  d.n_buckets = (uint32_t)n_buckets_;
-  return d;
-}
 
 UState UpdatingAggOp::state_view() const {
   UState s{};
@@ -409,7 +386,7 @@ UState UpdatingAggOp::state_view() const {
   s.flushed = flushed_.as<unsigned char>();
   s.list = list_.as<unsigned int>();
   s.n_touched = counters_.as<unsigned int>();
-  s.id_cap = id_cap_;
+  s.id_cap = dict_.id_cap();
   s.n_acc = plan_.n_acc;
   for (int a = 0; a < plan_.n_acc; ++a) {
     s.acc_kind[a] = plan_.acc_kind[a];
@@ -418,63 +395,44 @@ UState UpdatingAggOp::state_view() const {
   return s;
 }
 
-void UpdatingAggOp::alloc_state(uint64_t n_buckets) {
-  n_buckets_ = n_buckets;
-  id_cap_ = bd_id_cap(n_buckets_);
-  AB_REQUIRE(id_cap_ < (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
-  id_keys_.alloc(id_cap_ * 8);
-  bd_fill_keys_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(id_keys_.as<long long>(), id_cap_);
+// The per-id state for the dictionary's id capacity, every id at its identity.
+void UpdatingAggOp::alloc_state() {
+  const uint64_t id_cap = dict_.id_cap();
+  cur_.alloc((size_t)plan_.n_acc * id_cap * 8);
+  prev_.alloc((size_t)plan_.n_acc * id_cap * 8);
+  cur_ts_.alloc(id_cap * 8);
+  prev_ts_.alloc(id_cap * 8);
+  touched_.alloc(id_cap * 4);
+  flushed_.alloc(id_cap);
+  list_.alloc(id_cap * 4);
+  upd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(state_view(), id_cap);
   AB_CUDA(cudaGetLastError());
-  bucket_nkeys_.alloc(n_buckets_ * 4);
-  AB_CUDA(cudaMemsetAsync(bucket_nkeys_.p, 0, n_buckets_ * 4, stream_));
-  if (plan_.keyed) {
-    slots_.alloc(n_buckets_ * BD_KS * sizeof(BSlot));
-    bd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(slots_.as<BSlot>(), n_buckets_ * BD_KS);
-    AB_CUDA(cudaGetLastError());
-  }
-  cur_.alloc((size_t)plan_.n_acc * id_cap_ * 8);
-  prev_.alloc((size_t)plan_.n_acc * id_cap_ * 8);
-  cur_ts_.alloc(id_cap_ * 8);
-  prev_ts_.alloc(id_cap_ * 8);
-  touched_.alloc(id_cap_ * 4);
-  flushed_.alloc(id_cap_);
-  list_.alloc(id_cap_ * 4);
-  upd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(state_view(), id_cap_);
-  AB_CUDA(cudaGetLastError());
-  st_.kernel_launches += 2;
+  ++st_.kernel_launches;
 }
 
-// Doubles the bucket count: keys are re-inserted (ids change), the per-id state and the touched list follow the map.
-// A bucket's keys split between the two buckets that replace it, so the rehash itself never runs out of ids.
+// Doubles the bucket count (BucketDict::grow, refused before anything moves: the operator stays usable); the per-id
+// state and the touched list follow the old -> new id map.
 void UpdatingAggOp::grow() {
-  // refused before anything moves: the operator stays usable
-  AB_REQUIRE(bd_id_cap(n_buckets_ * 2) < (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
-  const BDict old_d = dict_view();
   const UState old_s = state_view();
-  const uint32_t old_ids = (uint32_t)(BD_ID_BASE + n_buckets_ * BD_CAPB);
-  const uint64_t old_cap = id_cap_;
-  DevBuf k_slots = std::move(slots_), k_nk = std::move(bucket_nkeys_), k_keys = std::move(id_keys_), k_cur = std::move(cur_),
-         k_prev = std::move(prev_), k_cts = std::move(cur_ts_), k_pts = std::move(prev_ts_), k_t = std::move(touched_),
-         k_f = std::move(flushed_), k_list = std::move(list_);
+  const BdGrowth g = dict_.grow();
+  DevBuf k_cur = std::move(cur_), k_prev = std::move(prev_), k_cts = std::move(cur_ts_), k_pts = std::move(prev_ts_),
+         k_t = std::move(touched_), k_f = std::move(flushed_), k_list = std::move(list_);
   unsigned int h_touched = 0;
   AB_CUDA(cudaMemcpyAsync(&h_touched, counters_.p, 4, cudaMemcpyDeviceToHost, stream_));
-  AB_CUDA(cudaMemsetAsync(n_total_.p, 0, 4, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
-  alloc_state(n_buckets_ * 2);
-  DevBuf map((size_t)old_cap * 4);
-  const int grid = (int)std::min<uint64_t>((old_ids + 255) / 256, (uint64_t)num_sms_ * 8);
-  bd_rehash_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_d, dict_view(), old_ids, map.as<uint32_t>());
+  alloc_state();
+  const int grid = (int)std::min<uint64_t>((g.old_ids + 255) / 256, (uint64_t)num_sms_ * 8);
+  upd_permute_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_s, state_view(), g.map.as<uint32_t>(), g.old_ids);
   AB_CUDA(cudaGetLastError());
-  upd_permute_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_s, state_view(), map.as<uint32_t>(), old_ids);
-  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
   if (h_touched) {
     AB_CUDA(cudaMemcpyAsync(list_.p, k_list.p, (size_t)h_touched * 4, cudaMemcpyDeviceToDevice, stream_));
-    upd_remap_list_kernel<<<(h_touched + 255) / 256, 256, 0, stream_>>>(list_.as<unsigned int>(), h_touched, map.as<uint32_t>());
+    upd_remap_list_kernel<<<(h_touched + 255) / 256, 256, 0, stream_>>>(list_.as<unsigned int>(), h_touched, g.map.as<uint32_t>());
     AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
   }
   AB_CUDA(cudaMemcpyAsync(&total_keys_, n_total_.p, 4, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
-  st_.kernel_launches += 3;
 }
 
 void UpdatingAggOp::reserve_defer(int set, uint64_t rows) {
@@ -525,7 +483,7 @@ void UpdatingAggOp::drain_deferred() {
 void UpdatingAggOp::ensure_room(uint64_t new_rows) {
   if (!plan_.keyed) return;
   drain_deferred();
-  while ((uint64_t)total_keys_ + new_rows > n_buckets_ * (uint64_t)BD_MEAN) grow();
+  while ((uint64_t)total_keys_ + new_rows > dict_.n_buckets() * (uint64_t)BD_MEAN) grow();
 }
 
 void UpdatingAggOp::ingest(const AggCols& d, int64_t n) {
@@ -537,7 +495,7 @@ void UpdatingAggOp::ingest(const AggCols& d, int64_t n) {
   p.n = n;
   p.keyed = plan_.keyed ? 1 : 0;
   p.n_vals = plan_.n_vals;
-  p.dict = dict_view();
+  p.dict = dict_.view();
   p.st = state_view();
   if (plan_.keyed) {  // every row of the launch may defer (all rows of a key whose bucket is full do)
     reserve_defer(defer_cur_, (uint64_t)n);
@@ -605,7 +563,7 @@ void UpdatingAggOp::flush_to(BatchesPriv* out) {
   }
   UFlush p{};
   p.st = state_view();
-  p.id_keys = id_keys_.as<long long>();
+  p.id_keys = dict_.id_keys();
   p.n = n;
   p.keyed = plan_.keyed ? 1 : 0;
   p.n_aggs = plan_.n_aggs;
@@ -691,7 +649,7 @@ std::vector<UpdatingAggOp::StateCol> UpdatingAggOp::state_layout() const {
 void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
   set_device();
   if (unexported_ == 0) return;
-  const uint64_t n_ids = plan_.keyed ? BD_ID_BASE + n_buckets_ * BD_CAPB : 1;
+  const uint64_t n_ids = plan_.keyed ? dict_.n_ids() : 1;
   const uint64_t cap = std::min<uint64_t>(unexported_, n_ids);
   if (cap > state_cap_) {
     state_cap_ = std::max<uint64_t>(cap, 1024);
@@ -703,7 +661,7 @@ void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
   AB_CUDA(cudaMemsetAsync(count, 0, 4, stream_));
   UExport p{};
   p.st = state_view();
-  p.id_keys = id_keys_.as<long long>();
+  p.id_keys = dict_.id_keys();
   p.n_ids = n_ids;
   p.o_key = s_key_.as<long long>();
   for (int a = 0; a < plan_.n_acc; ++a) p.o_acc[a] = s_acc_[a].as<unsigned long long>();
@@ -811,8 +769,12 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   set_device();
   if (plan_.keyed) {
     key_format_ = batches[0][0].format;
-    const uint64_t b = bd_buckets_for((uint64_t)total);  // the dictionary holds every restored key without growing
-    if (b > n_buckets_) alloc_state(b);
+    // the state is still empty: size the dictionary once to hold every restored key without growing
+    const uint64_t b = bd_buckets_for((uint64_t)total);
+    if (b > dict_.n_buckets()) {
+      dict_.alloc(b);
+      alloc_state();
+    }
   }
   // the columns of every batch, concatenated in batch order: a row's position is its index
   auto upload = [&](int c, DevBuf& dst) {
@@ -839,42 +801,18 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   uint64_t max_gen = 0;
   for (int64_t b = 0; b < n; ++b)
     for (int64_t i = 0; i < rows[b]; ++i) max_gen = std::max<uint64_t>(max_gen, batches[b][gen_col].data[i]);
-  DevBuf ids((size_t)total * 4), overflow(8);
-  p.key = d_key.as<long long>();
+  DevBuf ids((size_t)total * 4);
+  dict_.place(plan_.keyed ? d_key.as<long long>() : nullptr, total, ids.as<uint32_t>(), [&] { grow(); });
   p.gen = d_gen.as<unsigned long long>();
   p.ts = d_ts.as<long long>();
   p.ids = ids.as<unsigned int>();
-  p.overflow = overflow.as<unsigned long long>();
   p.n = total;
-  p.keyed = plan_.keyed ? 1 : 0;
   const int grid = std::max(1, (int)std::min<int64_t>((total + 255) / 256, (int64_t)num_sms_ * 8));
-  // keys whose bucket is out of ids: the dictionary doubles and every row looks its key up again (placed keys keep
-  // theirs).  A dictionary sized for few rows has few buckets, each covering a wide hash range, so crowded keys may
-  // need several doublings to split: below the default size (2^16 keys) it doubles freely; from there on,
-  // RESTORE_STALLS doublings in a row that place none of the rest give up
-  constexpr int RESTORE_STALLS = 4;
-  const uint64_t free_buckets = bd_buckets_for(1ull << 16);
-  for (uint64_t left = UINT64_MAX, stalls = 0;;) {
-    p.dict = dict_view();
-    AB_CUDA(cudaMemsetAsync(overflow.p, 0, 8, stream_));
-    upd_restore_insert_kernel<<<grid, 256, 0, stream_>>>(p);
-    AB_CUDA(cudaGetLastError());
-    ++st_.kernel_launches;
-    unsigned long long over = 0;
-    AB_CUDA(cudaMemcpyAsync(&over, overflow.p, 8, cudaMemcpyDeviceToHost, stream_));
-    AB_CUDA(cudaStreamSynchronize(stream_));
-    if (over == 0) break;
-    stalls = over < left || n_buckets_ < free_buckets ? 0 : stalls + 1;
-    left = over;
-    AB_REQUIRE(stalls < RESTORE_STALLS, ARROYO_B200_RUNTIME,
-               "updating aggregate: restored keys whose dictionary bucket is out of ids still do not fit after the "
-               "dictionary grew");
-    grow();
-  }
   p.st = state_view();
-  DevBuf best_gen(id_cap_ * 8), best_pos(id_cap_ * 8);
-  AB_CUDA(cudaMemsetAsync(best_gen.p, 0, id_cap_ * 8, stream_));
-  AB_CUDA(cudaMemsetAsync(best_pos.p, 0xFF, id_cap_ * 8, stream_));  // -1
+  const uint64_t id_cap = dict_.id_cap();
+  DevBuf best_gen(id_cap * 8), best_pos(id_cap * 8);
+  AB_CUDA(cudaMemsetAsync(best_gen.p, 0, id_cap * 8, stream_));
+  AB_CUDA(cudaMemsetAsync(best_pos.p, 0xFF, id_cap * 8, stream_));  // -1
   p.best_gen = best_gen.as<unsigned long long>();
   p.best_pos = best_pos.as<long long>();
   upd_restore_gen_kernel<<<grid, 256, 0, stream_>>>(p);

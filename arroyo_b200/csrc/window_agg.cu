@@ -527,32 +527,22 @@ __global__ void __launch_bounds__(THREADS, AB_INGEST_MIN_BLOCKS) ingest_kernel(c
 #include "ingest_two_pass.cuh"
 
 // Restore: merge a partial-state batch (AggregateExec(Partial) output written at a checkpoint,
-// sliding_aggregating_window.rs:725-733) into one pane block.
+// sliding_aggregating_window.rs:725-733) into one pane block, by the ids BucketDict::place gave its keys.
 struct PartialParams {
-  const long long* key;
+  const uint32_t* ids;
   const unsigned long long* state[MAX_ACC];  // state[0] = rows
   long long n;
-  int keyed;
   int n_acc;
   int acc_kind[MAX_ACC];
-  BDict dict;
   unsigned long long* pane;
   unsigned long long id_cap;
-  Counters* counters;
 };
 
 __global__ void ingest_partial_kernel(const __grid_constant__ PartialParams p) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long stride = (long long)gridDim.x * blockDim.x;
   for (; i < p.n; i += stride) {
-    uint32_t id = 0;
-    if (p.keyed) {
-      id = bd_lookup_or_insert(p.dict, p.key[i]);
-      if (id >= ID_OVERFLOW) {
-        atomicAdd(&p.counters->lost, 1ull);
-        continue;
-      }
-    }
+    const uint32_t id = p.ids[i];
     for (int a = 0; a < p.n_acc; ++a) {
       unsigned long long* dst = p.pane + (unsigned long long)a * p.id_cap + id;
       unsigned long long v = p.state[a][i];
@@ -861,10 +851,9 @@ class WindowAggOp final : public OpBase {
   bool profile_;
   std::string key_format_ = "l";
 
-  // dictionary (bdict.cuh): n_buckets_ buckets of BD_KS slots; ids = BD_ID_BASE + bucket * BD_CAPB + index
-  uint64_t id_cap_ = 0;
-  uint64_t n_buckets_ = 1;
-  DevBuf slots_, bucket_nkeys_, id_keys_;
+  // dictionary (bdict.cuh): buckets of BD_KS slots; ids = BD_ID_BASE + bucket * BD_CAPB + index; its key counter is
+  // Counters::n_keys
+  BucketDict dict_;
   // bookkeeping the kernels report back, one contiguous buffer = one device->host copy per launch:
   // [Counters | slot_rows[MAX_RING]].  slot_rows (on-time rows per ring slot) is cumulative; the host works with the
   // difference between consecutive launches (no per-launch memset).
@@ -873,7 +862,6 @@ class WindowAggOp final : public OpBase {
   Counters* d_counters() const { return reinterpret_cast<Counters*>(book_.p); }
   unsigned long long* d_slot_rows() const { return reinterpret_cast<unsigned long long*>((char*)book_.p + BOOK_SLOT_OFF); }
   std::vector<unsigned long long> slot_rows_seen_;
-  uint32_t n_keys_host_ = 1;       // ids in use = the id range the element-wise kernels walk (all of it: bucket ranges)
   uint32_t total_keys_host_ = 0;   // keys in the dictionary (statistics, growth policy)
   uint32_t dict_full_seen_ = 0;
   // two-pass ingest (ingest_two_pass.cuh)
@@ -886,7 +874,6 @@ class WindowAggOp final : public OpBase {
   mutable int two_pass_pause_ = 0;  // launches left on the one-pass kernel after a skewed launch
   bool two_pass_eligible(uint64_t rows) const;
   void launch_two_pass(IngestParams& p, uint64_t rows, long long tiles_direct);
-  BDict dict_view() const;
   // asynchronous emission (begin_watermark / poll_watermark): windows are copied back on a second stream so the
   // device->host traffic overlaps the host->device traffic of the batches that follow
   cudaStream_t out_stream_ = nullptr;
@@ -991,12 +978,11 @@ class WindowAggOp final : public OpBase {
   size_t emit_events_used_ = 0;
 
   // helpers
-  void alloc_dictionary(uint64_t n_buckets);
   void preallocate();
+  template <class Fill>
+  void rebuild_blocks(Fill fill);
   void grow_ids();
-  void apply_l2_policy();
   void promote_avg();
-  void relayout_blocks(int old_n_acc, const std::vector<std::pair<int, int>>& f64_from);
   unsigned long long* acquire_block();
   void release_block(unsigned long long* blk);
   void init_block(unsigned long long* blk, uint64_t n_ids);
@@ -1081,7 +1067,9 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
 
   // one bucket per ~BD_MEAN expected keys (the bucket count doubles when a bucket runs out of ids)
   uint64_t want = c.expected_keys ? c.expected_keys : (1ull << 16);
-  alloc_dictionary(plan_.keyed ? bd_buckets_for(want) : 1);
+  dict_.init(stream_, num_sms_, plan_.keyed, (unsigned int*)((char*)book_.p + offsetof(Counters, n_keys)),
+             &st_.kernel_launches);
+  dict_.alloc(plan_.keyed ? bd_buckets_for(want) : 1);
   {
     const char* e = getenv("ARROYO_B200_NO_TWO_PASS");
     two_pass_enabled_ = !(e && atoi(e) != 0) && !(c.flags & ARROYO_B200_FLAG_NO_TWO_PASS);
@@ -1134,19 +1122,19 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
 // cudaMalloc inside process_batch / handle_watermark serialises the device and showed up as milliseconds per
 // step in short runs (the driver's 5-warm-up / 20-step scaling runs timed little else).
 void WindowAggOp::preallocate() {
-  const size_t block_bytes = (size_t)plan_.n_acc * id_cap_ * sizeof(unsigned long long);
+  const size_t block_bytes = (size_t)plan_.n_acc * dict_.id_cap() * sizeof(unsigned long long);
   size_t want = (sliding_ ? (size_t)(width_ / slide_) : 1) + 4 + (running_mode_ ? 1 : 0);
   const size_t budget = (size_t)4 << 30;
   want = std::min<size_t>(std::min<size_t>(want, 64), std::max<size_t>(budget / std::max<size_t>(block_bytes, 1), 4));
   for (size_t i = 0; i < want; ++i) {
     pane_storage_.emplace_back(block_bytes);
     auto* blk = pane_storage_.back().as<unsigned long long>();
-    init_block(blk, id_cap_);
+    init_block(blk, dict_.id_cap());
     free_panes_.emplace_back(blk, 0);  // already holds the identity: nothing to reset when it is acquired
   }
   for (int c = 0; c < 2 + plan_.n_vals; ++c) defer_[0][c].alloc(defer_cap_ * 8);
-  out_set(0, id_cap_);
-  out_set(1, id_cap_);
+  out_set(0, dict_.id_cap());
+  out_set(1, dict_.id_cap());
 }
 
 WindowAggOp::~WindowAggOp() {
@@ -1190,61 +1178,11 @@ WindowAggOp::~WindowAggOp() {
   }
 }
 
-void WindowAggOp::alloc_dictionary(uint64_t n_buckets) {
-  n_buckets_ = n_buckets;
-  id_cap_ = bd_id_cap(n_buckets_);
-  AB_REQUIRE(id_cap_ < (1ull << 31), ARROYO_B200_RUNTIME, "key dictionary too large");
-  n_keys_host_ = (uint32_t)(BD_ID_BASE + n_buckets_ * BD_CAPB);
-  id_keys_.alloc(id_cap_ * sizeof(long long));
-  bd_fill_keys_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(id_keys_.as<long long>(), id_cap_);
-  AB_CUDA(cudaGetLastError());
-  bucket_nkeys_.alloc(n_buckets_ * sizeof(unsigned int));
-  AB_CUDA(cudaMemsetAsync(bucket_nkeys_.p, 0, n_buckets_ * sizeof(unsigned int), stream_));
-  if (plan_.keyed) {
-    slots_.alloc(n_buckets_ * BD_KS * sizeof(BSlot));
-    bd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(slots_.as<BSlot>(), n_buckets_ * BD_KS);
-    AB_CUDA(cudaGetLastError());
-    ++st_.kernel_launches;
-    apply_l2_policy();
-  }
-}
-
-BDict WindowAggOp::dict_view() const {
-  BDict d{};
-  d.slots = slots_.as<BSlot>();
-  d.nkeys = bucket_nkeys_.as<unsigned int>();
-  d.id_keys = id_keys_.as<long long>();
-  d.n_total = (unsigned int*)((char*)book_.p + offsetof(Counters, n_keys));
-  d.n_buckets = (uint32_t)n_buckets_;
-  return d;
-}
-
-// ARROYO_B200_L2_PERSIST=1: ask L2 to keep the key dictionary resident (persisting access-policy window on the
-// operator's stream); everything else the stream touches is treated as streaming.
-void WindowAggOp::apply_l2_policy() {
-  const char* e = getenv("ARROYO_B200_L2_PERSIST");
-  if (!e || atoi(e) == 0 || !slots_.p) return;
-  int max_persist = 0, max_window = 0;
-  cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, device_);
-  cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, device_);
-  size_t bytes = std::min<size_t>(n_buckets_ * BD_KS * sizeof(BSlot), (size_t)std::max(max_window, 0));
-  if (bytes == 0 || max_persist <= 0) return;
-  cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, std::min<size_t>(bytes, (size_t)max_persist));
-  cudaStreamAttrValue attr{};
-  attr.accessPolicyWindow.base_ptr = slots_.p;
-  attr.accessPolicyWindow.num_bytes = bytes;
-  attr.accessPolicyWindow.hitRatio = std::min(1.0f, (float)max_persist / (float)bytes);
-  attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-  attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-  cudaStreamSetAttribute(stream_, cudaStreamAttributeAccessPolicyWindow, &attr);
-  cudaGetLastError();
-}
-
 void WindowAggOp::init_block(unsigned long long* blk, uint64_t n_ids) {
   if (n_ids == 0) return;
   InitParams ip{};
   ip.pane = blk;
-  ip.id_cap = id_cap_;
+  ip.id_cap = dict_.id_cap();
   ip.n = n_ids;
   ip.n_acc = plan_.n_acc;
   for (int a = 0; a < plan_.n_acc; ++a) ip.acc_kind[a] = plan_.acc_kind[a];
@@ -1261,15 +1199,15 @@ unsigned long long* WindowAggOp::acquire_block() {
     init_block(pr.first, pr.second);
     return pr.first;
   }
-  pane_storage_.emplace_back((size_t)plan_.n_acc * id_cap_ * sizeof(unsigned long long));
+  pane_storage_.emplace_back((size_t)plan_.n_acc * dict_.id_cap() * sizeof(unsigned long long));
   auto* blk = pane_storage_.back().as<unsigned long long>();
-  init_block(blk, id_cap_);
+  init_block(blk, dict_.id_cap());
   return blk;
 }
 
 void WindowAggOp::release_block(unsigned long long* blk) {
   if (!blk) return;
-  free_panes_.emplace_back(blk, std::min<uint64_t>(id_cap_, (uint64_t)n_keys_host_ + 1));
+  free_panes_.emplace_back(blk, std::min<uint64_t>(dict_.id_cap(), (uint64_t)dict_.n_ids() + 1));
 }
 
 // new[a][map[i]] = old[a][i] for every old id that holds a key
@@ -1285,60 +1223,54 @@ __global__ void permute_block_kernel(const unsigned long long* __restrict__ old_
   }
 }
 
-// Doubles the bucket count: every key is re-inserted into the new dictionary (its id changes), and every live pane
-// block is permuted with the old -> new id map.
-void WindowAggOp::grow_ids() {
-  AB_REQUIRE(plan_.keyed, ARROYO_B200_RUNTIME, "grow_ids on an unkeyed aggregate");
-  const uint64_t old_cap = id_cap_;
-  const uint32_t old_ids = n_keys_host_;
-  BDict old_d = dict_view();
-  DevBuf old_slots = std::move(slots_), old_nkeys = std::move(bucket_nkeys_), old_keys = std::move(id_keys_);
-  old_d.slots = old_slots.as<BSlot>();
-  old_d.nkeys = old_nkeys.as<unsigned int>();
-  old_d.id_keys = old_keys.as<long long>();
-  const unsigned int zero = 0;
-  AB_CUDA(cudaMemcpyAsync((char*)book_.p + offsetof(Counters, n_keys), &zero, sizeof zero, cudaMemcpyHostToDevice, stream_));
-  alloc_dictionary(n_buckets_ * 2);
-  const uint64_t new_cap = id_cap_;
-  DevBuf map((size_t)old_cap * sizeof(uint32_t));
-  {
-    const int grid = (int)std::min<uint64_t>((old_ids + 255) / 256, (uint64_t)num_sms_ * 8);
-    bd_rehash_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_d, dict_view(), old_ids, map.as<uint32_t>());
-    AB_CUDA(cudaGetLastError());
-    ++st_.kernel_launches;
-  }
+// Replaces every live pane block (the panes' active and frozen blocks, the zombies', the running window) with a new
+// block of the current id capacity and accumulator count, at the identity, that fill(old block, new block) fills from
+// the old one.  Spare blocks are dropped: acquire_block allocates at the new size.
+template <class Fill>
+void WindowAggOp::rebuild_blocks(Fill fill) {
   std::vector<DevBuf> new_storage;
-  auto migrate = [&](unsigned long long* old_blk) -> unsigned long long* {
-    if (!old_blk) return nullptr;
-    new_storage.emplace_back((size_t)plan_.n_acc * new_cap * sizeof(unsigned long long));
+  auto rebuild = [&](unsigned long long*& blk) {
+    if (!blk) return;
+    new_storage.emplace_back((size_t)plan_.n_acc * dict_.id_cap() * sizeof(unsigned long long));
     auto* nb = new_storage.back().as<unsigned long long>();
-    init_block(nb, new_cap);
-    const int grid = (int)std::min<uint64_t>((old_ids + 255) / 256, (uint64_t)num_sms_ * 8);
-    permute_block_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_blk, nb, map.as<uint32_t>(), old_ids, old_cap, new_cap,
-                                                               plan_.n_acc);
-    AB_CUDA(cudaGetLastError());
-    ++st_.kernel_launches;
-    return nb;
+    init_block(nb, dict_.id_cap());
+    fill(blk, nb);
+    blk = nb;
   };
   for (auto& kv : panes_) {
-    kv.second.dev = migrate(kv.second.dev);
-    kv.second.frozen = migrate(kv.second.frozen);
+    rebuild(kv.second.dev);
+    rebuild(kv.second.frozen);
     if (kv.second.slot >= 0) h_pane_ptrs_[kv.second.slot] = kv.second.dev;
   }
   for (auto& kv : zombies_) {
-    kv.second.dev = migrate(kv.second.dev);
-    kv.second.frozen = migrate(kv.second.frozen);
+    rebuild(kv.second.dev);
+    rebuild(kv.second.frozen);
   }
-  running_ = migrate(running_);
+  rebuild(running_);
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  free_panes_.clear();
+  pane_storage_ = std::move(new_storage);
+  ring_dirty_ = true;
+}
+
+// Doubles the bucket count (BucketDict::grow: every key gets a new id), and permutes every live pane block with the
+// old -> new id map.
+void WindowAggOp::grow_ids() {
+  const BdGrowth g = dict_.grow();
+  const uint64_t new_cap = dict_.id_cap();
+  const int grid = (int)std::min<uint64_t>((g.old_ids + 255) / 256, (uint64_t)num_sms_ * 8);
+  rebuild_blocks([&](const unsigned long long* old_blk, unsigned long long* nb) {
+    permute_block_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_blk, nb, g.map.as<uint32_t>(), g.old_ids, g.old_cap,
+                                                               new_cap, plan_.n_acc);
+    AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
+  });
   Counters c{};
   AB_CUDA(cudaMemcpyAsync(&c, book_.p, sizeof c, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
   total_keys_host_ = c.n_keys;
-  free_panes_.clear();
-  pane_storage_ = std::move(new_storage);
   // (output sets stay: a caller may still hold the last emission's device pointers; out_set() grows them on demand)
-  part_cap_ = 0;      // the partition buffer is sized by the bucket count
-  ring_dirty_ = true;
+  part_cap_ = 0;  // the partition buffer is sized by the bucket count
 }
 
 // fsum[id] = (double)(int64)sum[id]
@@ -1346,43 +1278,6 @@ __global__ void i64_to_f64_kernel(const unsigned long long* __restrict__ src, un
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (; i < n; i += stride) dst[i] = (unsigned long long)__double_as_longlong((double)(long long)src[i]);
-}
-
-// Re-creates every live block with the current plan_.n_acc; accumulators [0, old_n_acc) are copied, and each
-// (new index, source index) pair in f64_from is filled with the f64 image of the source integer sum.
-void WindowAggOp::relayout_blocks(int old_n_acc, const std::vector<std::pair<int, int>>& f64_from) {
-  std::vector<DevBuf> new_storage;
-  const uint32_t n_valid = (uint32_t)std::min<uint64_t>(n_keys_host_, id_cap_);
-  auto migrate = [&](unsigned long long* old_blk) -> unsigned long long* {
-    if (!old_blk) return nullptr;
-    new_storage.emplace_back((size_t)plan_.n_acc * id_cap_ * sizeof(unsigned long long));
-    auto* nb = new_storage.back().as<unsigned long long>();
-    init_block(nb, id_cap_);
-    for (int a = 0; a < old_n_acc; ++a)
-      AB_CUDA(cudaMemcpyAsync(nb + (size_t)a * id_cap_, old_blk + (size_t)a * id_cap_,
-                              (size_t)n_valid * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream_));
-    for (auto& pr : f64_from) {
-      int grid = (int)std::min<uint64_t>((n_valid + 255) / 256 + 1, (uint64_t)num_sms_ * 8);
-      i64_to_f64_kernel<<<grid, 256, 0, stream_>>>(old_blk + (size_t)pr.second * id_cap_, nb + (size_t)pr.first * id_cap_, n_valid);
-      AB_CUDA(cudaGetLastError());
-      ++st_.kernel_launches;
-    }
-    return nb;
-  };
-  for (auto& kv : panes_) {
-    kv.second.dev = migrate(kv.second.dev);
-    kv.second.frozen = migrate(kv.second.frozen);
-    if (kv.second.slot >= 0) h_pane_ptrs_[kv.second.slot] = kv.second.dev;
-  }
-  for (auto& kv : zombies_) {
-    kv.second.dev = migrate(kv.second.dev);
-    kv.second.frozen = migrate(kv.second.frozen);
-  }
-  running_ = migrate(running_);
-  AB_CUDA(cudaStreamSynchronize(stream_));
-  free_panes_.clear();
-  pane_storage_ = std::move(new_storage);
-  ring_dirty_ = true;
 }
 
 // Leaves exact-sum AVG: every AVG gets its own f64 accumulator, seeded from the (still exact) integer sums.
@@ -1424,7 +1319,21 @@ void WindowAggOp::promote_avg() {
     release_block(running_);
     running_ = nullptr;
   }
-  relayout_blocks(old_n_acc, f64_from);
+  // every live block again with the new accumulators: [0, old_n_acc) copied, each (new, source) pair in f64_from filled
+  // with the f64 image of the source integer sum
+  const uint64_t cap = dict_.id_cap();
+  const uint32_t n_valid = (uint32_t)std::min<uint64_t>(dict_.n_ids(), cap);
+  rebuild_blocks([&](const unsigned long long* old_blk, unsigned long long* nb) {
+    for (int a = 0; a < old_n_acc; ++a)
+      AB_CUDA(cudaMemcpyAsync(nb + (size_t)a * cap, old_blk + (size_t)a * cap, (size_t)n_valid * sizeof(unsigned long long),
+                              cudaMemcpyDeviceToDevice, stream_));
+    for (auto& pr : f64_from) {
+      const int grid = (int)std::min<uint64_t>((n_valid + 255) / 256 + 1, (uint64_t)num_sms_ * 8);
+      i64_to_f64_kernel<<<grid, 256, 0, stream_>>>(old_blk + (size_t)pr.second * cap, nb + (size_t)pr.first * cap, n_valid);
+      AB_CUDA(cudaGetLastError());
+      ++st_.kernel_launches;
+    }
+  });
 }
 
 // Gives pane `bin` a ring slot, creating the pane if needed.  Only called with no launch in flight (the slot_rows of a
@@ -1719,7 +1628,7 @@ void WindowAggOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols,
 bool WindowAggOp::two_pass_eligible(uint64_t rows) const {
   if (!two_pass_enabled_ || !plan_.keyed || rows_slot_ >= 0 || plan_.n_vals > 1 || plan_.n_acc > 2) return false;
   if (plan_.n_acc == 2 && plan_.acc_kind[1] != ACC_SUM_I64) return false;
-  if (n_buckets_ > (uint64_t)P1_NR) return false;
+  if (dict_.n_buckets() > (uint64_t)P1_NR) return false;
   if (max_bin_seen_ == LLONG_MIN) return false;  // no pane known yet: the first launch finds out where the stream is
   if (two_pass_pause_ > 0) {
     --two_pass_pause_;
@@ -1733,6 +1642,7 @@ bool WindowAggOp::two_pass_eligible(uint64_t rows) const {
 }
 
 void WindowAggOp::launch_two_pass(IngestParams& p, uint64_t rows, long long tiles) {
+  const uint64_t n_buckets = dict_.n_buckets();
   TwoPassParams tp{};
   // fast panes: the newest pane seen and the next one (in-order streams write nothing else)
   int nf = 0;
@@ -1750,9 +1660,9 @@ void WindowAggOp::launch_two_pass(IngestParams& p, uint64_t rows, long long tile
     tp.fast_ptr[f] = nullptr;
     tp.fast_slot[f] = 0;
   }
-  const uint32_t n_regions = (uint32_t)(TP_NP * n_buckets_);
+  const uint32_t n_regions = (uint32_t)(TP_NP * n_buckets);
   // a region holds a bucket's share of one pane's rows: mean rows / buckets, plus slack for the spread
-  const uint64_t mean = (uint64_t)launch_rows_ / n_buckets_ + 1;
+  const uint64_t mean = (uint64_t)launch_rows_ / n_buckets + 1;
   const uint32_t cap = (uint32_t)std::min<uint64_t>(((mean + mean / 4 + 2048 + 63) / 64) * 64, 1u << 30);
   if (part_cap_ != cap || !part_.p) {
     AB_CUDA(cudaStreamSynchronize(stream_));
@@ -1768,8 +1678,8 @@ void WindowAggOp::launch_two_pass(IngestParams& p, uint64_t rows, long long tile
   tp.cap = cap;
   // blocks per region in pass 2: enough blocks to fill the GPU when there are few buckets
   const uint32_t want_blocks = (uint32_t)num_sms_ * 2;
-  tp.slices = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((want_blocks + n_buckets_ - 1) / n_buckets_,
-                                                                 std::max<uint64_t>(1, rows / n_buckets_ / 4096)));
+  tp.slices = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((want_blocks + n_buckets - 1) / n_buckets,
+                                                                 std::max<uint64_t>(1, rows / n_buckets / 4096)));
   if (!two_pass_attr_set_) {
     AB_CUDA(cudaFuncSetAttribute(part_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P1_SMEM));
     AB_CUDA(cudaFuncSetAttribute(part_kernel<1, sig_of(ACC_SUM_I64)>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P1_SMEM));
@@ -1782,16 +1692,16 @@ void WindowAggOp::launch_two_pass(IngestParams& p, uint64_t rows, long long tile
   // blocks: the fourth round keeps 136 blocks busy and 160 idle for a whole bucket); cutting the buckets of that round
   // into slices turns it into a short round of part-buckets (each slice builds the bucket's table again).
   const uint32_t max_blocks = (uint32_t)num_sms_ * P2_BLOCKS_PER_SM;
-  tp.tail_first = (uint32_t)n_buckets_;
+  tp.tail_first = (uint32_t)n_buckets;
   tp.tail_slices = 1;
-  if (tp.slices == 1 && n_buckets_ > max_blocks && rows / n_buckets_ >= 2048) {
-    const uint32_t rest = (uint32_t)(n_buckets_ % max_blocks);
+  if (tp.slices == 1 && n_buckets > max_blocks && rows / n_buckets >= 2048) {
+    const uint32_t rest = (uint32_t)(n_buckets % max_blocks);
     if (rest && max_blocks / rest >= 2) {
-      tp.tail_first = (uint32_t)n_buckets_ - rest;
+      tp.tail_first = (uint32_t)n_buckets - rest;
       tp.tail_slices = std::min<uint32_t>(max_blocks / rest, 4);
     }
   }
-  const uint32_t n_work = tp.tail_first * tp.slices + ((uint32_t)n_buckets_ - tp.tail_first) * tp.tail_slices;
+  const uint32_t n_work = tp.tail_first * tp.slices + ((uint32_t)n_buckets - tp.tail_first) * tp.tail_slices;
   const int grid2 = (int)std::max<uint32_t>(1, std::min<uint32_t>(n_work, max_blocks));
   if (plan_.n_vals == 0) {
     part_kernel<0, 0><<<grid1, P1_THREADS, P1_SMEM, stream_>>>(p, tp);
@@ -1842,7 +1752,7 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
   p.n_segs = (int)segs_in.size();
   p.keyed = plan_.keyed ? 1 : 0;
   p.n_tiles = tiles;
-  p.dict = dict_view();
+  p.dict = dict_.view();
   p.slide_div = FastDivU64::make((uint64_t)slide_);
   p.slide = slide_;
   p.late_bin = late_bin_;
@@ -1855,7 +1765,7 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
   p.n_acc = plan_.n_acc;
   p.pane_bins = d_pane_bins_.as<long long>();
   p.pane_ptrs = d_pane_ptrs_.as<unsigned long long*>();
-  p.id_cap = id_cap_;
+  p.id_cap = dict_.id_cap();
   p.ring_inline = ring_ <= RING_INLINE ? 1 : 0;
   if (p.ring_inline)
     for (uint32_t i = 0; i < ring_; ++i) {
@@ -2050,7 +1960,7 @@ void WindowAggOp::drain_deferred() {
     // dictionary pressure: a bucket ran out of ids (its rows were deferred), or the mean bucket fill is past the
     // point where that becomes likely: double the bucket count
     if (plan_.keyed && (last_counters_.dict_full != dict_full_seen_ ||
-                   (uint64_t)last_counters_.n_keys > n_buckets_ * (uint64_t)(BD_MEAN + BD_MEAN / 8))) {
+                   (uint64_t)last_counters_.n_keys > dict_.n_buckets() * (uint64_t)(BD_MEAN + BD_MEAN / 8))) {
       dict_full_seen_ = last_counters_.dict_full;
       grow_ids();
       last_counters_.n_keys = total_keys_host_;
@@ -2128,7 +2038,7 @@ WindowAggOp::OutSet* WindowAggOp::out_set(size_t i, uint64_t cap) {
   while (out_sets_.size() <= i) out_sets_.emplace_back(new OutSet());
   OutSet* os = out_sets_[i].get();
   if (os->cap < cap) {
-    uint64_t c = std::max<uint64_t>(std::max<uint64_t>(cap, id_cap_), 1024);
+    uint64_t c = std::max<uint64_t>(std::max<uint64_t>(cap, dict_.id_cap()), 1024);
     os->key.alloc(c * 8);
     os->wstart.alloc(c * 8);
     os->wend.alloc(c * 8);
@@ -2144,7 +2054,7 @@ WindowAggOp::OutSet* WindowAggOp::out_set(size_t i, uint64_t cap) {
 int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& blocks, int n_add, bool use_running,
                               bool partial, int64_t wstart, int64_t wend, int64_t ts, OutSet* os) {
   AB_REQUIRE(blocks.size() <= (size_t)INT_MAX, ARROYO_B200_RUNTIME, "too many panes in one window");
-  const uint32_t n_ids = n_keys_host_;
+  const uint32_t n_ids = dict_.n_ids();
   EmitParams p{};
   p.panes_inline = blocks.size() <= (size_t)EMIT_INLINE ? 1 : 0;
   if (p.panes_inline) {
@@ -2161,7 +2071,7 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
   p.panes = d_emit_panes_.as<const unsigned long long*>();
   p.n_panes = (int)blocks.size();
   p.n_acc = plan_.n_acc;
-  p.id_cap = id_cap_;
+  p.id_cap = dict_.id_cap();
   p.n_ids = n_ids;
   p.keyed = plan_.keyed ? 1 : 0;
   for (int a = 0; a < plan_.n_acc; ++a) p.acc_kind[a] = plan_.acc_kind[a];
@@ -2180,7 +2090,7 @@ int64_t WindowAggOp::run_emit(const std::vector<const unsigned long long*>& bloc
       else slot = col;
     }
   }
-  p.id_keys = id_keys_.as<long long>();
+  p.id_keys = dict_.id_keys();
   p.out_key = os->key.as<long long>();
   const bool proj = cfg.final_projection != 0 && !partial;
   p.out_wstart = proj ? os->wstart.as<long long>() : nullptr;
@@ -2382,7 +2292,7 @@ void WindowAggOp::emit_window(int64_t a, int64_t b, size_t out_index, BatchesPri
   }
   // device output and asynchronous host output keep every window of the emission alive until the caller (or the
   // copy stream) is done with it: one output set per window; blocking host output reuses set 0
-  OutSet* os = out_set(out_dev || async_out_ ? out_index : 0, std::max<uint64_t>(n_keys_host_, 1));
+  OutSet* os = out_set(out_dev || async_out_ ? out_index : 0, std::max<uint64_t>(dict_.n_ids(), 1));
   const int64_t ts = cfg.final_projection ? b - 1 : a;
   int64_t n = run_emit(blocks, n_add, use_running, false, a, b, ts, os);
   // blocks of panes that had already left the store have now been subtracted from W
@@ -2583,7 +2493,7 @@ void WindowAggOp::handle_checkpoint(int64_t wm, BatchesPriv* out) {
     auto it = panes_.find(s.a);
     AB_REQUIRE(it != panes_.end(), ARROYO_B200_RUNTIME, "checkpointing a pane that is not resident");
     Pane& p = it->second;
-    OutSet* os = out_set(0, std::max<uint64_t>(n_keys_host_, 1));
+    OutSet* os = out_set(0, std::max<uint64_t>(dict_.n_ids(), 1));
     // the rows received since the last drain = the active block (the reference drains the running
     // Partial exec and writes its output, sliding :705-733)
     int64_t n = run_emit({p.dev}, 1, false, true, 0, 0, s.a, os);
@@ -2594,11 +2504,11 @@ void WindowAggOp::handle_checkpoint(int64_t wm, BatchesPriv* out) {
     FoldParams fp{};
     fp.active = p.dev;
     fp.frozen = p.frozen;
-    fp.id_cap = id_cap_;
-    fp.n_ids = n_keys_host_;
+    fp.id_cap = dict_.id_cap();
+    fp.n_ids = dict_.n_ids();
     fp.n_acc = plan_.n_acc;
     for (int a = 0; a < plan_.n_acc; ++a) fp.acc_kind[a] = plan_.acc_kind[a];
-    int grid = (int)std::min<uint32_t>((n_keys_host_ + 255) / 256, (uint32_t)num_sms_ * 8);
+    int grid = (int)std::min<uint32_t>((dict_.n_ids() + 255) / 256, (uint32_t)num_sms_ * 8);
     fold_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(fp);
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
@@ -2613,7 +2523,7 @@ void WindowAggOp::handle_checkpoint(int64_t wm, BatchesPriv* out) {
     // checkpoint (or the restore) already wrote it
     std::vector<const unsigned long long*> blocks{p.dev};
     if (p.frozen && !p.delta_exported) blocks.push_back(p.frozen);
-    OutSet* os = out_set(0, std::max<uint64_t>(n_keys_host_, 1));
+    OutSet* os = out_set(0, std::max<uint64_t>(dict_.n_ids(), 1));
     int64_t n = run_emit(blocks, (int)blocks.size(), false, true, 0, 0, kv.first, os);
     if (n > 0) export_partial(os, n, out);
     p.exported = true;
@@ -2657,7 +2567,6 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
     // upload columns
     PartialParams pp{};
     pp.n = rows;
-    pp.keyed = plan_.keyed ? 1 : 0;
     pp.n_acc = plan_.n_acc;
     for (int a = 0; a < plan_.n_acc; ++a) pp.acc_kind[a] = plan_.acc_kind[a];
     auto up = [&](const uint64_t* h) -> const unsigned long long* {
@@ -2666,7 +2575,7 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
       return keep.back().as<unsigned long long>();
     };
     int ci = 0;
-    if (plan_.keyed) pp.key = (const long long*)up(cols[ci++].data);
+    const long long* keys = plan_.keyed ? (const long long*)up(cols[ci++].data) : nullptr;
     for (int a = 0; a < MAX_ACC; ++a) pp.state[a] = nullptr;
     std::vector<std::pair<int, int>> avg_sum_cols;  // (agg, column of its f64 sum)
     for (int g = 0; g < plan_.n_aggs; ++g) {
@@ -2714,14 +2623,16 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
       pp.state[0] = keep.back().as<unsigned long long>();
     }
     // room for every key of the batch at the target bucket fill (most of them are usually known already)
-    while (plan_.keyed && (uint64_t)total_keys_host_ + (uint64_t)rows > n_buckets_ * (uint64_t)BD_MEAN) {
+    while (plan_.keyed && (uint64_t)total_keys_host_ + (uint64_t)rows > dict_.n_buckets() * (uint64_t)BD_MEAN) {
       AB_CUDA(cudaStreamSynchronize(stream_));
       grow_ids();
     }
-    pp.dict = dict_view();
+    // every key gets its id before anything is merged (a bucket out of ids grows the dictionary), then merge by id
+    uint32_t* ids = keep.emplace_back((size_t)rows * sizeof(uint32_t)).as<uint32_t>();
+    dict_.place(keys, rows, ids, [&] { grow_ids(); });
+    pp.ids = ids;
     pp.pane = panes_.at(bin).frozen;
-    pp.id_cap = id_cap_;
-    pp.counters = d_counters();
+    pp.id_cap = dict_.id_cap();
     int grid = (int)std::min<int64_t>((rows + 255) / 256, (int64_t)num_sms_ * 8);
     ingest_partial_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(pp);
     AB_CUDA(cudaGetLastError());
@@ -2729,7 +2640,6 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
     Counters c{};
     AB_CUDA(cudaMemcpyAsync(&c, book_.p, sizeof c, cudaMemcpyDeviceToHost, stream_));
     AB_CUDA(cudaStreamSynchronize(stream_));
-    AB_REQUIRE(c.lost == 0, ARROYO_B200_RUNTIME, "dictionary overflow during restore");
     total_keys_host_ = c.n_keys;
     last_counters_ = c;
     max_bin_seen_ = std::max<int64_t>(max_bin_seen_, bin);

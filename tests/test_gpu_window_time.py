@@ -323,7 +323,8 @@ def device_rows(wins, names):
 
 
 def run_gpu(st, kind, cfg, entry, expected_keys=0):
-    """The CUDA operator on the same events.  Returns (one list of output rows per watermark, rows_in, rows_late).
+    """The CUDA operator on the same events.  Returns (one list of output rows per watermark, rows_in, rows_late,
+    n_keys of the last operator).
     `poll_host` feeds device batches and alternates the watermarks between the host call (even ones) and the device
     begin / poll pair (odd ones), so host emissions and checkpoints follow device emissions of any size."""
     import torch
@@ -408,7 +409,7 @@ def run_gpu(st, kind, cfg, entry, expected_keys=0):
     totals[0] += s["rows_in"]
     totals[1] += s["rows_late"]
     op.close()
-    return outs, totals[0], totals[1]
+    return outs, totals[0], totals[1], s["n_keys"]
 
 
 def check_emissions(want, got, cfg, who):
@@ -505,7 +506,7 @@ def test_window_event_time(shape, kind, keys, plan, entry):
     cfg = config(st, kind, plan)
     want, late = reference(st, cfg)
     # small dictionaries keep thousands of live pane blocks cheap
-    got, rows_in, rows_late = run_gpu(st, kind, cfg, entry, expected_keys=0 if keys == "many" else 64)
+    got, rows_in, rows_late, _ = run_gpu(st, kind, cfg, entry, expected_keys=0 if keys == "many" else 64)
     check_emissions(want, got, cfg, "gpu")
     assert rows_in == sum(ev[1].num_rows for ev in st.events if ev[0] == "batch")
     assert rows_late == late

@@ -141,7 +141,7 @@ def main():
             t0 = time.perf_counter()
             op.on_start(rctx)
             restore_call = (time.perf_counter() - t0) * 1000
-        restore_kernels = {k: sum(kernel_ms(prof, k)) for k in ("upd_restore_insert_kernel", "upd_restore_gen_kernel",
+        restore_kernels = {k: sum(kernel_ms(prof, k)) for k in ("bd_place_kernel", "upd_restore_gen_kernel",
                                                                  "upd_restore_pos_kernel", "upd_restore_seed_kernel")}
         assert op.stats()["n_keys"] == n
         op.close()
