@@ -17,7 +17,12 @@ class WindowAggConfig:
     Input  [key cols..., value cols..., _timestamp]; output = aggregate output [keys, aggs] with the
     window struct {start, end} inserted at `window_index`, then `_timestamp = bin + width - 1 ns`
     (arroyo-planner/src/extension/aggregate.rs:292-390).  `final_projection=False` (tumbling only)
-    gives [keys, aggs, _timestamp = bin]."""
+    gives [keys, aggs, _timestamp = bin].
+
+    `width=0` is the instant window (InstantAggregatingWindowFunc): each `_timestamp` is its own bin.  Its
+    `final_projection=False` form is [keys, aggs, _timestamp = instant]; with `final_projection=True` it is the nested
+    form behind an upstream window of width `nested_width`: window{start = ts - nested_width + 1, end = ts + 1} at
+    `window_index`, `_timestamp = instant` (extension/aggregate.rs:392-452)."""
     width: int
     slide: int = 0
     key_names: List[str] = field(default_factory=list)
@@ -27,6 +32,8 @@ class WindowAggConfig:
     # final stage of a partial -> shuffle -> final plan: name of the input column that carries how many
     # original rows each (partial-aggregate) input row stands for; None = inputs are raw rows
     partial_count_col: Optional[str] = None
+    # instant window, nested form: the upstream window's width
+    nested_width: int = 0
 
 
 @dataclass

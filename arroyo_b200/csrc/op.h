@@ -98,5 +98,6 @@ OpBase* make_instant_join_op(const ArroyoB200OpConfig& cfg);
 OpBase* make_session_op(const ArroyoB200OpConfig& cfg);
 OpBase* make_updating_agg_op(const ArroyoB200OpConfig& cfg);
 OpBase* make_ttl_join_op(const ArroyoB200OpConfig& cfg);
+OpBase* make_instant_agg_op(const ArroyoB200OpConfig& cfg);
 
 }  // namespace ab

@@ -13,6 +13,7 @@ MAX_COLS = 16
 
 OK, INVALID_ARGUMENT, UNSUPPORTED, RUNTIME, FATAL, PANIC = 0, 1, 2, 3, 4, 5
 TUMBLING_AGGREGATE, SLIDING_AGGREGATE, SESSION_AGGREGATE, INSTANT_JOIN, UPDATING_AGGREGATE, TTL_JOIN = 1, 2, 3, 4, 5, 6
+INSTANT_AGGREGATE = 7
 AGG_COUNT_STAR, AGG_SUM_I64, AGG_AVG_I64, AGG_MIN_I64, AGG_MAX_I64 = 1, 2, 3, 4, 5
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_FULL = 0, 1, 2, 3
 FLAG_PROFILE, FLAG_REMERGE_ONLY, FLAG_COMBINE, FLAG_AVG_F64, FLAG_NO_COMBINE, FLAG_ZERO_COPY = 1, 2, 4, 8, 16, 32

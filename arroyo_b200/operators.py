@@ -228,7 +228,7 @@ class _WindowAggregate(_NativeOperator):
         if len(c.aggs) > ffi.MAX_AGGS:
             raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, "too many aggregates")
         cfg = _agg_config(self.kind, c, names)
-        cfg.width_ns = int(c.width)
+        cfg.width_ns = self._width_ns()
         cfg.slide_ns = int(getattr(c, "slide", 0) or 0)
         pc = getattr(c, "partial_count_col", None)
         cfg.partial_count_col_plus1 = names.index(pc) + 1 if pc else 0
@@ -236,6 +236,9 @@ class _WindowAggregate(_NativeOperator):
         cfg.window_index = int(c.window_index)
         self._create(cfg)
         self._names = list(names)
+
+    def _width_ns(self) -> int:
+        return int(self.config.width)
 
     def output_names(self) -> List[str]:
         c = self.config
@@ -384,6 +387,24 @@ class SlidingAggregatingWindowFunc(_WindowAggregate):
 
     def name(self):
         return "sliding_window"
+
+
+class InstantAggregatingWindowFunc(_WindowAggregate):
+    """tumbling_aggregating_window.rs with width 0: the instant window the planner puts behind an upstream window
+    (arroyo-planner extension/aggregate.rs:233-289).  Each `_timestamp` is one bin; at watermark w every instant < w
+    leaves in ascending order.  `config.width` is 0.  `final_projection=False` gives [keys, aggs, _timestamp];
+    `final_projection=True` is the nested form: window{start = ts - nested_width + 1, end = ts + 1} at `window_index`,
+    `_timestamp = instant`.  Table "t" (retention 0) holds per instant the partial rows since the previous checkpoint."""
+    kind = ffi.INSTANT_AGGREGATE
+
+    def name(self):
+        return "instant_window"
+
+    def _width_ns(self) -> int:
+        c = self.config
+        if int(c.width) != 0:
+            raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "the instant window has width 0")
+        return int(getattr(c, "nested_width", 0)) if c.final_projection else 0
 
 
 

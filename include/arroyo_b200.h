@@ -94,9 +94,17 @@ typedef enum ArroyoB200OpKind {
                                        * arroyo-worker/src/arrow/incremental_aggregator.rs (append-only inputs;
                                        * COUNT(*) / SUM / AVG / MIN / MAX over Int64; emits on ticks, checkpoints and
                                        * end of data: rows [key?, aggregates..., _timestamp, is_retract bool])      */
-  ARROYO_B200_TTL_JOIN = 6            /* OperatorName::Join: JoinWithExpiration, arroyo-worker/src/arrow/
+  ARROYO_B200_TTL_JOIN = 6,           /* OperatorName::Join: JoinWithExpiration, arroyo-worker/src/arrow/
                                        * join_with_expiration.rs (inner joins of append-only inputs; same column fields as
                                        * INSTANT_JOIN; matches leave from arroyo_b200_op_process_batch_emit)            */
+  ARROYO_B200_INSTANT_AGGREGATE = 7   /* OperatorName::TumblingWindowAggregate with width_micros == 0: the instant window
+                                       * the planner puts after an upstream window (extension/aggregate.rs:233-289).  The
+                                       * bin is _timestamp itself; at watermark w every instant < w leaves in ascending
+                                       * order.  Output [key?, aggregates..., _timestamp = instant], or with
+                                       * final_projection the window{start = ts - (width_ns - 1), end = ts + 1} struct
+                                       * inserted at window_index.  Checkpoints write table "t" (partial_schema, one
+                                       * batch per instant, the rows since the previous checkpoint).  Host output only:
+                                       * handle_watermark_device* => ARROYO_B200_UNSUPPORTED                           */
 } ArroyoB200OpKind;
 
 typedef enum ArroyoB200AggKind {
@@ -140,7 +148,10 @@ typedef struct ArroyoB200OpConfig {
   uint32_t task_index;   /* TaskInfo.task_index  (arroyo-types/src/lib.rs TaskInfo)     */
   uint32_t parallelism;  /* TaskInfo.parallelism                                        */
 
-  int64_t width_ns;      /* width_micros * 1000; 0 is not supported (instant window)    */
+  int64_t width_ns;      /* width_micros * 1000; 0 (the instant window) is refused here:*/
+                         /* that plan is INSTANT_AGGREGATE                              */
+                         /* INSTANT_AGGREGATE: read only when final_projection = 1, as  */
+                         /* the upstream window's width W (> 0) of the window struct    */
   int64_t slide_ns;      /* slide_micros * 1000 (sliding only)                          */
   int64_t gap_ns;        /* gap_micros * 1000 (session only)                            */
 
