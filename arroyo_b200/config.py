@@ -47,9 +47,12 @@ class SessionConfig:
 
 @dataclass
 class JoinConfig:
-    """JoinOperator for the instant (windowed) join (arroyo-worker/src/arrow/instant_join.rs)."""
+    """JoinOperator for the instant (windowed) join (arroyo-worker/src/arrow/instant_join.rs) and the join with
+    expiration (join_with_expiration.rs).  `ttl` (ns) is the join with expiration's state retention, 0 meaning 24 h
+    (:239-248); the instant join ignores it."""
     left_on: List[str]
     right_on: List[str]
     join_type: str = "inner"
     left_routing_keys: List[str] = field(default_factory=list)
     right_routing_keys: List[str] = field(default_factory=list)
+    ttl: int = 0

@@ -367,6 +367,11 @@ int32_t arroyo_b200_op_checkpoint_state(ArroyoB200Op* op, ArroyoB200Batches* sta
   return emit_batches(op, state_out, [&](OpBase* o, BatchesPriv* b) { o->checkpoint_state(b); });
 }
 
+int32_t arroyo_b200_op_restore_side(ArroyoB200Op* op, uint32_t side, struct ArrowArray* batches,
+                                    struct ArrowSchema* schemas, int64_t n) {
+  return guarded(op, [&](OpBase* o) { o->restore_side(side, batches, schemas, n); });
+}
+
 int32_t arroyo_b200_op_on_close(ArroyoB200Op* op, int32_t end_of_data, ArroyoB200Batches* out) {
   return emit_batches(op, out, [&](OpBase* o, BatchesPriv* b) { o->on_close(end_of_data, b); }, nullptr, true);
 }

@@ -37,6 +37,10 @@ class OpBase {
   virtual void handle_tick(BatchesPriv* /*out*/) {}
   // the key-value state table the updating aggregate writes at a checkpoint; every other operator has none
   virtual void checkpoint_state(BatchesPriv* /*out*/) {}
+  // stores rows of a join side's key-time table without probing (the TTL join); every other operator has none
+  virtual void restore_side(uint32_t /*side*/, ArrowArray* /*batches*/, ArrowSchema* /*schemas*/, int64_t /*n*/) {
+    throw Error(ARROYO_B200_UNSUPPORTED, name + ": restore_side is only for the join with expiration");
+  }
   virtual void flush() = 0;
   // enqueue whatever input is still being batched on the host side; does not wait
   virtual void submit() {}

@@ -16,6 +16,11 @@
 //             (arroyo-planner/src/plan/join.rs:165-185), which leave with the call (`process_batch_emit`).
 // Rows leave the tables only through the state backend's retention (`ttl`, applied at restore / compaction), never
 // inside a run: like the oracle, not restated.  Outer / updating joins are refused (ARROYO_B200_UNSUPPORTED).
+//
+// Restore (`restore_side`): the shim writes the key-time tables "left" / "right" from the host batches and hands
+// what it reads back to the side they came from.  Those rows are appended and linked, the first step of a batch,
+// and never probed: the reference's `insert_internal` (expiring_time_key_map.rs:1008-1049) stores restored rows
+// without joining them, so no pair among them leaves again.
 #include <algorithm>
 #include <climits>
 
@@ -139,8 +144,10 @@ class TtlJoinOp final : public OpBase {
   explicit TtlJoinOp(const ArroyoB200OpConfig& c);
   ~TtlJoinOp() override;
   void on_start(ArrowArray*, ArrowSchema*, int64_t n, int64_t, int64_t) override {
-    AB_REQUIRE(n == 0, ARROYO_B200_UNSUPPORTED, "JoinWithExpiration restore: replay the key-time tables through process_batch");
+    AB_REQUIRE(n == 0, ARROYO_B200_UNSUPPORTED,
+               "JoinWithExpiration restore: hand each key-time table to arroyo_b200_op_restore_side");
   }
+  void restore_side(uint32_t side, ArrowArray* batches, ArrowSchema* schemas, int64_t n) override;
   void process_batch(uint32_t index, uint32_t parts, ArrowArray* batch, const ArrowSchema* schema) override {
     BatchesPriv sink;
     process_batch_emit(index, parts, batch, schema, &sink);
@@ -167,6 +174,7 @@ class TtlJoinOp final : public OpBase {
   DevBuf cnt_, off_, total_, sums_, pair_new_, pair_old_, out_ts_;
   std::vector<DevBuf> out_cols_;
   int64_t scratch_cap_ = 0, pair_cap_ = 0;
+  bool took_input_ = false;  // process_batch has accepted a batch: restore_side is refused from then on
   ArroyoB200Stats st_{};
 
   int grid_for(int64_t n) const { return (int)std::max<int64_t>(1, std::min<int64_t>((n + TJ - 1) / TJ, (int64_t)num_sms_ * 8)); }
@@ -222,6 +230,57 @@ void TtlJoinOp::ensure_table(TSide& s, uint64_t more_rows) {
   s.tab_cap = (uint32_t)nc;
 }
 
+// KeyTimeView::insert_internal (:1008-1049) for the batches of one side's table: every batch is checked before anything
+// changes, then the call's rows are copied into consecutive arena ranges and linked by one launch.  A restore that
+// succeeds takes every batch.
+void TtlJoinOp::restore_side(uint32_t side, ArrowArray* batches, ArrowSchema* schemas, int64_t n) {
+  AB_REQUIRE(side <= 1, ARROYO_B200_INVALID_ARGUMENT, "restore_side: side must be 0 (left) or 1 (right)");
+  AB_REQUIRE(n >= 0 && (n == 0 || (batches != nullptr && schemas != nullptr)), ARROYO_B200_INVALID_ARGUMENT,
+             "restore_side: null batches");
+  AB_REQUIRE(!took_input_, ARROYO_B200_INVALID_ARGUMENT,
+             "JoinWithExpiration: restore_side after process_batch (restore before the first batch)");
+  TSide& s = side_[side];
+  std::vector<std::vector<InColumn>> cols((size_t)n);
+  std::vector<int64_t> rows((size_t)n, 0);
+  std::string key_format = s.key_format;
+  int64_t total = 0;
+  for (int64_t b = 0; b < n; ++b) {
+    cols[b] = import_batch(&batches[b], &schemas[b], &rows[b]);
+    AB_REQUIRE((int)cols[b].size() == s.n_cols, ARROYO_B200_INVALID_ARGUMENT,
+               "restore_side: batch does not have the side's number of columns");
+    require_join_key_type(cols[b][s.key_col].format, key_format, side_[1 - side].key_format);
+    key_format = cols[b][s.key_col].format;
+    total += rows[b];
+  }
+  set_device();
+  if (total > 0) {
+    reserve(s, total);
+    ensure_table(s, (uint64_t)total);
+    long long at = s.n;
+    for (int64_t b = 0; b < n; ++b) {
+      for (int c = s.n_routing; c < s.n_cols; ++c)
+        if (rows[b])
+          AB_CUDA(cudaMemcpyAsync(s.cols[c].as<long long>() + at, cols[b][c].data, (size_t)rows[b] * 8,
+                                  cudaMemcpyHostToDevice, stream_));
+      at += rows[b];
+    }
+    st_.h2d_bytes += (uint64_t)total * 8 * (uint64_t)(s.n_cols - s.n_routing);
+    tj_link_kernel<<<grid_for(total), TJ, 0, stream_>>>(s.cols[s.key_col].as<long long>(), s.n, total, s.tab.as<MSlot>(),
+                                                      s.tab_cap - 1, s.next.as<int>());
+    AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    s.n += total;
+    s.keys_bound += (uint64_t)total;
+  }
+  if (n > 0) {
+    for (int c = 0; c < s.n_cols; ++c) s.formats[c] = cols[n - 1][c].format;
+    s.key_format = key_format;
+  }
+  for (int64_t b = 0; b < n; ++b)
+    if (batches[b].release) batches[b].release(&batches[b]);
+}
+
 void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* batch, const ArrowSchema* schema, BatchesPriv* out) {
   set_device();
   AB_REQUIRE(parts >= 2 && parts % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
@@ -235,6 +294,7 @@ void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* b
   require_join_key_type(cols[s.key_col].format, s.key_format, o.key_format);
   for (int c = 0; c < s.n_cols; ++c) s.formats[c] = cols[c].format;
   s.key_format = cols[s.key_col].format;
+  took_input_ = true;
   st_.rows_in += (uint64_t)n;
   if (n == 0) {
     if (batch->release) batch->release(batch);

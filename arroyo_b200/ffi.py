@@ -126,6 +126,8 @@ SYMBOLS = [
     ("arroyo_b200_op_handle_tick", C.c_int32, [_VP, C.POINTER(Batches)]),
     ("arroyo_b200_op_process_batch_emit", C.c_int32, [_VP, C.c_uint32, C.c_uint32, C.POINTER(ArrowArray), C.POINTER(ArrowSchema),
                                                       C.POINTER(Batches)]),
+    ("arroyo_b200_op_restore_side", C.c_int32, [_VP, C.c_uint32, C.POINTER(ArrowArray), C.POINTER(ArrowSchema),
+                                                C.c_int64]),
     ("arroyo_b200_op_flush", C.c_int32, [_VP]),
     ("arroyo_b200_op_submit", C.c_int32, [_VP]),
     ("arroyo_b200_release_batches", None, [C.POINTER(Batches)]),

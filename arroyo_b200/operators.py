@@ -175,20 +175,25 @@ class _NativeOperator:
             _release(sch)
         _check(self._lib, self._h, st)
 
-    def _on_start(self, batches: List[pa.RecordBatch], wm: int, t: int):
-        """arroyo_b200_op_on_start with `batches` as the state, the restored watermark `wm` and the table time `t`
-        (ffi.INT64_MIN: none).  The library takes the batches it consumed; the rest are released here."""
+    def _hand_over_state(self, call, batches: List[pa.RecordBatch]):
+        """Exports `batches` as C arrays and calls `call(arrays, schemas, n)` (on_start, restore_side).  The library
+        takes the batches it consumed; the rest are released here."""
         n = len(batches)
         arrs = (ffi.ArrowArray * max(n, 1))()
         schs = (ffi.ArrowSchema * max(n, 1))()
         for i, b in enumerate(batches):
             b._export_to_c(C.addressof(arrs[i]), C.addressof(schs[i]))
         try:
-            st = self._lib.arroyo_b200_op_on_start(self._h, arrs, schs, n, wm, t)
+            st = call(arrs, schs, n)
         finally:
             for s in list(arrs) + list(schs):
                 _release(s)
         _check(self._lib, self._h, st)
+
+    def _on_start(self, batches: List[pa.RecordBatch], wm: int, t: int):
+        """arroyo_b200_op_on_start with `batches` as the state, the restored watermark `wm` and the table time `t`
+        (ffi.INT64_MIN: none)."""
+        self._hand_over_state(lambda a, s, n: self._lib.arroyo_b200_op_on_start(self._h, a, s, n, wm, t), batches)
 
     def _collect(self, out: ffi.Batches, collector: Optional[Collector]):
         """Imports the batches of `out` under `output_names()` into `collector` (None: they are dropped)."""
@@ -763,22 +768,78 @@ class InstantJoin(_NativeOperator):
         return wm
 
 
+DAY_NS = 24 * 3600 * 10 ** 9
+
+
 class JoinWithExpiration(InstantJoin):
     """arroyo-worker/src/arrow/join_with_expiration.rs: the non-windowed join (inner, append-only inputs).  Every
-    matching pair leaves once, from the `process_batch_index` call that brings its later row (:42-108)."""
+    matching pair leaves once, from the `process_batch_index` call that brings its later row (:42-108).
+
+    State: every non-empty input batch goes into its side's key-time table, "left" or "right", under its newest
+    `_timestamp` (KeyTimeView::insert, arroyo-state/src/tables/expiring_time_key_map.rs:997-1006), and a checkpoint
+    flushes both tables at the watermark.  After `on_start` the first batch loads both tables from watermark - ttl on
+    (get_key_time_view :200-236) and hands them to arroyo_b200_op_restore_side: the restored rows join their side's
+    stored rows and are never paired with each other (insert_internal :1008-1049)."""
     kind = ffi.TTL_JOIN
+
+    def __init__(self, config, left_schema: Optional[pa.Schema] = None, right_schema: Optional[pa.Schema] = None, **kw):
+        self._restore_pending = False
+        self._restored = [[], []]  # per side: table batches that wait for the operator to be built
+        super().__init__(config, left_schema, right_schema, **kw)
 
     def name(self):
         return "JoinWithExpiration"
 
+    def ttl(self) -> int:
+        """The tables' retention in ns: `config.ttl`, where 0 means 24 h (join_with_expiration.rs:239-248)."""
+        return int(getattr(self.config, "ttl", 0) or 0) or DAY_NS
+
     def tables(self):
-        return {"left": 0, "right": 0}  # key-time tables with retention = ttl (:228-262); restore is a replay
+        return {"left": self.ttl(), "right": self.ttl()}  # key-time tables (:228-262)
+
+    def _table(self, ctx: OperatorContext, side: int):
+        return ctx.table("left" if side == 0 else "right", self.ttl())
 
     def on_start(self, ctx: OperatorContext):
-        raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, "JoinWithExpiration restore: replay the key-time tables through process_batch_index")
+        """Nothing is read yet: like the reference, the first batch after the restart loads both tables, with the
+        watermark of that moment (process_left / process_right -> get_key_time_table)."""
+        self._restore_pending = True
+
+    def _restore(self, ctx: OperatorContext):
+        wm = ctx.last_present_watermark()
+        for side in (0, 1):
+            batches = [b for _, b in self._table(ctx, side).all_batches_for_watermark(wm)]
+            if not batches:
+                continue
+            if self._schemas[side] is None:
+                self._schemas[side] = batches[0].schema
+            if self.created:
+                self._restore_side(side, batches)
+            else:
+                self._restored[side] += batches
+        if not self.created and self._schemas[0] is not None and self._schemas[1] is not None:
+            self._build()
+
+    def _restore_side(self, side: int, batches: List[pa.RecordBatch]):
+        if batches:
+            self._hand_over_state(
+                lambda a, s, n: self._lib.arroyo_b200_op_restore_side(self._h, side, a, s, n), batches)
+
+    def _build(self):
+        """Creates the operator, then restores the table batches that waited for it, then sends the buffered input."""
+        buffered, self._buffered = self._buffered, []
+        super()._build()
+        restored, self._restored = self._restored, [[], []]
+        for side in (0, 1):
+            self._restore_side(side, restored[side])
+        for index, parts, batch in buffered:
+            self._send(index, parts, batch)
 
     def handle_checkpoint(self, barrier, ctx: OperatorContext, collector: Collector):
-        return
+        """The tables keep what is at or after watermark - ttl (the checkpointer, expiring_time_key_map.rs:747-760)."""
+        wm = ctx.last_present_watermark()
+        for side in (0, 1):
+            self._table(ctx, side).flush(wm)
 
     def _send(self, index, parts, batch, collector=None):
         out = ffi.Batches()
@@ -788,18 +849,21 @@ class JoinWithExpiration(InstantJoin):
     def process_batch_index(self, index: int, in_partitions: int, batch: pa.RecordBatch, ctx: OperatorContext,
                             collector: Collector):
         side = index // (in_partitions // 2)
+        if self._restore_pending:
+            self._restore_pending = False
+            self._restore(ctx)
         if self._schemas[side] is None:
             self._schemas[side] = batch.schema
-        if not self.created:
-            if self._schemas[0] is not None and self._schemas[1] is not None:
+        if self.created or (self._schemas[0] is not None and self._schemas[1] is not None):
+            if not self.created:
                 self._build()
-                pending, self._buffered = self._buffered, []
-                for i, parts, b in pending:
-                    self._send(i, parts, b, collector)
-            else:
-                self._buffered.append((index, in_partitions, batch))
-                return
-        self._send(index, in_partitions, batch, collector)
+            self._send(index, in_partitions, batch, collector)
+        else:
+            self._buffered.append((index, in_partitions, batch))
+        if batch.num_rows:  # the table takes the batches the operator took (KeyTimeView::insert)
+            import pyarrow.compute as pc
+            ts = batch.column(batch.schema.names.index(TIMESTAMP)).cast(pa.int64())
+            self._table(ctx, side).insert(int(pc.max(ts).as_py()), batch)
 
     def handle_watermark(self, watermark, ctx: OperatorContext, collector: Collector):
         return watermark

@@ -96,7 +96,9 @@ typedef enum ArroyoB200OpKind {
                                        * end of data: rows [key?, aggregates..., _timestamp, is_retract bool])      */
   ARROYO_B200_TTL_JOIN = 6,           /* OperatorName::Join: JoinWithExpiration, arroyo-worker/src/arrow/
                                        * join_with_expiration.rs (inner joins of append-only inputs; same column fields as
-                                       * INSTANT_JOIN; matches leave from arroyo_b200_op_process_batch_emit)            */
+                                       * INSTANT_JOIN; matches leave from arroyo_b200_op_process_batch_emit).  The shim
+                                       * writes the key-time tables "left" / "right" from the input batches; a restart
+                                       * hands them back through arroyo_b200_op_restore_side                           */
   ARROYO_B200_INSTANT_AGGREGATE = 7   /* OperatorName::TumblingWindowAggregate with width_micros == 0: the instant window
                                        * the planner puts after an upstream window (extension/aggregate.rs:233-289).  The
                                        * bin is _timestamp itself; at watermark w every instant < w leaves in ascending
@@ -295,9 +297,31 @@ const char* arroyo_b200_op_name(const ArroyoB200Op* op);
  * grows when a bucket runs out of ids; keys that still cannot be placed => ARROYO_B200_RUNTIME.
  * ARROYO_B200_INVALID_ARGUMENT, with nothing changed: a column count or type that is not the plan's
  * layout, or an operator that has already taken rows or been restored.  Restored rows do not count in
- * `rows_in`; their keys count in `n_keys`. */
+ * `rows_in`; their keys count in `n_keys`.
+ * TTL join: `n > 0` => ARROYO_B200_UNSUPPORTED; its tables go through arroyo_b200_op_restore_side. */
 int32_t arroyo_b200_op_on_start(ArroyoB200Op* op, struct ArrowArray* state, struct ArrowSchema* schemas,
                                 int64_t n, int64_t watermark_ns, int64_t table_min_time_ns);
+
+/* The TTL join's restore: KeyTimeView::insert_internal (arroyo-state/src/tables/expiring_time_key_map.rs:1008-1049)
+ * for the batches the shim read from table "left" (`side` 0) or "right" (`side` 1).  The reference loads both tables
+ * at the first batch after a restart (get_key_time_view :200-236): batches whose newest `_timestamp` is below
+ * last_present_watermark - ttl (UNIX_EPOCH without a watermark) are dropped by the shim, the rest are handed here.
+ * The rows of the `n` batches, in the side's input layout (the layout process_batch takes), join that side's stored
+ * rows.  Nothing is emitted, and pairs among restored rows never are; a later batch of the other side matches restored
+ * rows exactly like rows it had received itself.
+ *  - When: any number of calls, for either side, in any order, but only before the first batch process_batch /
+ *    process_batch_emit accepts.  After that => ARROYO_B200_INVALID_ARGUMENT, nothing changed.
+ *  - All `n` batches are checked before anything changes: the side's column count (INVALID_ARGUMENT), the key type
+ *    rule of process_batch, counting earlier restored batches and the other side's key (UNSUPPORTED), no nulls
+ *    (UNSUPPORTED).  On failure no row of the call is kept.  A restored key type binds later batches, as a first batch
+ *    does.  Zero-row batches are accepted.  A side that would pass 2^31 rows => ARROYO_B200_RUNTIME, nothing changed.
+ *  - Ownership as for on_start: the library takes the arrays on success, the caller keeps them on error, and the
+ *    caller always keeps the schemas.
+ *  - Restored rows count in no statistic but `h2d_bytes` and `kernel_launches`.
+ * Every other operator kind => ARROYO_B200_UNSUPPORTED.  Device-resident input to the TTL join stays unsupported, so
+ * a shim writes the tables only from host batches. */
+int32_t arroyo_b200_op_restore_side(ArroyoB200Op* op, uint32_t side, struct ArrowArray* batches,
+                                    struct ArrowSchema* schemas, int64_t n);
 
 /* ArrowOperator::process_batch_index(index, in_partitions, batch, ctx, collector)
  * (operator.rs:1174-1188).  On success the library owns `batch` and calls its `release`
