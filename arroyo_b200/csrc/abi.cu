@@ -372,6 +372,10 @@ int32_t arroyo_b200_op_restore_side(ArroyoB200Op* op, uint32_t side, struct Arro
   return guarded(op, [&](OpBase* o) { o->restore_side(side, batches, schemas, n); });
 }
 
+int32_t arroyo_b200_op_set_clock(ArroyoB200Op* op, int64_t now_ns) {
+  return guarded(op, [&](OpBase* o) { o->set_clock(now_ns); });
+}
+
 int32_t arroyo_b200_op_on_close(ArroyoB200Op* op, int32_t end_of_data, ArroyoB200Batches* out) {
   return emit_batches(op, out, [&](OpBase* o, BatchesPriv* b) { o->on_close(end_of_data, b); }, nullptr, true);
 }

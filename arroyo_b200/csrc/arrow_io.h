@@ -16,6 +16,8 @@ namespace ab {
 struct InColumn {
   const uint64_t* data;  // first logical element (offsets applied)
   std::string format;
+  const uint8_t* validity = nullptr;  // import_batch's `nullable_col` only, when it has nulls: bit validity_bit + row
+  int64_t validity_bit = 0;
 };
 
 inline bool format_is_64bit(const char* f) {
@@ -26,8 +28,10 @@ inline bool format_is_64bit(const char* f) {
   return false;
 }
 
-// Validates a record batch exported as a struct array and returns its columns.
-inline std::vector<InColumn> import_batch(const ArrowArray* a, const ArrowSchema* s, int64_t* n_rows) {
+// Validates a record batch exported as a struct array and returns its columns.  Nulls are refused, except in column
+// `nullable_col`, whose validity bitmap is then handed back.
+inline std::vector<InColumn> import_batch(const ArrowArray* a, const ArrowSchema* s, int64_t* n_rows,
+                                          int64_t nullable_col = -1) {
   AB_REQUIRE(a && s, ARROYO_B200_INVALID_ARGUMENT, "null batch or schema");
   AB_REQUIRE(s->format && !strcmp(s->format, "+s"), ARROYO_B200_INVALID_ARGUMENT,
              "batch must be exported as a struct array (format +s)");
@@ -47,7 +51,13 @@ inline std::vector<InColumn> import_batch(const ArrowArray* a, const ArrowSchema
     }
     AB_REQUIRE(c->length >= a->length + a->offset, ARROYO_B200_INVALID_ARGUMENT, "child shorter than batch");
     AB_REQUIRE(c->n_buffers == 2, ARROYO_B200_INVALID_ARGUMENT, "primitive column must have 2 buffers");
-    if (c->null_count != 0 && c->buffers[0] != nullptr) {
+    InColumn ic;
+    if (i == nullable_col) {
+      if (c->null_count != 0 && c->buffers[0] != nullptr) {
+        ic.validity = (const uint8_t*)c->buffers[0];
+        ic.validity_bit = c->offset + a->offset;
+      }
+    } else if (c->null_count != 0 && c->buffers[0] != nullptr) {
       // null_count may be -1 (unknown): count the zero validity bits of the logical range.
       int64_t nulls = c->null_count;
       if (nulls < 0) {
@@ -63,7 +73,6 @@ inline std::vector<InColumn> import_batch(const ArrowArray* a, const ArrowSchema
                                                  " has nulls: NULL keys/values are outside the supported subset");
     }
     AB_REQUIRE(a->length == 0 || c->buffers[1] != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null data buffer");
-    InColumn ic;
     ic.data = (const uint64_t*)c->buffers[1] + c->offset + a->offset;
     ic.format = cs->format;
     cols.push_back(ic);

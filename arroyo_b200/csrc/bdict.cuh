@@ -16,7 +16,8 @@
 // BucketDict, at the end of this file, is the host side both operators share: it owns the device buffers, and when a
 // bucket runs out of ids or the table outgrows its mean fill it doubles n_buckets and rebuilds.  Ids change: each
 // operator moves its own per-id state with the old->new id map (the window's pane blocks, the updating aggregate's
-// accumulators).  BucketDict::place gives restored keys their ids before anything is merged.
+// accumulators).  BucketDict::place gives restored keys their ids before anything is merged; BucketDict::rebuild
+// makes a fresh, smaller table from the keys of chosen ids (the updating aggregate gives back the ids of expired keys).
 #pragma once
 
 #include <algorithm>
@@ -202,8 +203,39 @@ static __global__ void __launch_bounds__(256) bd_place_kernel(const BDict d, con
   }
 }
 
-// What BucketDict::grow hands back: map[old id] = new id (ID_UNSET: the id held no key) for the old ids [0, old_ids),
-// and the old id capacity (the stride of the caller's per-id arrays before the growth).
+// Rebuild from a subset: the keys of the ids [BD_ID_BASE, n_ids) that hold a key and have keep[id] != 0, with their
+// old ids, compacted with one atomic per warp.  Thread 0 also maps id 0 (the INT64_MIN key's) to itself.
+static __global__ void __launch_bounds__(256) bd_gather_kernel(const long long* id_keys, const unsigned char* keep,
+                                                               uint32_t n_ids, long long* keys, uint32_t* old_ids,
+                                                               unsigned int* count, uint32_t* map) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t stride = gridDim.x * blockDim.x;
+  const unsigned int lane = threadIdx.x & 31;
+  if (i == 0) map[0] = 0;
+  for (; i < n_ids; i += stride) {
+    const bool mine = i >= BD_ID_BASE && keep[i] && id_keys[i] != EMPTY_KEY;
+    const unsigned int active = __activemask();
+    const unsigned int mask = __ballot_sync(active, mine);
+    if (!mask) continue;
+    const int leader = __ffs(active) - 1;
+    unsigned int base = 0;
+    if ((int)lane == leader) base = atomicAdd(count, (unsigned int)__popc(mask));
+    base = __shfl_sync(active, base, leader);
+    if (!mine) continue;
+    const unsigned int o = base + __popc(mask & ((1u << lane) - 1u));
+    keys[o] = id_keys[i];
+    old_ids[o] = i;
+  }
+}
+static __global__ void bd_map_kernel(const uint32_t* old_ids, const uint32_t* new_ids, unsigned int n, uint32_t* map) {
+  unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned int stride = gridDim.x * blockDim.x;
+  for (; i < n; i += stride) map[old_ids[i]] = new_ids[i];
+}
+
+// What BucketDict::grow and ::rebuild hand back: map[old id] = new id (ID_UNSET: the id held no key, or a key that
+// was not kept) for the old ids [0, old_ids), and the old id capacity (the stride of the caller's per-id arrays
+// before the change).
 struct BdGrowth {
   DevBuf map;
   uint32_t old_ids;
@@ -300,6 +332,38 @@ class BucketDict {
                  "restored keys whose dictionary bucket is out of ids still do not fit after the dictionary grew");
       grow_step();
     }
+  }
+
+  // A fresh dictionary holding only the keys of the ids with keep[id] != 0 (device, one byte per id of n_ids()), with
+  // at least `min_buckets` buckets and room for the kept keys at the mean fill: what was handed out to keys that are
+  // gone is reclaimed.  The kept keys are placed like restored ones (place, doubling when a bucket runs out of ids).
+  // Id 0 maps to itself.  Returns with the stream drained.
+  BdGrowth rebuild(const unsigned char* keep, uint64_t min_buckets) {
+    AB_REQUIRE(keyed_, ARROYO_B200_RUNTIME, "rebuild of an unkeyed dictionary");
+    BdGrowth g{DevBuf((size_t)id_cap_ * sizeof(uint32_t)), n_ids(), id_cap_};
+    DevBuf keys((size_t)g.old_ids * sizeof(long long)), old_ids((size_t)g.old_ids * sizeof(uint32_t)),
+        count(sizeof(unsigned int));
+    AB_CUDA(cudaMemsetAsync(g.map.p, 0xFF, (size_t)id_cap_ * sizeof(uint32_t), stream_));  // ID_UNSET
+    AB_CUDA(cudaMemsetAsync(count.p, 0, sizeof(unsigned int), stream_));
+    bd_gather_kernel<<<grid(g.old_ids), 256, 0, stream_>>>(id_keys(), keep, g.old_ids, keys.as<long long>(),
+                                                          old_ids.as<uint32_t>(), count.as<unsigned int>(),
+                                                          g.map.as<uint32_t>());
+    AB_CUDA(cudaGetLastError());
+    ++*launches_;
+    unsigned int n = 0;
+    AB_CUDA(cudaMemcpyAsync(&n, count.p, sizeof n, cudaMemcpyDeviceToHost, stream_));
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    AB_CUDA(cudaMemsetAsync(n_total_, 0, sizeof(unsigned int), stream_));
+    alloc(std::max<uint64_t>(min_buckets, bd_buckets_for(n)));
+    DevBuf new_ids((size_t)std::max(n, 1u) * sizeof(uint32_t));
+    place(keys.as<long long>(), n, new_ids.as<uint32_t>(), [&] { grow(); });
+    if (n) {
+      bd_map_kernel<<<grid(n), 256, 0, stream_>>>(old_ids.as<uint32_t>(), new_ids.as<uint32_t>(), n, g.map.as<uint32_t>());
+      AB_CUDA(cudaGetLastError());
+      ++*launches_;
+    }
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    return g;
   }
 
  private:

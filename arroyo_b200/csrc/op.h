@@ -41,6 +41,10 @@ class OpBase {
   virtual void restore_side(uint32_t /*side*/, ArrowArray* /*batches*/, ArrowSchema* /*schemas*/, int64_t /*n*/) {
     throw Error(ARROYO_B200_UNSUPPORTED, name + ": restore_side is only for the join with expiration");
   }
+  // the clock the updating aggregate's time-to-idle runs on; every other operator has none
+  virtual void set_clock(int64_t /*now_ns*/) {
+    throw Error(ARROYO_B200_UNSUPPORTED, name + ": set_clock is only for the updating aggregate");
+  }
   virtual void flush() = 0;
   // enqueue whatever input is still being batched on the host side; does not wait
   virtual void submit() {}

@@ -24,13 +24,30 @@
 //           which grows it when a bucket runs out of ids), the row with the largest (_generation, position) wins per key and seeds both the
 //           live accumulators and the previous-flush snapshot, so the first flush retracts what the uninterrupted run
 //           would have retracted.
+//   ttl     time-to-idle (UpdatingCache::with_time_to_idle, updating_cache.rs:42-62; time_out at every flush,
+//           :688-705), on the clock the shim sets (arroyo_b200_op_set_clock; the library reads no clock).  Only when
+//           the ttl (config gap_ns) is > 0: the ingest stamps each row's id with the clock of its call (a store only
+//           when the stamp changes, so a hot key costs one load per row); rows that defer are drained before the
+//           clock moves, so they keep the clock of the call that brought them.  After the flush kernel,
+//           upd_expire_kernel evicts every live id with clock - stamp >= ttl: one retraction row of its previous-flush
+//           values (what the reference's evaluate() returns after the flush), the id back to identity, and
+//           flushed = 2: "evicted since the last export", which the export writes as a tombstone (null _timestamp,
+//           the reference's deletion encoding in initialize :591-614) unless the key is flushed again first.  When
+//           the ids that hold neither a live key nor a pending tombstone are half of the ids handed out (from 2^16
+//           on), the dictionary is rebuilt from the kept keys (BucketDict::rebuild) and the per-id state follows the
+//           old -> new id map, so device memory follows the live keys.  With ttl 0 none of this runs: the ingest is
+//           the TTL = false instance, and the flush and export kernels do what they did without a ttl.
 // Output rows: [key?, aggregates..., _timestamp, is_retract] -- retractions first, then appends (a key's retraction
-// must precede its append; the order between keys is unspecified in the reference too: it iterates a HashMap).
+// must precede its append; the order between keys is unspecified in the reference too: it iterates a HashMap), then
+// the eviction retractions (the reference appends them last, :690-701).
 // The shim wraps `is_retract` into the `_updating_meta` struct together with the row id its metadata expression
 // computes (:719-729).
+// Deviations with a ttl (INTEGRATION.md §3): eviction retractions leave even when the flush has no other row (the
+// reference returns None then, :703-705, after it has evicted the keys); evicted keys leave tombstones in table "a",
+// so a restore does not bring them back (the reference's table keeps their last rows).
 //
-// Not restated: retractions on the input (an updating upstream), count(distinct), TTL expiry (wall clock).  Such
-// plans are refused at construction (ARROYO_B200_UNSUPPORTED) and stay on the stock operator.
+// Not restated: retractions on the input (an updating upstream), count(distinct).  Such plans are refused at
+// construction (ARROYO_B200_UNSUPPORTED) and stay on the stock operator.
 #include <algorithm>
 #include <climits>
 
@@ -70,6 +87,11 @@ struct UIngest {
   long long* d_ts;
   long long* d_val[MAX_VALS];
   unsigned long long* deferred;
+  // TTL only: per id the clock of its last row, the clock of this launch, and the live-key count (a key becomes live
+  // on its first row after a flush that left it without rows: new, or back after an eviction)
+  long long* last;
+  long long now;
+  unsigned int* n_live;
 };
 
 __device__ __noinline__ void upd_defer_row(const UIngest& p, long long i, long long key) {
@@ -79,6 +101,7 @@ __device__ __noinline__ void upd_defer_row(const UIngest& p, long long i, long l
   for (int v = 0; v < p.n_vals; ++v) p.d_val[v][d] = p.val[v][i];
 }
 
+template <bool TTL>
 __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__ UIngest p) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -92,6 +115,7 @@ __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__
         continue;
       }
     }
+    if (TTL && p.last[id] != p.now) p.last[id] = p.now;  // every writer stores the same value
     atomicAdd(p.st.cur + id, 1ull);
 #pragma unroll
     for (int a = 1; a < MAX_ACC; ++a) {
@@ -106,7 +130,10 @@ __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__
       }
     }
     atomicMax(p.st.cur_ts + id, __ldcs(p.ts + i));
-    if (atomicExch(p.st.touched + id, 1u) == 0u) p.st.list[atomicAdd(p.st.n_touched, 1u)] = id;
+    if (atomicExch(p.st.touched + id, 1u) == 0u) {
+      p.st.list[atomicAdd(p.st.n_touched, 1u)] = id;
+      if (TTL && p.st.prev[id] == 0) atomicAdd(p.n_live, 1u);  // prev rows == 0: no rows at the last flush
+    }
   }
 }
 
@@ -164,8 +191,71 @@ __global__ void __launch_bounds__(256) upd_flush_kernel(const __grid_constant__ 
   }
 }
 
+// Expiry (time_out, :690-701), after the flush kernel: every live id idle for at least the ttl leaves as one
+// retraction row of its previous-flush values, compacted with one atomic per warp, and goes back to identity, marked
+// flushed = 2 (a tombstone for the next export).  The touched list is empty here.
+struct UExpire {
+  UState st;
+  const long long* id_keys;
+  const long long* last;
+  long long now, ttl;
+  unsigned long long n_ids;  // ids to scan: [0, n_ids)
+  int keyed;
+  int n_aggs;
+  int agg_kind[ARROYO_B200_MAX_AGGS];
+  int agg_acc[ARROYO_B200_MAX_AGGS];
+  long long* o_key;  // the eviction region of the flush's output
+  unsigned long long* o_agg[ARROYO_B200_MAX_AGGS];
+  long long* o_ts;
+  unsigned int* count;   // rows written
+  unsigned int* n_live;  // live keys, less the evicted ones
+};
+
+__global__ void __launch_bounds__(256) upd_expire_kernel(const __grid_constant__ UExpire p) {
+  unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  const unsigned int lane = threadIdx.x & 31;
+  for (; i < p.n_ids; i += stride) {
+    // clock >= every stamp >= 0: the difference cannot overflow
+    const bool mine = p.st.prev[i] != 0 && p.now - p.last[i] >= p.ttl;
+    const unsigned int active = __activemask();
+    const unsigned int mask = __ballot_sync(active, mine);
+    if (!mask) continue;
+    const int leader = __ffs(active) - 1;
+    unsigned int base = 0;
+    if ((int)lane == leader) {
+      base = atomicAdd(p.count, (unsigned int)__popc(mask));
+      atomicSub(p.n_live, (unsigned int)__popc(mask));
+    }
+    base = __shfl_sync(active, base, leader);
+    if (!mine) continue;
+    const unsigned int o = base + __popc(mask & ((1u << lane) - 1u));
+    unsigned long long old[MAX_ACC];
+    for (int a = 0; a < p.st.n_acc; ++a) old[a] = p.st.prev[(unsigned long long)a * p.st.id_cap + i];
+    if (p.keyed) p.o_key[o] = p.id_keys[i];
+    for (int g = 0; g < p.n_aggs; ++g) p.o_agg[g][o] = agg_finalise(p.agg_kind[g], old[p.agg_acc[g]], old[0]);
+    p.o_ts[o] = p.st.prev_ts[i];
+    for (int a = 0; a < p.st.n_acc; ++a) {
+      const unsigned long long v = acc_identity(p.st.acc_kind[a]);
+      p.st.cur[(unsigned long long)a * p.st.id_cap + i] = v;
+      p.st.prev[(unsigned long long)a * p.st.id_cap + i] = a == 0 ? 0 : v;
+    }
+    p.st.cur_ts[i] = LLONG_MIN;
+    p.st.prev_ts[i] = LLONG_MIN;
+    p.st.flushed[i] = 2;
+  }
+}
+
+// Compaction: the ids to keep -- a live key (rows now or at the last flush) or one with a pending export row
+__global__ void upd_keep_kernel(UState st, unsigned char* keep, uint32_t n_ids) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (; i < n_ids; i += stride) keep[i] = st.cur[i] != 0 || st.prev[i] != 0 || st.flushed[i] != 0;
+}
+
 // State export: every id flushed since the last export leaves as one row of its previous-flush snapshot (the values
-// the last flush emitted), compacted with one atomic per warp.
+// the last flush emitted), compacted with one atomic per warp; an id evicted since (flushed = 2) leaves as a
+// tombstone, o_dead[row] = 1 (o_dead is null without a ttl).
 struct UExport {
   UState st;
   const long long* id_keys;
@@ -174,6 +264,7 @@ struct UExport {
   unsigned long long* o_acc[MAX_ACC];
   long long* o_ts;
   unsigned int* count;
+  unsigned char* o_dead;
 };
 
 __global__ void __launch_bounds__(256) upd_export_kernel(const __grid_constant__ UExport p) {
@@ -191,6 +282,7 @@ __global__ void __launch_bounds__(256) upd_export_kernel(const __grid_constant__
     base = __shfl_sync(active, base, leader);
     if (!mine) continue;
     const unsigned int o = base + __popc(mask & ((1u << lane) - 1u));
+    if (p.o_dead) p.o_dead[o] = p.st.flushed[i] == 2;
     p.st.flushed[i] = 0;
     p.o_key[o] = p.id_keys[i];
     for (int a = 0; a < p.st.n_acc; ++a) p.o_acc[a][o] = p.st.prev[(unsigned long long)a * p.st.id_cap + i];
@@ -208,6 +300,10 @@ struct URestore {
   unsigned long long* best_gen;   // per id
   long long* best_pos;            // per id, -1: no row
   long long n;
+  const unsigned char* dead;      // per row, 1: a tombstone (null _timestamp); null when the table has none
+  long long* last;                // TTL only: per id, stamped with `now`
+  long long now;
+  unsigned int* won;              // [0] keys restored live, [1] keys whose winning row is a tombstone
 };
 
 // the largest generation per id, then the last row of that generation
@@ -225,13 +321,23 @@ __global__ void __launch_bounds__(256) upd_restore_pos_kernel(const __grid_const
   }
 }
 
-// the winning row seeds the live accumulators and the previous-flush snapshot alike
+// the winning row seeds the live accumulators and the previous-flush snapshot alike; a winning tombstone leaves the
+// id at identity (the key is absent)
 __global__ void __launch_bounds__(256) upd_restore_seed_kernel(const __grid_constant__ URestore p) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (; i < p.n; i += stride) {
     const unsigned int id = p.ids[i];
-    if (p.best_pos[id] != i) continue;
+    const bool win = p.best_pos[id] == i;
+    const bool dead = win && p.dead && p.dead[i];
+    const unsigned int active = __activemask();
+    const unsigned int live_mask = __ballot_sync(active, win && !dead), dead_mask = __ballot_sync(active, dead);
+    if ((int)(threadIdx.x & 31) == __ffs(active) - 1) {  // one atomic per warp
+      if (live_mask) atomicAdd(p.won, (unsigned int)__popc(live_mask));
+      if (dead_mask) atomicAdd(p.won + 1, (unsigned int)__popc(dead_mask));
+    }
+    if (!win || dead) continue;
+    if (p.last) p.last[id] = p.now;
     for (int a = 0; a < p.st.n_acc; ++a) {
       const unsigned long long v = p.val[a] ? p.val[a][i] : 1ull;
       p.st.cur[(unsigned long long)a * p.st.id_cap + id] = v;
@@ -258,8 +364,9 @@ __global__ void upd_init_kernel(UState st, unsigned long long n) {
   }
 }
 
-// after the dictionary grew: new[map[i]] = old[i]
-__global__ void upd_permute_kernel(UState o, UState n, const uint32_t* __restrict__ map, uint32_t old_ids) {
+// after the dictionary grew or was rebuilt: new[map[i]] = old[i]; o_last / n_last (the TTL stamps) may be null
+__global__ void upd_permute_kernel(UState o, UState n, const long long* o_last, long long* n_last,
+                                   const uint32_t* __restrict__ map, uint32_t old_ids) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const uint32_t stride = gridDim.x * blockDim.x;
   for (; i < old_ids; i += stride) {
@@ -273,6 +380,7 @@ __global__ void upd_permute_kernel(UState o, UState n, const uint32_t* __restric
     n.prev_ts[m] = o.prev_ts[i];
     n.touched[m] = o.touched[i];
     n.flushed[m] = o.flushed[i];
+    if (n_last) n_last[m] = o_last[i];
   }
 }
 __global__ void upd_remap_list_kernel(unsigned int* list, unsigned int n, const uint32_t* __restrict__ map) {
@@ -295,13 +403,18 @@ class UpdatingAggOp final : public OpBase {
   }
   void handle_tick(BatchesPriv* out) override { flush_to(out); }  // :994-1004
   void checkpoint_state(BatchesPriv* out) override;
+  void set_clock(int64_t now_ns) override;
   void flush() override {
     set_device();
     AB_CUDA(cudaStreamSynchronize(stream_));
   }
   void stats(ArroyoB200Stats* out) override {
     st_.n_keys = 0;
-    if (plan_.keyed) {
+    if (plan_.keyed && ttl_ns_ > 0) {
+      set_device();
+      drain_deferred();
+      st_.n_keys = read_live();
+    } else if (plan_.keyed) {
       set_device();
       drain_deferred();  // also reads the dictionary's count (ids from BD_ID_BASE on)
       // id 0 is the INT64_MIN key's: it has rows once that key arrived
@@ -332,8 +445,14 @@ class UpdatingAggOp final : public OpBase {
   // generation the next export writes, and the export's output buffers
   uint64_t unexported_ = 0, generation_ = 0, state_cap_ = 0;
   bool restored_ = false;
-  DevBuf s_key_, s_ts_, s_acc_[MAX_ACC];
+  DevBuf s_key_, s_ts_, s_acc_[MAX_ACC], s_dead_;
   ArroyoB200Stats st_{};
+  // time-to-idle: the ttl (0: keys never expire), the clock, per id the clock of its last row, [live keys, evicted
+  // by the last expiry pass] (u32), the evictions since the last export (an upper bound on the pending tombstones),
+  // and the dictionary's size at construction (a compaction does not go below it)
+  int64_t ttl_ns_ = 0, clock_ = 0;
+  DevBuf last_, ttl_counters_;
+  uint64_t tombstones_ = 0, min_buckets_ = 1;
 
   // One column of table "a" after the key: its Arrow format and what it holds.
   enum StateRole { S_ROWS, S_ACC, S_TS, S_GEN };
@@ -348,11 +467,18 @@ class UpdatingAggOp final : public OpBase {
   UState state_view() const;
   void alloc_state();
   void grow();
+  void follow(const UState& old_s, const BdGrowth& g);
+  uint32_t read_live();
+  void maybe_compact(uint64_t live);
+  void compact();
   void reserve_defer(int set, uint64_t rows);
   void drain_deferred();
   void ensure_room(uint64_t new_rows);
   void ingest(const AggCols& d, int64_t n);
   void flush_to(BatchesPriv* out);
+  void launch_flush(unsigned int n);
+  void launch_expire(unsigned int n);
+  void export_state(BatchesPriv* out, unsigned int rows, bool dead);
 };
 
 UpdatingAggOp::UpdatingAggOp(const ArroyoB200OpConfig& c) {
@@ -363,13 +489,20 @@ UpdatingAggOp::UpdatingAggOp(const ArroyoB200OpConfig& c) {
   // AVG sums the inputs as f64, like the reference's accumulator (each value cast to f64, then added): an integer
   // sum would wrap and average to garbage once the values pass 2^63 in total
   plan_ = AggPlan(c, ACC_SUM_F64);
+  AB_REQUIRE(c.gap_ns >= 0, ARROYO_B200_INVALID_ARGUMENT, "updating aggregate: negative ttl (gap_ns)");
+  ttl_ns_ = c.gap_ns;
   open_device(c);
   counters_.alloc(32);
   AB_CUDA(cudaMemsetAsync(counters_.p, 0, 32, stream_));
   n_total_.alloc(4);
   AB_CUDA(cudaMemsetAsync(n_total_.p, 0, 4, stream_));
+  if (ttl_ns_ > 0) {
+    ttl_counters_.alloc(8);
+    AB_CUDA(cudaMemsetAsync(ttl_counters_.p, 0, 8, stream_));
+  }
   dict_.init(stream_, num_sms_, plan_.keyed, n_total_.as<unsigned int>(), &st_.kernel_launches);
-  dict_.alloc(plan_.keyed ? bd_buckets_for(c.expected_keys ? c.expected_keys : (1ull << 16)) : 1);
+  min_buckets_ = plan_.keyed ? bd_buckets_for(c.expected_keys ? c.expected_keys : (1ull << 16)) : 1;
+  dict_.alloc(min_buckets_);
   alloc_state();
   AB_CUDA(cudaStreamSynchronize(stream_));
 }
@@ -405,6 +538,10 @@ void UpdatingAggOp::alloc_state() {
   touched_.alloc(id_cap * 4);
   flushed_.alloc(id_cap);
   list_.alloc(id_cap * 4);
+  if (ttl_ns_ > 0) {
+    last_.alloc(id_cap * 8);
+    AB_CUDA(cudaMemsetAsync(last_.p, 0, id_cap * 8, stream_));
+  }
   upd_init_kernel<<<num_sms_ * 4, 256, 0, stream_>>>(state_view(), id_cap);
   AB_CUDA(cudaGetLastError());
   ++st_.kernel_launches;
@@ -414,15 +551,20 @@ void UpdatingAggOp::alloc_state() {
 // state and the touched list follow the old -> new id map.
 void UpdatingAggOp::grow() {
   const UState old_s = state_view();
-  const BdGrowth g = dict_.grow();
+  follow(old_s, dict_.grow());
+}
+
+// The per-id state (viewed by `old_s`), the TTL stamps and the touched list move to the dictionary's new ids.
+void UpdatingAggOp::follow(const UState& old_s, const BdGrowth& g) {
   DevBuf k_cur = std::move(cur_), k_prev = std::move(prev_), k_cts = std::move(cur_ts_), k_pts = std::move(prev_ts_),
-         k_t = std::move(touched_), k_f = std::move(flushed_), k_list = std::move(list_);
+         k_t = std::move(touched_), k_f = std::move(flushed_), k_list = std::move(list_), k_last = std::move(last_);
   unsigned int h_touched = 0;
   AB_CUDA(cudaMemcpyAsync(&h_touched, counters_.p, 4, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
   alloc_state();
   const int grid = (int)std::min<uint64_t>((g.old_ids + 255) / 256, (uint64_t)num_sms_ * 8);
-  upd_permute_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_s, state_view(), g.map.as<uint32_t>(), g.old_ids);
+  upd_permute_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_s, state_view(), k_last.as<long long>(),
+                                                             last_.as<long long>(), g.map.as<uint32_t>(), g.old_ids);
   AB_CUDA(cudaGetLastError());
   ++st_.kernel_launches;
   if (h_touched) {
@@ -433,6 +575,50 @@ void UpdatingAggOp::grow() {
   }
   AB_CUDA(cudaMemcpyAsync(&total_keys_, n_total_.p, 4, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+// TTL only: the live-key count
+uint32_t UpdatingAggOp::read_live() {
+  uint32_t live = 0;
+  AB_CUDA(cudaMemcpyAsync(&live, ttl_counters_.p, 4, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  return live;
+}
+
+// After an expiry pass or an export (TTL only): once the ids handed out that hold neither a live key (`live` of
+// them) nor a pending tombstone are at least half of them, from 2^16 ids on, the dictionary is rebuilt from the kept
+// keys and the per-id state follows.  Id 0 (the INT64_MIN key) keeps its place.
+void UpdatingAggOp::maybe_compact(uint64_t live) {
+  constexpr uint64_t COMPACT_MIN_IDS = 1ull << 16;
+  if (!plan_.keyed || total_keys_ < COMPACT_MIN_IDS) return;
+  const uint64_t kept = std::min<uint64_t>(live + tombstones_, total_keys_);
+  if (2 * (total_keys_ - kept) < total_keys_) return;
+  compact();
+}
+
+// Rebuilds the dictionary from the keys of the ids that hold a live key or a pending export row.
+void UpdatingAggOp::compact() {
+  const UState old_s = state_view();
+  const uint32_t n_ids = dict_.n_ids();
+  DevBuf keep(n_ids);
+  const int grid = (int)std::min<uint64_t>((n_ids + 255) / 256, (uint64_t)num_sms_ * 8);
+  upd_keep_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(old_s, keep.as<unsigned char>(), n_ids);
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  follow(old_s, dict_.rebuild(keep.as<unsigned char>(), min_buckets_));
+}
+
+void UpdatingAggOp::set_clock(int64_t now_ns) {
+  AB_REQUIRE(now_ns >= clock_, ARROYO_B200_INVALID_ARGUMENT,
+             "updating aggregate: the clock moved backwards (" + std::to_string(now_ns) + " < " +
+                 std::to_string(clock_) + ")");
+  if (now_ns == clock_) return;
+  // rows that deferred are stamped when they are re-ingested: with the clock of the call that brought them
+  if (ttl_ns_ > 0 && plan_.keyed) {
+    set_device();
+    drain_deferred();
+  }
+  clock_ = now_ns;
 }
 
 void UpdatingAggOp::reserve_defer(int set, uint64_t rows) {
@@ -505,7 +691,14 @@ void UpdatingAggOp::ingest(const AggCols& d, int64_t n) {
   }
   p.deferred = reinterpret_cast<unsigned long long*>((char*)counters_.p + 16);
   const int grid = (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms_ * 8);
-  upd_ingest_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(p);
+  if (ttl_ns_ > 0) {
+    p.last = last_.as<long long>();
+    p.now = clock_;
+    p.n_live = ttl_counters_.as<unsigned int>();
+    upd_ingest_kernel<true><<<std::max(grid, 1), 256, 0, stream_>>>(p);
+  } else {
+    upd_ingest_kernel<false><<<std::max(grid, 1), 256, 0, stream_>>>(p);
+  }
   AB_CUDA(cudaGetLastError());
   ++st_.kernel_launches;
   ++st_.ingest_launches;
@@ -543,24 +736,78 @@ static void* d2h_part(const void* dev, size_t off_rows, int64_t n, void* host, s
   return host;
 }
 
-// flush (:637-738): one batch [key?, aggregates..., _timestamp, is_retract], or nothing when no key changed
+// flush (:637-738): one batch [key?, aggregates..., _timestamp, is_retract], or nothing when no key changed (and,
+// with a ttl, none expired).  Output regions: retractions at [0, n), appends at [n, 2n), evictions at [2n, ...).
 void UpdatingAggOp::flush_to(BatchesPriv* out) {
   set_device();
   if (plan_.keyed) drain_deferred();
   struct {
     unsigned int touched, retracts, appends, pad;
   } h{};
+  const bool ttl = ttl_ns_ > 0;
+  unsigned int ttl_h[2] = {0, 0};  // live keys, evicted
   AB_CUDA(cudaMemcpyAsync(&h, counters_.p, 16, cudaMemcpyDeviceToHost, stream_));
+  if (ttl) AB_CUDA(cudaMemcpyAsync(ttl_h, ttl_counters_.p, 8, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
   const unsigned int n = h.touched;
-  if (n == 0 || !out) return;
+  const unsigned int live = ttl_h[0];  // the flush kernel does not change it: every key the expiry pass may evict
+  if ((n == 0 && live == 0) || !out) return;
   unexported_ += n;
-  if (2ull * n > out_cap_) {
-    out_cap_ = std::max<uint64_t>(2ull * n, 1024);
+  const uint64_t cap = 2ull * n + live;
+  if (cap > out_cap_) {
+    out_cap_ = std::max<uint64_t>(cap, 1024);
     o_key_.alloc(out_cap_ * 8);
     o_ts_.alloc(out_cap_ * 8);
     for (int g = 0; g < plan_.n_aggs; ++g) o_agg_[g].alloc(out_cap_ * 8);
   }
+  if (n) launch_flush(n);
+  if (ttl) launch_expire(n);
+  AB_CUDA(cudaMemcpyAsync(&h, counters_.p, 16, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaMemsetAsync(counters_.p, 0, 16, stream_));  // touched list and output counters start over
+  if (ttl) AB_CUDA(cudaMemcpyAsync(ttl_h, ttl_counters_.p, 8, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  const int64_t nr = h.retracts, na = h.appends, ne = ttl_h[1], total = nr + na + ne;
+  unexported_ += (uint64_t)ne;
+  tombstones_ += (uint64_t)ne;
+  if (total > 0) {
+    std::vector<OutColumn> cols;
+    auto column = [&](const char* nm, const std::string& fmt, const void* dev) {
+      OutColumn c;
+      c.name = nm;
+      c.format = fmt;
+      void* host = PinnedPool::get().alloc((size_t)std::max<int64_t>(total, 1) * 8);
+      d2h_part(dev, 0, nr, host, 0, stream_);
+      d2h_part(dev, n, na, host, (size_t)nr, stream_);
+      d2h_part(dev, 2ull * n, ne, host, (size_t)(nr + na), stream_);
+      st_.d2h_bytes += (uint64_t)total * 8;
+      c.data = host;
+      cols.push_back(c);
+    };
+    if (plan_.keyed) column("key", key_format_, o_key_.p);
+    for (int g = 0; g < plan_.n_aggs; ++g) column(("agg" + std::to_string(g)).c_str(), plan_.agg_format[g], o_agg_[g].p);
+    column("_timestamp", "tsn:", o_ts_.p);
+    {
+      OutColumn r;
+      r.name = "is_retract";
+      r.format = "b";
+      unsigned char* bits = (unsigned char*)PinnedPool::get().alloc((size_t)(total + 7) / 8 + 8);
+      memset(bits, 0, (size_t)(total + 7) / 8 + 8);
+      for (int64_t i = 0; i < nr; ++i) bits[i >> 3] |= (unsigned char)(1u << (i & 7));
+      for (int64_t i = nr + na; i < total; ++i) bits[i >> 3] |= (unsigned char)(1u << (i & 7));
+      r.data = bits;
+      cols.push_back(r);
+    }
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    st_.rows_out += (uint64_t)total;
+    ++st_.windows_out;
+    out->arrays.emplace_back();
+    out->schemas.emplace_back();
+    export_batch(cols, total, &out->arrays.back(), &out->schemas.back());
+  }
+  if (ne) maybe_compact(live - (uint64_t)ne);
+}
+
+void UpdatingAggOp::launch_flush(unsigned int n) {
   UFlush p{};
   p.st = state_view();
   p.id_keys = dict_.id_keys();
@@ -580,42 +827,34 @@ void UpdatingAggOp::flush_to(BatchesPriv* out) {
   AB_CUDA(cudaGetLastError());
   ++st_.kernel_launches;
   ++st_.emit_launches;
-  AB_CUDA(cudaMemcpyAsync(&h, counters_.p, 16, cudaMemcpyDeviceToHost, stream_));
-  AB_CUDA(cudaMemsetAsync(counters_.p, 0, 16, stream_));  // touched list and output counters start over
-  AB_CUDA(cudaStreamSynchronize(stream_));
-  const int64_t nr = h.retracts, na = h.appends, total = nr + na;
-  if (total == 0) return;
-  std::vector<OutColumn> cols;
-  auto column = [&](const char* nm, const std::string& fmt, const void* dev) {
-    OutColumn c;
-    c.name = nm;
-    c.format = fmt;
-    void* host = PinnedPool::get().alloc((size_t)std::max<int64_t>(total, 1) * 8);
-    d2h_part(dev, 0, nr, host, 0, stream_);
-    d2h_part(dev, n, na, host, (size_t)nr, stream_);
-    st_.d2h_bytes += (uint64_t)total * 8;
-    c.data = host;
-    cols.push_back(c);
-  };
-  if (plan_.keyed) column("key", key_format_, o_key_.p);
-  for (int g = 0; g < plan_.n_aggs; ++g) column(("agg" + std::to_string(g)).c_str(), plan_.agg_format[g], o_agg_[g].p);
-  column("_timestamp", "tsn:", o_ts_.p);
-  {
-    OutColumn r;
-    r.name = "is_retract";
-    r.format = "b";
-    unsigned char* bits = (unsigned char*)PinnedPool::get().alloc((size_t)(total + 7) / 8 + 8);
-    memset(bits, 0, (size_t)(total + 7) / 8 + 8);
-    for (int64_t i = 0; i < nr; ++i) bits[i >> 3] |= (unsigned char)(1u << (i & 7));
-    r.data = bits;
-    cols.push_back(r);
+}
+
+// The expiry pass after the flush kernel of a flush with `n` touched keys: its rows go after the 2n of the flush.
+void UpdatingAggOp::launch_expire(unsigned int n) {
+  UExpire p{};
+  p.st = state_view();
+  p.id_keys = dict_.id_keys();
+  p.last = last_.as<long long>();
+  p.now = clock_;
+  p.ttl = ttl_ns_;
+  p.n_ids = plan_.keyed ? dict_.n_ids() : 1;
+  p.keyed = plan_.keyed ? 1 : 0;
+  p.n_aggs = plan_.n_aggs;
+  for (int g = 0; g < plan_.n_aggs; ++g) {
+    p.agg_kind[g] = plan_.agg_kind[g];
+    p.agg_acc[g] = plan_.agg_acc[g];
+    p.o_agg[g] = o_agg_[g].as<unsigned long long>() + 2ull * n;
   }
-  AB_CUDA(cudaStreamSynchronize(stream_));
-  st_.rows_out += (uint64_t)total;
-  ++st_.windows_out;
-  out->arrays.emplace_back();
-  out->schemas.emplace_back();
-  export_batch(cols, total, &out->arrays.back(), &out->schemas.back());
+  p.o_key = o_key_.as<long long>() + 2ull * n;
+  p.o_ts = o_ts_.as<long long>() + 2ull * n;
+  p.n_live = ttl_counters_.as<unsigned int>();
+  p.count = p.n_live + 1;
+  AB_CUDA(cudaMemsetAsync(p.count, 0, 4, stream_));
+  const int grid = (int)std::min<uint64_t>((p.n_ids + 255) / 256, (uint64_t)num_sms_ * 8);
+  upd_expire_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  ++st_.emit_launches;
 }
 
 
@@ -667,6 +906,11 @@ void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
   for (int a = 0; a < plan_.n_acc; ++a) p.o_acc[a] = s_acc_[a].as<unsigned long long>();
   p.o_ts = s_ts_.as<long long>();
   p.count = count;
+  const bool dead = tombstones_ > 0;  // evictions since the last export: rows may be tombstones
+  if (dead) {
+    if (s_dead_.bytes < cap) s_dead_.alloc(state_cap_);
+    p.o_dead = s_dead_.as<unsigned char>();
+  }
   const int grid = (int)std::min<uint64_t>((n_ids + 255) / 256, (uint64_t)num_sms_ * 8);
   upd_export_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(p);
   AB_CUDA(cudaGetLastError());
@@ -675,7 +919,14 @@ void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
   AB_CUDA(cudaMemcpyAsync(&rows, count, 4, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
   unexported_ = 0;
-  if (rows == 0) return;
+  tombstones_ = 0;
+  if (rows > 0) export_state(out, rows, dead);
+  if (dead) maybe_compact(read_live());
+}
+
+// The table-"a" batch of the `rows` rows the export kernel wrote; with `dead`, the rows it marked are tombstones: a
+// null `_timestamp`.
+void UpdatingAggOp::export_state(BatchesPriv* out, unsigned int rows, bool dead) {
   std::vector<OutColumn> cols;
   auto column = [&](const std::string& name, const std::string& format, const void* dev) {
     OutColumn c;
@@ -703,7 +954,21 @@ void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
       column(name, sc.format, s_acc_[sc.role == S_ROWS ? 0 : sc.acc].p);
     }
   }
+  const unsigned char* is_dead = dead ? (const unsigned char*)d2h_pinned(s_dead_.p, rows, stream_, &st_.d2h_bytes) : nullptr;
   AB_CUDA(cudaStreamSynchronize(stream_));
+  if (is_dead) {
+    OutColumn& ts = cols[(plan_.keyed ? 1 : 0) + layout.size() - 2];
+    uint8_t* valid = (uint8_t*)PinnedPool::get().alloc((size_t)rows / 8 + 8);
+    memset(valid, 0, (size_t)rows / 8 + 8);
+    for (unsigned int r = 0; r < rows; ++r) {
+      if (is_dead[r]) ++ts.null_count;
+      else valid[r >> 3] |= (uint8_t)(1u << (r & 7));
+    }
+    PinnedPool::get().free((void*)is_dead);
+    ts.nullable = true;
+    if (ts.null_count) ts.validity = valid;
+    else PinnedPool::get().free(valid);
+  }
   ++generation_;
   out->arrays.emplace_back();
   out->schemas.emplace_back();
@@ -724,8 +989,8 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   std::vector<int64_t> rows((size_t)n, 0);
   int64_t total = 0;
   for (int64_t b = 0; b < n; ++b) {
-    try {
-      batches[b] = import_batch(&state[b], &schemas[b], &rows[b]);
+    try {  // `_timestamp` may be null: a tombstone
+      batches[b] = import_batch(&state[b], &schemas[b], &rows[b], kc + (int64_t)layout.size() - 2);
     } catch (const Error& e) {
       throw Error(ARROYO_B200_INVALID_ARGUMENT, std::string("state batch: ") + e.what());
     }
@@ -801,6 +1066,27 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   uint64_t max_gen = 0;
   for (int64_t b = 0; b < n; ++b)
     for (int64_t i = 0; i < rows[b]; ++i) max_gen = std::max<uint64_t>(max_gen, batches[b][gen_col].data[i]);
+  // tombstones: the rows whose `_timestamp` is null
+  DevBuf d_dead;
+  bool any_dead = false;
+  for (int64_t b = 0; b < n; ++b) any_dead = any_dead || batches[b][ts_col].validity != nullptr;
+  if (any_dead) {
+    std::vector<unsigned char> h_dead((size_t)total, 0);
+    int64_t off = 0;
+    for (int64_t b = 0; b < n; ++b) {
+      const InColumn& c = batches[b][ts_col];
+      for (int64_t i = 0; c.validity && i < rows[b]; ++i) {
+        const int64_t bit = c.validity_bit + i;
+        h_dead[off + i] = !((c.validity[bit >> 3] >> (bit & 7)) & 1);
+      }
+      off += rows[b];
+    }
+    d_dead.alloc((size_t)total);
+    AB_CUDA(cudaMemcpyAsync(d_dead.p, h_dead.data(), (size_t)total, cudaMemcpyHostToDevice, stream_));
+    AB_CUDA(cudaStreamSynchronize(stream_));  // h_dead goes when this block ends
+    st_.h2d_bytes += (uint64_t)total;
+    p.dead = d_dead.as<unsigned char>();
+  }
   DevBuf ids((size_t)total * 4);
   dict_.place(plan_.keyed ? d_key.as<long long>() : nullptr, total, ids.as<uint32_t>(), [&] { grow(); });
   p.gen = d_gen.as<unsigned long long>();
@@ -815,6 +1101,13 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   AB_CUDA(cudaMemsetAsync(best_pos.p, 0xFF, id_cap * 8, stream_));  // -1
   p.best_gen = best_gen.as<unsigned long long>();
   p.best_pos = best_pos.as<long long>();
+  DevBuf won(8);
+  AB_CUDA(cudaMemsetAsync(won.p, 0, 8, stream_));
+  p.won = won.as<unsigned int>();
+  if (ttl_ns_ > 0) {
+    p.last = last_.as<long long>();
+    p.now = clock_;
+  }
   upd_restore_gen_kernel<<<grid, 256, 0, stream_>>>(p);
   AB_CUDA(cudaGetLastError());
   upd_restore_pos_kernel<<<grid, 256, 0, stream_>>>(p);
@@ -822,8 +1115,14 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   upd_restore_seed_kernel<<<grid, 256, 0, stream_>>>(p);
   AB_CUDA(cudaGetLastError());
   st_.kernel_launches += 3;
+  if (ttl_ns_ > 0)  // the operator was empty: the live keys are the restored ones
+    AB_CUDA(cudaMemcpyAsync(ttl_counters_.p, won.p, 4, cudaMemcpyDeviceToDevice, stream_));
+  unsigned int h_won[2] = {0, 0};
+  AB_CUDA(cudaMemcpyAsync(h_won, won.p, 8, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaMemcpyAsync(&total_keys_, n_total_.p, 4, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
+  // keys whose latest row is a tombstone hold ids without state: give them back, so n_keys counts live keys
+  if (h_won[1] && plan_.keyed) compact();
   generation_ = max_gen + 1;
   restored_ = true;
   take_all();

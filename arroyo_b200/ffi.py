@@ -122,6 +122,7 @@ SYMBOLS = [
                                                                 C.POINTER(C.c_int64)]),
     ("arroyo_b200_op_handle_checkpoint", C.c_int32, [_VP, C.c_int64, C.POINTER(Batches)]),
     ("arroyo_b200_op_checkpoint_state", C.c_int32, [_VP, C.POINTER(Batches)]),
+    ("arroyo_b200_op_set_clock", C.c_int32, [_VP, C.c_int64]),
     ("arroyo_b200_op_on_close", C.c_int32, [_VP, C.c_int32, C.POINTER(Batches)]),
     ("arroyo_b200_op_handle_tick", C.c_int32, [_VP, C.POINTER(Batches)]),
     ("arroyo_b200_op_process_batch_emit", C.c_int32, [_VP, C.c_uint32, C.c_uint32, C.POINTER(ArrowArray), C.POINTER(ArrowSchema),

@@ -7,6 +7,7 @@ handle_checkpoint(barrier, ctx, collector), on_close(final_message, ctx, collect
 Batches are pyarrow RecordBatches crossing the boundary through the Arrow C Data Interface."""
 import ctypes as C
 import functools
+import time
 from typing import List, Optional
 
 import pyarrow as pa
@@ -530,14 +531,23 @@ class UpdatingAggregatingFunc(_NativeOperator):
     and `aggs` (oracle.updating_oracle.UpdatingAggConfig has the shape).  Append-only inputs only.
 
     State: a checkpoint also writes the accumulators of the keys flushed since the last checkpoint to the key-value
-    table "a" (`state_names()` columns, :619-635), and `on_start` restores them from it (:446-503)."""
+    table "a" (`state_names()` columns, :619-635), and `on_start` restores them from it (:446-503).
+
+    Time-to-idle: `ttl` in ns, read as the reference reads `ttl_micros` (0 means 24 h, :1043-1048); a flush then
+    retracts and drops every key idle for at least `ttl` on the clock `clock()` (ns, default time.monotonic_ns), which
+    is passed to the library before every call that ingests, flushes or restores.  `ttl=None`: keys never expire and
+    the clock is never read."""
     kind = ffi.UPDATING_AGGREGATE
     IS_RETRACT = "_is_retract"
+    DEFAULT_TTL_NS = 24 * 60 * 60 * 1_000_000_000
 
-    def __init__(self, config, input_schema: Optional[pa.Schema] = None, updating_input: bool = False, **kw):
+    def __init__(self, config, input_schema: Optional[pa.Schema] = None, updating_input: bool = False,
+                 ttl: Optional[int] = None, clock=None, **kw):
         super().__init__(**kw)
         self.config = config
         self.updating_input = updating_input
+        self.ttl = None if ttl is None else (int(ttl) or self.DEFAULT_TTL_NS)
+        self.clock = clock or time.monotonic_ns
         self._key_type = None
         if input_schema is not None:
             self._build(input_schema.names)
@@ -568,13 +578,20 @@ class UpdatingAggregatingFunc(_NativeOperator):
             return
         if not self.created:
             raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "restore needs input_schema at construction")
+        self._tick_clock()
         self._on_start(batches, ffi.INT64_MIN, ffi.INT64_MIN)
 
     def _build(self, names: List[str]):
         cfg = _agg_config(self.kind, self.config, names)
+        cfg.gap_ns = self.ttl or 0
         if self.updating_input:
             self._flags |= ffi.FLAG_UPDATING_INPUT
         self._create(cfg)
+
+    def _tick_clock(self):
+        """arroyo_b200_op_set_clock(clock()) before a call that stamps, expires or restores (with a ttl only)."""
+        if self.ttl is not None and self.created:
+            _check(self._lib, self._h, self._lib.arroyo_b200_op_set_clock(self._h, int(self.clock())))
 
     def output_names(self) -> List[str]:
         return list(self.config.key_names) + [a.name for a in self.config.aggs] + [TIMESTAMP, self.IS_RETRACT]
@@ -583,16 +600,19 @@ class UpdatingAggregatingFunc(_NativeOperator):
         if not self.created:
             self._build(batch.schema.names)
         self._note_key_type(batch.schema)
+        self._tick_clock()
         self._process_batch(self._lib.arroyo_b200_op_process_batch, 0, 1, batch)
 
     def process_device_batch(self, cols: List[int], n_rows: int):
         """`cols` = device pointers (ints), one per input column; needs `input_schema` at construction."""
         arr = (C.c_uint64 * len(cols))(*cols)
+        self._tick_clock()
         _check(self._lib, self._h, self._lib.arroyo_b200_op_process_device_batch(self._h, 0, 1, arr, len(cols), n_rows))
 
     def process_device_batches(self, cols_flat, n_rows, n_cols: int):
         """A run of device batches in one FFI call; `cols_flat`/`n_rows` are prebuilt ctypes arrays
         ((c_uint64 * (n_batches * n_cols)), (c_int64 * n_batches))."""
+        self._tick_clock()
         st = self._lib.arroyo_b200_op_process_device_batches(self._h, 0, 1, cols_flat, n_cols, n_rows, len(n_rows))
         _check(self._lib, self._h, st)
 
@@ -617,6 +637,7 @@ class UpdatingAggregatingFunc(_NativeOperator):
         if not self.created:
             return
         out = ffi.Batches()
+        self._tick_clock()
         _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_tick(self._h, C.byref(out)))
         self._emit(out, collector)
 
@@ -624,6 +645,7 @@ class UpdatingAggregatingFunc(_NativeOperator):
         if not self.created:
             return
         out = ffi.Batches()
+        self._tick_clock()
         _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_checkpoint(self._h, ffi.INT64_MIN, C.byref(out)))
         self._emit(out, collector)
         if ctx is not None:  # then the state of the keys flushed since the last checkpoint (:951-961)
@@ -641,6 +663,7 @@ class UpdatingAggregatingFunc(_NativeOperator):
         if not self.created:
             return
         out = ffi.Batches()
+        self._tick_clock()
         _check(self._lib, self._h, self._lib.arroyo_b200_op_on_close(self._h, 1 if final_message == "end_of_data" else 0,
                                                                       C.byref(out)))
         self._emit(out, collector)

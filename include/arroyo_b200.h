@@ -155,7 +155,12 @@ typedef struct ArroyoB200OpConfig {
                          /* INSTANT_AGGREGATE: read only when final_projection = 1, as  */
                          /* the upstream window's width W (> 0) of the window struct    */
   int64_t slide_ns;      /* slide_micros * 1000 (sliding only)                          */
-  int64_t gap_ns;        /* gap_micros * 1000 (session only)                            */
+  int64_t gap_ns;        /* gap_micros * 1000 (session)                                 */
+                         /* UPDATING_AGGREGATE: the time-to-idle ttl in ns, 0 = keys    */
+                         /* never expire, < 0 = INVALID_ARGUMENT.  A shim passes        */
+                         /* ttl_micros * 1000, or 24 h when ttl_micros == 0, as the     */
+                         /* reference does (incremental_aggregator.rs:1043-1048); see   */
+                         /* arroyo_b200_op_set_clock                                    */
 
   int32_t n_cols;        /* columns in each input batch (join: left side)               */
   int32_t timestamp_col; /* ArroyoSchema.timestamp_index                                */
@@ -298,6 +303,8 @@ const char* arroyo_b200_op_name(const ArroyoB200Op* op);
  * ARROYO_B200_INVALID_ARGUMENT, with nothing changed: a column count or type that is not the plan's
  * layout, or an operator that has already taken rows or been restored.  Restored rows do not count in
  * `rows_in`; their keys count in `n_keys`.
+ * A null `_timestamp` (and only there) marks a tombstone: when it wins, its key stays absent (see
+ * arroyo_b200_op_set_clock).  With a ttl, restored keys are stamped with the clock at this call.
  * TTL join: `n > 0` => ARROYO_B200_UNSUPPORTED; its tables go through arroyo_b200_op_restore_side. */
 int32_t arroyo_b200_op_on_start(ArroyoB200Op* op, struct ArrowArray* state, struct ArrowSchema* schemas,
                                 int64_t n, int64_t watermark_ns, int64_t table_min_time_ns);
@@ -425,6 +432,26 @@ int32_t arroyo_b200_op_handle_checkpoint(ArroyoB200Op* op, int64_t watermark_ns,
  * generation, larger than any the operator wrote or restored before.  State rows count in no statistic
  * but `d2h_bytes`.  Every other operator kind returns no batches. */
 int32_t arroyo_b200_op_checkpoint_state(ArroyoB200Op* op, ArroyoB200Batches* state_out);
+
+/* The updating aggregate's clock for its time-to-idle ttl (`gap_ns`): the reference's `Instant::now()`, which the shim
+ * reads from a monotonic source and passes in ns before every call that ingests, flushes or restores.  The library
+ * never reads a clock of its own.  The clock starts at 0; a value below the current one => ARROYO_B200_INVALID_ARGUMENT,
+ * nothing changed.  Every other operator kind => ARROYO_B200_UNSUPPORTED.
+ * Time-to-idle (UpdatingCache::with_time_to_idle, updating_cache.rs:42-62; incremental_aggregator.rs:688-705):
+ *  - every row ingested by process_batch, process_device_batch(es) or run_batches sets its key's last-update time to
+ *    the clock at that call (rows deferred for dictionary growth included);
+ *  - a flush (handle_tick, handle_checkpoint, on_close with end of data) first emits the change rows as without a
+ *    ttl, then evicts every live key with clock - last update >= ttl: one retraction row with the values and
+ *    `_timestamp` the key's last flush emitted, and its state is dropped.  A key that returns is a new key (append
+ *    only).  The unkeyed plan's one group expires the same way.  Rows of one flush: retractions, appends, eviction
+ *    retractions.  Eviction retractions leave even when the flush has no other row (the reference loses them then);
+ *  - the next checkpoint_state writes a tombstone for every key evicted since the last export and not flushed again:
+ *    a table-"a" row with a null `_timestamp` (the reference's deletion encoding, :591-614).  on_start accepts nulls
+ *    in `_timestamp` only: a winning tombstone leaves its key absent; restored keys are stamped with the clock at
+ *    on_start;
+ *  - `n_keys` counts live keys; `rows_out` includes eviction retractions.  With ttl 0 nothing expires and the clock
+ *    changes nothing. */
+int32_t arroyo_b200_op_set_clock(ArroyoB200Op* op, int64_t now_ns);
 
 /* ArrowOperator::on_close(final_message, ctx, collector) (operator.rs:1247-1256). */
 int32_t arroyo_b200_op_on_close(ArroyoB200Op* op, int32_t end_of_data, ArroyoB200Batches* out);
