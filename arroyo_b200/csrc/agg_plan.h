@@ -34,6 +34,49 @@ __host__ __device__ __forceinline__ unsigned long long acc_identity(int kind) {
   return v;
 }
 
+// What folding `b` into `a` gives for an accumulator of `kind` (ACC_ROWS and ACC_SUM_I64 add, wrapping).
+__device__ __forceinline__ unsigned long long acc_merge(int kind, unsigned long long a, unsigned long long b) {
+  switch (kind) {
+    case ACC_SUM_F64:
+      return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) + __longlong_as_double((long long)b));
+    case ACC_MIN_I64: return (unsigned long long)min((long long)a, (long long)b);
+    case ACC_MAX_I64: return (unsigned long long)max((long long)a, (long long)b);
+    default: return a + b;
+  }
+}
+
+// acc_merge of `v` into `*dst`, as one atomic.
+__device__ __forceinline__ void acc_atomic_merge(int kind, unsigned long long* dst, unsigned long long v) {
+  switch (kind) {
+    case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), __longlong_as_double((long long)v)); break;
+    case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(dst), (long long)v); break;
+    case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(dst), (long long)v); break;
+    default: atomicAdd(dst, v); break;
+  }
+}
+
+// Two SoA accumulator blocks of `cap` ids each.  After a checkpoint has written `delta`, ids [0, n) fold it into
+// `base` and start it over from the identities, so that the next checkpoint writes only the rows that arrive later.
+struct FoldParams {
+  unsigned long long* base;
+  unsigned long long* delta;
+  unsigned long long cap;
+  uint32_t n;
+  int n_acc;
+  int acc_kind[MAX_ACC];
+};
+static __global__ void acc_fold_kernel(const __grid_constant__ FoldParams p) {
+  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (; i < p.n; i += stride) {
+    for (int a = 0; a < p.n_acc; ++a) {
+      const unsigned long long off = (unsigned long long)a * p.cap + i;
+      p.base[off] = acc_merge(p.acc_kind[a], p.base[off], p.delta[off]);
+      p.delta[off] = acc_identity(p.acc_kind[a]);
+    }
+  }
+}
+
 // Output value of an aggregate of `agg_kind` (ARROYO_B200_AGG_*) whose accumulator holds `acc`: COUNT(*) is the row
 // count, AVG the f64 sum over the rows, anything else the accumulator itself.
 __device__ __forceinline__ unsigned long long agg_finalise(int agg_kind, unsigned long long acc, unsigned long long rows) {
@@ -42,6 +85,16 @@ __device__ __forceinline__ unsigned long long agg_finalise(int agg_kind, unsigne
     return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)acc) / (double)rows);
   return acc;
 }
+
+// One column of a checkpoint table after the key.
+enum StateRole { S_ROWS, S_ACC, S_TS, S_GEN };
+struct StateCol {
+  std::string name;    // agg<g>[<field>], _timestamp or _generation
+  const char* format;  // Arrow format ("tsn:": any timestamp[ns])
+  int role;            // S_ROWS: the key's row count; S_ACC: accumulator `acc`
+  int acc;             // 0 for every role but S_ACC
+  bool count_star;     // the COUNT(*) aggregate's own row count
+};
 
 struct AggPlan {
   bool keyed = false;
@@ -119,7 +172,140 @@ struct AggPlan {
     for (int v = 0; v < n_vals; ++v) d.val[v] = (const long long*)cols[val_cols[v]];
     return d;
   }
+
+  // The columns of a checkpoint table after the key, per aggregate in plan order, then `_timestamp`.
+  //  - Table "t" of the window and instant aggregates (`partial_schema`, arroyo-planner builder.rs:163-192):
+  //    COUNT(*) -> [count] Int64; SUM -> [sum] Int64; AVG -> [count] UInt64, [sum] Float64; MIN / MAX -> [min] /
+  //    [max] Int64; `_timestamp` is the pane start or the instant.
+  //  - Table "a" of the updating aggregate (`sliding_state_schema`, incremental_aggregator.rs:1083-1160): the same,
+  //    but SUM -> [sum] Int64, [count] UInt64; `_timestamp` is max(_timestamp), then `_generation` UInt64.
+  // Every count column holds the key's row count.
+  std::vector<StateCol> state_layout(bool table_a) const {
+    std::vector<StateCol> l;
+    for (int g = 0; g < n_aggs; ++g) {
+      const std::string p = "agg" + std::to_string(g);
+      const int acc = agg_acc[g];
+      switch (agg_kind[g]) {
+        case ARROYO_B200_AGG_COUNT_STAR: l.push_back({p + "[count]", "l", S_ROWS, 0, true}); break;
+        case ARROYO_B200_AGG_SUM_I64:
+          l.push_back({p + "[sum]", "l", S_ACC, acc, false});
+          if (table_a) l.push_back({p + "[count]", "L", S_ROWS, 0, false});
+          break;
+        case ARROYO_B200_AGG_AVG_I64:
+          l.push_back({p + "[count]", "L", S_ROWS, 0, false});
+          l.push_back({p + "[sum]", "g", S_ACC, acc, false});
+          break;
+        case ARROYO_B200_AGG_MIN_I64: l.push_back({p + "[min]", "l", S_ACC, acc, false}); break;
+        case ARROYO_B200_AGG_MAX_I64: l.push_back({p + "[max]", "l", S_ACC, acc, false}); break;
+      }
+    }
+    l.push_back({"_timestamp", "tsn:", S_TS, 0, false});
+    if (table_a) l.push_back({"_generation", "L", S_GEN, 0, false});
+    return l;
+  }
 };
+
+// The batches of one checkpoint table handed to on_start, imported and checked against the plan's layout: a column
+// count, key type or column type that is not the layout's is refused (INVALID_ARGUMENT) before the caller has changed
+// anything.  Table "a" may hold nulls in `_timestamp` (tombstones).  The caller takes the batches (take_batches) only
+// once its restore has succeeded.
+struct StateBatches {
+  std::vector<StateCol> layout;
+  int kc = 0;                               // key columns: the layout's columns start at kc
+  int ts_col = 0;                           // `_timestamp` (table "a": `_generation` follows it)
+  std::vector<std::vector<InColumn>> cols;  // per batch
+  std::vector<int64_t> rows;                // per batch
+  int64_t total = 0;
+  // The column each accumulator is restored from; -1: none, which only the row count can lack (each row then counts
+  // one).  The row count comes from COUNT(*)'s column, else the first count column; an accumulator from its first
+  // column, but an Int64 one before a Float64 one: an exact-sum AVG shares its integer accumulator with a SUM over the
+  // same column, whose Int64 column restores it exactly.
+  int seed[MAX_ACC];
+
+  StateBatches(const AggPlan& plan, bool table_a, const ArrowArray* state, const ArrowSchema* schemas, int64_t n)
+      : layout(plan.state_layout(table_a)), kc(plan.keyed ? 1 : 0) {
+    if (n > 0) AB_REQUIRE(state != nullptr && schemas != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null state batches");
+    ts_col = kc + (int)layout.size() - (table_a ? 2 : 1);
+    cols.resize((size_t)std::max<int64_t>(n, 0));
+    rows.assign(cols.size(), 0);
+    for (size_t b = 0; b < cols.size(); ++b) {
+      try {
+        cols[b] = import_batch(&state[b], &schemas[b], &rows[b], table_a ? ts_col : -1);
+      } catch (const Error& e) {
+        throw Error(ARROYO_B200_INVALID_ARGUMENT, std::string("state batch: ") + e.what());
+      }
+      const std::vector<InColumn>& c = cols[b];
+      AB_REQUIRE(c.size() == (size_t)kc + layout.size(), ARROYO_B200_INVALID_ARGUMENT,
+                 "state batch has " + std::to_string(c.size()) + " columns, the plan's layout " +
+                     std::to_string(kc + layout.size()));
+      if (kc) {
+        const std::string& f = c[0].format;
+        AB_REQUIRE(f == "l" || f == "L" || f.compare(0, 4, "tsn:") == 0, ARROYO_B200_INVALID_ARGUMENT,
+                   "state batch: key of type '" + f + "' (supported: l, L, tsn:)");
+      }
+      for (size_t j = 0; j < layout.size(); ++j) {
+        const std::string& f = c[kc + j].format;
+        const std::string want = layout[j].format;
+        AB_REQUIRE(want == "tsn:" ? f.compare(0, 4, "tsn:") == 0 : f == want, ARROYO_B200_INVALID_ARGUMENT,
+                   "state batch: column " + std::to_string(kc + j) + " has type '" + f + "', the layout '" + want + "'");
+      }
+      total += rows[b];
+    }
+    for (int a = 0; a < MAX_ACC; ++a) seed[a] = -1;
+    for (size_t j = 0; j < layout.size(); ++j) {
+      const StateCol& sc = layout[j];
+      const int c = kc + (int)j;
+      if (sc.role == S_ROWS && (seed[0] < 0 || (sc.count_star && !layout[seed[0] - kc].count_star))) seed[0] = c;
+      if (sc.role == S_ACC &&
+          (seed[sc.acc] < 0 || (!strcmp(layout[seed[sc.acc] - kc].format, "g") && strcmp(sc.format, "g"))))
+        seed[sc.acc] = c;
+    }
+  }
+
+  // Column `c` of batches [b0, b1), concatenated in batch order into `dst` (a row's position is its index there),
+  // copied on `s`; the copies count in `*h2d_bytes`.  The batches must outlive the copies.
+  const unsigned long long* upload(int c, int64_t b0, int64_t b1, DevBuf& dst, cudaStream_t s,
+                                   uint64_t* h2d_bytes) const {
+    int64_t n = 0;
+    for (int64_t b = b0; b < b1; ++b) n += rows[b];
+    dst.alloc((size_t)n * 8);
+    int64_t off = 0;
+    for (int64_t b = b0; b < b1; ++b) {
+      if (rows[b])
+        AB_CUDA(cudaMemcpyAsync((char*)dst.p + off * 8, cols[b][c].data, (size_t)rows[b] * 8, cudaMemcpyHostToDevice, s));
+      off += rows[b];
+    }
+    *h2d_bytes += (uint64_t)n * 8;
+    return dst.as<unsigned long long>();
+  }
+};
+
+// Takes the `n` state batches of a restore that succeeded.
+inline void take_batches(ArrowArray* state, int64_t n) {
+  for (int64_t b = 0; b < n; ++b)
+    if (state[b].release) state[b].release(&state[b]);
+}
+
+// The columns of a checkpoint table's batch of `n` rows in `layout`, copied on `s` into pinned buffers (the copies
+// count in `*d2h_bytes`): the key (`key` null: unkeyed), then the layout's columns from `acc` (one device column per
+// accumulator, acc[0] the row count) and `ts`.  `_generation` is left to the caller.  Nothing may read the columns
+// before `s` has passed the copies.
+inline std::vector<OutColumn> state_columns(const std::vector<StateCol>& layout, int64_t n, const void* key,
+                                            const std::string& key_format, const DevBuf* acc, const void* ts,
+                                            cudaStream_t s, uint64_t* d2h_bytes) {
+  std::vector<OutColumn> cols;
+  auto column = [&](const std::string& name, const std::string& format, const void* dev) {
+    OutColumn c;
+    c.name = name;
+    c.format = format;
+    c.data = d2h_pinned(dev, (size_t)n * 8, s, d2h_bytes);
+    cols.push_back(c);
+  };
+  if (key) column("key", key_format, key);
+  for (const StateCol& sc : layout)
+    if (sc.role != S_GEN) column(sc.name, sc.format, sc.role == S_TS ? ts : acc[sc.acc].p);
+  return cols;
+}
 
 // The device copies of the columns an aggregate reads from its host batches, in one buffer reused in stream order.
 struct AggStaging {

@@ -112,25 +112,6 @@ __device__ uint32_t ia_find_or_insert(const IGroups& g, long long inst, long lon
   }
 }
 
-// What folding `b` into `a` gives for an accumulator of `kind` (ACC_ROWS adds like a sum).
-__device__ __forceinline__ unsigned long long ia_combine(int kind, unsigned long long a, unsigned long long b) {
-  switch (kind) {
-    case ACC_SUM_F64: return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) + __longlong_as_double((long long)b));
-    case ACC_MIN_I64: return (unsigned long long)min((long long)a, (long long)b);
-    case ACC_MAX_I64: return (unsigned long long)max((long long)a, (long long)b);
-    default: return a + b;
-  }
-}
-
-__device__ __forceinline__ void ia_atomic(int kind, unsigned long long* dst, unsigned long long v) {
-  switch (kind) {
-    case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), __longlong_as_double((long long)v)); break;
-    case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(dst), (long long)v); break;
-    case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(dst), (long long)v); break;
-    default: atomicAdd(dst, v); break;
-  }
-}
-
 struct IIngest {
   IGroups g;
   const long long* key;
@@ -185,7 +166,7 @@ __global__ void __launch_bounds__(IA_THREADS) ia_ingest_kernel(const __grid_cons
       for (int a = 1; a < MAX_ACC; ++a) {
         if (a >= p.g.n_acc) break;
         const unsigned long long t = __shfl_sync(FULL, v[a], src < 0 ? (int)lane : src);
-        if (src >= 0) v[a] = ia_combine(p.g.acc_kind[a], v[a], t);
+        if (src >= 0) v[a] = acc_merge(p.g.acc_kind[a], v[a], t);
       }
       rest &= ~__ballot_sync(FULL, rank & 1u);
       rank >>= 1;
@@ -195,7 +176,7 @@ __global__ void __launch_bounds__(IA_THREADS) ia_ingest_kernel(const __grid_cons
 #pragma unroll
       for (int a = 1; a < MAX_ACC; ++a) {
         if (a >= p.g.n_acc) break;
-        ia_atomic(p.g.acc_kind[a], p.g.delta + (unsigned long long)a * p.g.cap + id, v[a]);
+        acc_atomic_merge(p.g.acc_kind[a], p.g.delta + (unsigned long long)a * p.g.cap + id, v[a]);
       }
     }
   }
@@ -259,7 +240,7 @@ __global__ void __launch_bounds__(IA_THREADS) ia_final_kernel(const __grid_const
     unsigned long long m[MAX_ACC];
     for (int a = 0; a < p.g.n_acc; ++a) {
       const unsigned long long off = (unsigned long long)a * p.g.cap + id;
-      m[a] = ia_combine(p.g.acc_kind[a], p.g.base[off], p.g.delta[off]);
+      m[a] = acc_merge(p.g.acc_kind[a], p.g.base[off], p.g.delta[off]);
     }
     if (p.keyed) p.o_key[j] = p.g.key[id];
     for (int g = 0; g < p.n_aggs; ++g) p.o_agg[g][j] = agg_finalise(p.agg_kind[g], m[p.agg_acc[g]], m[0]);
@@ -291,19 +272,6 @@ __global__ void ia_state_kernel(const __grid_constant__ IState p) {
     p.o_key[j] = p.g.key[id];
     for (int a = 0; a < p.g.n_acc; ++a) p.o_acc[a][j] = p.g.delta[(unsigned long long)a * p.g.cap + id];
     p.o_ts[j] = (long long)p.inst[j];
-  }
-}
-
-// after a checkpoint has written `delta`: base += delta, delta = identity
-__global__ void ia_fold_kernel(const __grid_constant__ IGroups g, unsigned int n) {
-  unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned int stride = gridDim.x * blockDim.x;
-  for (; i < n; i += stride) {
-    for (int a = 0; a < g.n_acc; ++a) {
-      const unsigned long long off = (unsigned long long)a * g.cap + i;
-      g.base[off] = ia_combine(g.acc_kind[a], g.base[off], g.delta[off]);
-      g.delta[off] = acc_identity(g.acc_kind[a]);
-    }
   }
 }
 
@@ -357,7 +325,7 @@ __global__ void ia_restore_kernel(const __grid_constant__ IRestore p) {
     const uint32_t id = ia_find_or_insert(p.g, p.ts[i], p.keyed ? p.key[i] : 0);
     for (int a = 0; a < p.g.n_acc; ++a) {
       const unsigned long long v = p.state[a] ? p.state[a][i] : 1ull;
-      ia_atomic(a == 0 ? ACC_ROWS : p.g.acc_kind[a], p.g.base + (unsigned long long)a * p.g.cap + id, v);
+      acc_atomic_merge(p.g.acc_kind[a], p.g.base + (unsigned long long)a * p.g.cap + id, v);
     }
   }
 }
@@ -686,15 +654,21 @@ void InstantAggOp::handle_checkpoint(int64_t, BatchesPriv* out) {
   if (g == 0) return;
   const uint64_t d = select(LLONG_MIN);
   if (d > 0) export_state(d, out);
-  ia_fold_kernel<<<grid_for(g), IA_THREADS, 0, stream_>>>(view(cur_), (unsigned int)g);
+  FoldParams fp{};
+  fp.base = cur_.base.as<unsigned long long>();
+  fp.delta = cur_.delta.as<unsigned long long>();
+  fp.cap = cap_;
+  fp.n = (uint32_t)g;
+  fp.n_acc = plan_.n_acc;
+  for (int a = 0; a < plan_.n_acc; ++a) fp.acc_kind[a] = plan_.acc_kind[a];
+  acc_fold_kernel<<<grid_for(g), IA_THREADS, 0, stream_>>>(fp);
   AB_CUDA(cudaGetLastError());
   ++st_.kernel_launches;
   AB_CUDA(cudaStreamSynchronize(stream_));
 }
 
-// Partial-state batches in `partial_schema`: [key?, state cols..., _timestamp = instant] (builder.rs:163-192);
-// COUNT -> count; SUM -> sum; AVG -> (count u64, sum f64); MIN / MAX -> min / max.  One batch per instant: the shim
-// files a batch under its first row's timestamp and expires it by that time.
+// Partial-state batches in `partial_schema` (AggPlan::state_layout), `_timestamp` = instant.  One batch per instant:
+// the shim files a batch under its first row's timestamp and expires it by that time.
 void InstantAggOp::export_state(uint64_t d, BatchesPriv* out) {
   reserve(o_key_, d * 8);
   reserve(o_ts_, d * 8);
@@ -711,45 +685,18 @@ void InstantAggOp::export_state(uint64_t d, BatchesPriv* out) {
   AB_CUDA(cudaGetLastError());
   ++st_.kernel_launches;
   // the columns once, on the host; each instant's rows are then a slice of them
-  struct Col {
-    std::string name, format;
-    const uint64_t* host;
-  };
-  std::vector<Col> cols;
-  std::vector<void*> staged;
-  auto add = [&](const std::string& nm, const std::string& fmt, const DevBuf& dev) {
-    void* h = d2h_pinned(dev.p, (size_t)d * 8, stream_, &st_.d2h_bytes);
-    staged.push_back(h);
-    cols.push_back({nm, fmt, (const uint64_t*)h});
-  };
-  if (plan_.keyed) add("key", key_format_, o_key_);
-  for (int g = 0; g < plan_.n_aggs; ++g) {
-    const std::string base = "agg" + std::to_string(g);
-    const int acc = plan_.agg_acc[g];
-    switch (plan_.agg_kind[g]) {
-      case ARROYO_B200_AGG_COUNT_STAR: add(base + "[count]", "l", o_acc_[0]); break;
-      case ARROYO_B200_AGG_SUM_I64: add(base + "[sum]", "l", o_acc_[acc]); break;
-      case ARROYO_B200_AGG_AVG_I64:
-        add(base + "[count]", "L", o_acc_[0]);
-        add(base + "[sum]", "g", o_acc_[acc]);
-        break;
-      case ARROYO_B200_AGG_MIN_I64: add(base + "[min]", "l", o_acc_[acc]); break;
-      case ARROYO_B200_AGG_MAX_I64: add(base + "[max]", "l", o_acc_[acc]); break;
-    }
-  }
-  add("_timestamp", "tsn:", o_ts_);
+  const std::vector<OutColumn> cols = state_columns(plan_.state_layout(false), (int64_t)d, plan_.keyed ? o_key_.p : nullptr,
+                                                    key_format_, o_acc_, o_ts_.p, stream_, &st_.d2h_bytes);
   AB_CUDA(cudaStreamSynchronize(stream_));
-  const uint64_t* ts = cols.back().host;
+  const uint64_t* ts = (const uint64_t*)cols.back().data;
   for (uint64_t s = 0; s < d;) {
     uint64_t e = s + 1;
     while (e < d && ts[e] == ts[s]) ++e;
     std::vector<OutColumn> oc;
-    for (const Col& c : cols) {
-      OutColumn o;
-      o.name = c.name;
-      o.format = c.format;
+    for (const OutColumn& c : cols) {
+      OutColumn o = c;
       o.data = PinnedPool::get().alloc((size_t)(e - s) * 8);
-      memcpy(o.data, c.host + s, (size_t)(e - s) * 8);
+      memcpy(o.data, (const uint64_t*)c.data + s, (size_t)(e - s) * 8);
       oc.push_back(o);
     }
     out->arrays.emplace_back();
@@ -757,90 +704,34 @@ void InstantAggOp::export_state(uint64_t d, BatchesPriv* out) {
     export_batch(oc, (int64_t)(e - s), &out->arrays.back(), &out->schemas.back());
     s = e;
   }
-  for (void* h : staged) PinnedPool::get().free(h);
+  for (const OutColumn& c : cols) PinnedPool::get().free(c.data);
 }
 
 // on_start (:228-248): partial batches of table "t", in any order and with any number of rows per group, merged into
-// their groups' `base` blocks.  The restored watermark is the late watermark.  Every batch is checked before anything
-// changes; a restore that succeeds takes every batch.
+// their groups' `base` blocks.  The restored watermark is the late watermark.
 void InstantAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t watermark, int64_t) {
   set_device();
-  if (n > 0) AB_REQUIRE(state != nullptr && schemas != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null state batches");
-  // the partial layout: per column after the key, its format and the accumulator it seeds (-1: none)
-  std::vector<std::pair<std::string, int>> layout;
-  for (int g = 0; g < plan_.n_aggs; ++g) {
-    const int acc = plan_.agg_acc[g];
-    switch (plan_.agg_kind[g]) {
-      case ARROYO_B200_AGG_COUNT_STAR: layout.push_back({"l", 0}); break;
-      case ARROYO_B200_AGG_AVG_I64:
-        layout.push_back({"L", 0});
-        layout.push_back({"g", acc});
-        break;
-      default: layout.push_back({"l", acc}); break;
-    }
-  }
-  const int kc = plan_.keyed ? 1 : 0;
-  std::vector<std::vector<InColumn>> batches((size_t)std::max<int64_t>(n, 0));
-  std::vector<int64_t> rows(batches.size(), 0);
-  int64_t total = 0;
-  for (int64_t b = 0; b < n; ++b) {
-    try {
-      batches[b] = import_batch(&state[b], &schemas[b], &rows[b]);
-    } catch (const Error& e) {
-      throw Error(ARROYO_B200_INVALID_ARGUMENT, std::string("state batch: ") + e.what());
-    }
-    const std::vector<InColumn>& cols = batches[b];
-    AB_REQUIRE(cols.size() == (size_t)kc + layout.size() + 1, ARROYO_B200_INVALID_ARGUMENT,
-               "state batch does not match the partial schema");
-    if (plan_.keyed) {
-      const std::string& f = cols[0].format;
-      AB_REQUIRE(f == "l" || f == "L" || f.compare(0, 4, "tsn:") == 0, ARROYO_B200_INVALID_ARGUMENT,
-                 "state batch: key of type '" + f + "' (supported: l, L, tsn:)");
-    }
-    for (size_t j = 0; j < layout.size(); ++j)
-      AB_REQUIRE(cols[kc + j].format == layout[j].first, ARROYO_B200_INVALID_ARGUMENT,
-                 "state batch: column " + std::to_string(kc + j) + " has type '" + cols[kc + j].format +
-                     "', the partial schema has '" + layout[j].first + "'");
-    AB_REQUIRE(cols.back().format.compare(0, 4, "tsn:") == 0, ARROYO_B200_INVALID_ARGUMENT,
-               "state batch: the last column is not the _timestamp");
-    total += rows[b];
-  }
+  const StateBatches sb(plan_, false, state, schemas, n);
   if (watermark != INT64_MIN) late_wm_ = std::max<int64_t>(late_wm_, watermark);
-  if (total > 0) {
-    if (plan_.keyed) key_format_ = batches[0][0].format;
-    // the columns of every batch, concatenated in batch order
-    std::vector<DevBuf> keep;
-    auto upload = [&](int c) {
-      DevBuf& dst = keep.emplace_back((size_t)total * 8);
-      int64_t off = 0;
-      for (int64_t b = 0; b < n; ++b) {
-        if (rows[b])
-          AB_CUDA(cudaMemcpyAsync((char*)dst.p + off * 8, batches[b][c].data, (size_t)rows[b] * 8, cudaMemcpyHostToDevice,
-                                  stream_));
-        off += rows[b];
-      }
-      st_.h2d_bytes += (uint64_t)total * 8;
-      return dst.p;
-    };
-    reserve_groups((uint64_t)total);
+  if (sb.total > 0) {
+    if (plan_.keyed) key_format_ = sb.cols[0][0].format;
+    reserve_groups((uint64_t)sb.total);
+    DevBuf d_key, d_ts, d_acc[MAX_ACC];
     IRestore p{};
-    p.keyed = kc;
-    p.key = plan_.keyed ? (const long long*)upload(0) : nullptr;
-    p.ts = (const long long*)upload(kc + (int)layout.size());
-    for (size_t j = 0; j < layout.size(); ++j) {
-      const int acc = layout[j].second;
-      if (!p.state[acc]) p.state[acc] = (const unsigned long long*)upload(kc + (int)j);
-    }
-    p.n = total;
+    p.keyed = plan_.keyed ? 1 : 0;
+    p.key = plan_.keyed ? (const long long*)sb.upload(0, 0, n, d_key, stream_, &st_.h2d_bytes) : nullptr;
+    p.ts = (const long long*)sb.upload(sb.ts_col, 0, n, d_ts, stream_, &st_.h2d_bytes);
+    for (int a = 0; a < plan_.n_acc; ++a)
+      if (sb.seed[a] >= 0) p.state[a] = sb.upload(sb.seed[a], 0, n, d_acc[a], stream_, &st_.h2d_bytes);
+    p.n = sb.total;
     p.g = view(cur_);
-    ia_restore_kernel<<<grid_for((uint64_t)total), IA_THREADS, 0, stream_>>>(p);
+    ia_restore_kernel<<<grid_for((uint64_t)sb.total), IA_THREADS, 0, stream_>>>(p);
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
-    groups_hi_ += (uint64_t)total;
+    groups_hi_ += (uint64_t)sb.total;
     read_counters();
   }
-  for (int64_t b = 0; b < n; ++b)
-    if (state[b].release) state[b].release(&state[b]);
+  take_batches(state, n);
 }
 
 }  // namespace

@@ -454,16 +454,6 @@ class UpdatingAggOp final : public OpBase {
   DevBuf last_, ttl_counters_;
   uint64_t tombstones_ = 0, min_buckets_ = 1;
 
-  // One column of table "a" after the key: its Arrow format and what it holds.
-  enum StateRole { S_ROWS, S_ACC, S_TS, S_GEN };
-  struct StateCol {
-    const char* format;
-    int role;
-    int acc;         // S_ACC: the accumulator
-    bool count_star;  // S_ROWS: the COUNT(*) aggregate's own column
-  };
-  std::vector<StateCol> state_layout() const;
-
   UState state_view() const;
   void alloc_state();
   void grow();
@@ -858,32 +848,6 @@ void UpdatingAggOp::launch_expire(unsigned int n) {
 }
 
 
-// Table "a" after the key column (sliding_state_schema, :1083-1160): per aggregate in plan order the state of its
-// sliding accumulator -- count(*) [count: Int64], sum [sum: Int64, count: UInt64], avg [count: UInt64, sum: Float64],
-// min [min: Int64], max [max: Int64] -- then the trailing max(_timestamp) aggregate's state as `_timestamp` and the
-// generation.  Every count column holds the key's row count.
-std::vector<UpdatingAggOp::StateCol> UpdatingAggOp::state_layout() const {
-  std::vector<StateCol> l;
-  for (int g = 0; g < plan_.n_aggs; ++g) {
-    const int acc = plan_.agg_acc[g];
-    switch (plan_.agg_kind[g]) {
-      case ARROYO_B200_AGG_COUNT_STAR: l.push_back({"l", S_ROWS, 0, true}); break;
-      case ARROYO_B200_AGG_SUM_I64:
-        l.push_back({"l", S_ACC, acc, false});
-        l.push_back({"L", S_ROWS, 0, false});
-        break;
-      case ARROYO_B200_AGG_AVG_I64:
-        l.push_back({"L", S_ROWS, 0, false});
-        l.push_back({"g", S_ACC, acc, false});
-        break;
-      default: l.push_back({"l", S_ACC, acc, false}); break;  // min / max
-    }
-  }
-  l.push_back({"tsn:", S_TS, 0, false});
-  l.push_back({"L", S_GEN, 0, false});
-  return l;
-}
-
 // checkpoint_sliding (:272-340): one batch of table "a" with the keys flushed since the last call, or nothing.
 void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
   set_device();
@@ -924,40 +888,15 @@ void UpdatingAggOp::checkpoint_state(BatchesPriv* out) {
   if (dead) maybe_compact(read_live());
 }
 
-// The table-"a" batch of the `rows` rows the export kernel wrote; with `dead`, the rows it marked are tombstones: a
-// null `_timestamp`.
+// The table-"a" batch (AggPlan::state_layout) of the `rows` rows the export kernel wrote; with `dead`, the rows it
+// marked are tombstones: a null `_timestamp`.
 void UpdatingAggOp::export_state(BatchesPriv* out, unsigned int rows, bool dead) {
-  std::vector<OutColumn> cols;
-  auto column = [&](const std::string& name, const std::string& format, const void* dev) {
-    OutColumn c;
-    c.name = name;
-    c.format = format;
-    c.data = d2h_pinned(dev, (size_t)rows * 8, stream_, &st_.d2h_bytes);
-    cols.push_back(c);
-  };
-  if (plan_.keyed) column("key", key_format_, s_key_.p);
-  const std::vector<StateCol> layout = state_layout();
-  for (size_t j = 0; j < layout.size(); ++j) {
-    const StateCol& sc = layout[j];
-    const std::string name = "state" + std::to_string(j);
-    if (sc.role == S_GEN) {
-      OutColumn c;
-      c.name = "_generation";
-      c.format = sc.format;
-      uint64_t* g = (uint64_t*)PinnedPool::get().alloc((size_t)rows * 8);
-      std::fill(g, g + rows, (uint64_t)generation_);
-      c.data = g;
-      cols.push_back(c);
-    } else if (sc.role == S_TS) {
-      column("_timestamp", sc.format, s_ts_.p);
-    } else {
-      column(name, sc.format, s_acc_[sc.role == S_ROWS ? 0 : sc.acc].p);
-    }
-  }
+  std::vector<OutColumn> cols = state_columns(plan_.state_layout(true), rows, plan_.keyed ? s_key_.p : nullptr,
+                                              key_format_, s_acc_, s_ts_.p, stream_, &st_.d2h_bytes);
   const unsigned char* is_dead = dead ? (const unsigned char*)d2h_pinned(s_dead_.p, rows, stream_, &st_.d2h_bytes) : nullptr;
   AB_CUDA(cudaStreamSynchronize(stream_));
   if (is_dead) {
-    OutColumn& ts = cols[(plan_.keyed ? 1 : 0) + layout.size() - 2];
+    OutColumn& ts = cols.back();
     uint8_t* valid = (uint8_t*)PinnedPool::get().alloc((size_t)rows / 8 + 8);
     memset(valid, 0, (size_t)rows / 8 + 8);
     for (unsigned int r = 0; r < rows; ++r) {
@@ -969,6 +908,12 @@ void UpdatingAggOp::export_state(BatchesPriv* out, unsigned int rows, bool dead)
     if (ts.null_count) ts.validity = valid;
     else PinnedPool::get().free(valid);
   }
+  OutColumn g;
+  g.name = "_generation";
+  g.format = "L";
+  g.data = PinnedPool::get().alloc((size_t)rows * 8);
+  std::fill((uint64_t*)g.data, (uint64_t*)g.data + rows, (uint64_t)generation_);
+  cols.push_back(g);
   ++generation_;
   out->arrays.emplace_back();
   out->schemas.emplace_back();
@@ -979,61 +924,18 @@ void UpdatingAggOp::export_state(BatchesPriv* out, unsigned int rows, bool dead)
 // succeeds takes every batch once the copies have completed.
 void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t, int64_t) {
   if (n <= 0) return;
-  AB_REQUIRE(state != nullptr && schemas != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null state batches");
+  const StateBatches sb(plan_, true, state, schemas, n);
   AB_REQUIRE(st_.rows_in == 0 && !restored_, ARROYO_B200_INVALID_ARGUMENT,
              "updating aggregate: restore into an operator that already holds rows or restored state");
-  // every batch is checked before anything changes
-  const std::vector<StateCol> layout = state_layout();
-  const int kc = plan_.keyed ? 1 : 0;
-  std::vector<std::vector<InColumn>> batches((size_t)n);
-  std::vector<int64_t> rows((size_t)n, 0);
-  int64_t total = 0;
-  for (int64_t b = 0; b < n; ++b) {
-    try {  // `_timestamp` may be null: a tombstone
-      batches[b] = import_batch(&state[b], &schemas[b], &rows[b], kc + (int64_t)layout.size() - 2);
-    } catch (const Error& e) {
-      throw Error(ARROYO_B200_INVALID_ARGUMENT, std::string("state batch: ") + e.what());
-    }
-    const std::vector<InColumn>& cols = batches[b];
-    AB_REQUIRE(cols.size() == (size_t)kc + layout.size(), ARROYO_B200_INVALID_ARGUMENT,
-               "state batch does not have the columns of table 'a' for this plan");
-    if (plan_.keyed) {
-      const std::string& f = cols[0].format;
-      AB_REQUIRE(f == "l" || f == "L" || f.compare(0, 4, "tsn:") == 0, ARROYO_B200_INVALID_ARGUMENT,
-                 "state batch: key of type '" + f + "' (supported: l, L, tsn:)");
-    }
-    for (size_t j = 0; j < layout.size(); ++j) {
-      const std::string& f = cols[kc + j].format;
-      const std::string want = layout[j].format;
-      const bool ok = want == "tsn:" ? f.compare(0, 4, "tsn:") == 0 : f == want;
-      AB_REQUIRE(ok, ARROYO_B200_INVALID_ARGUMENT,
-                 "state batch: column " + std::to_string(kc + j) + " has type '" + f + "', table 'a' has '" + want + "'");
-    }
-    total += rows[b];
-  }
-  auto take_all = [&]() {
-    for (int64_t b = 0; b < n; ++b)
-      if (state[b].release) state[b].release(&state[b]);
-  };
+  const int64_t total = sb.total;
   if (total == 0) {
-    take_all();
+    take_batches(state, n);
     return;
   }
-  // which column seeds each accumulator: the row count from COUNT(*), else from a SUM's or AVG's count, else 1
-  int rows_col = -1, ts_col = -1, gen_col = -1, acc_col[MAX_ACC];
-  for (int a = 0; a < MAX_ACC; ++a) acc_col[a] = -1;
-  for (size_t j = 0; j < layout.size(); ++j) {
-    const StateCol& sc = layout[j];
-    const int c = kc + (int)j;
-    if (sc.role == S_ROWS && (rows_col < 0 || (sc.count_star && !layout[rows_col - kc].count_star))) rows_col = c;
-    if (sc.role == S_ACC && acc_col[sc.acc] < 0) acc_col[sc.acc] = c;
-    if (sc.role == S_TS) ts_col = c;
-    if (sc.role == S_GEN) gen_col = c;
-  }
-  acc_col[0] = rows_col;
+  const int ts_col = sb.ts_col, gen_col = sb.ts_col + 1;
   set_device();
   if (plan_.keyed) {
-    key_format_ = batches[0][0].format;
+    key_format_ = sb.cols[0][0].format;
     // the state is still empty: size the dictionary once to hold every restored key without growing
     const uint64_t b = bd_buckets_for((uint64_t)total);
     if (b > dict_.n_buckets()) {
@@ -1041,45 +943,30 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
       alloc_state();
     }
   }
-  // the columns of every batch, concatenated in batch order: a row's position is its index
-  auto upload = [&](int c, DevBuf& dst) {
-    dst.alloc((size_t)total * 8);
-    int64_t off = 0;
-    for (int64_t b = 0; b < n; ++b) {
-      if (rows[b])
-        AB_CUDA(cudaMemcpyAsync((char*)dst.p + off * 8, batches[b][c].data, (size_t)rows[b] * 8, cudaMemcpyHostToDevice,
-                                stream_));
-      off += rows[b];
-    }
-    st_.h2d_bytes += (uint64_t)total * 8;
-  };
   DevBuf d_key, d_gen, d_ts, d_val[MAX_ACC];
-  if (plan_.keyed) upload(0, d_key);
-  upload(gen_col, d_gen);
-  upload(ts_col, d_ts);
+  if (plan_.keyed) sb.upload(0, 0, n, d_key, stream_, &st_.h2d_bytes);
+  sb.upload(gen_col, 0, n, d_gen, stream_, &st_.h2d_bytes);
+  sb.upload(ts_col, 0, n, d_ts, stream_, &st_.h2d_bytes);
   URestore p{};
-  for (int a = 0; a < plan_.n_acc; ++a) {
-    if (acc_col[a] < 0) continue;
-    upload(acc_col[a], d_val[a]);
-    p.val[a] = d_val[a].as<unsigned long long>();
-  }
+  for (int a = 0; a < plan_.n_acc; ++a)
+    if (sb.seed[a] >= 0) p.val[a] = sb.upload(sb.seed[a], 0, n, d_val[a], stream_, &st_.h2d_bytes);
   uint64_t max_gen = 0;
   for (int64_t b = 0; b < n; ++b)
-    for (int64_t i = 0; i < rows[b]; ++i) max_gen = std::max<uint64_t>(max_gen, batches[b][gen_col].data[i]);
+    for (int64_t i = 0; i < sb.rows[b]; ++i) max_gen = std::max<uint64_t>(max_gen, sb.cols[b][gen_col].data[i]);
   // tombstones: the rows whose `_timestamp` is null
   DevBuf d_dead;
   bool any_dead = false;
-  for (int64_t b = 0; b < n; ++b) any_dead = any_dead || batches[b][ts_col].validity != nullptr;
+  for (int64_t b = 0; b < n; ++b) any_dead = any_dead || sb.cols[b][ts_col].validity != nullptr;
   if (any_dead) {
     std::vector<unsigned char> h_dead((size_t)total, 0);
     int64_t off = 0;
     for (int64_t b = 0; b < n; ++b) {
-      const InColumn& c = batches[b][ts_col];
-      for (int64_t i = 0; c.validity && i < rows[b]; ++i) {
+      const InColumn& c = sb.cols[b][ts_col];
+      for (int64_t i = 0; c.validity && i < sb.rows[b]; ++i) {
         const int64_t bit = c.validity_bit + i;
         h_dead[off + i] = !((c.validity[bit >> 3] >> (bit & 7)) & 1);
       }
-      off += rows[b];
+      off += sb.rows[b];
     }
     d_dead.alloc((size_t)total);
     AB_CUDA(cudaMemcpyAsync(d_dead.p, h_dead.data(), (size_t)total, cudaMemcpyHostToDevice, stream_));
@@ -1125,7 +1012,7 @@ void UpdatingAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n,
   if (h_won[1] && plan_.keyed) compact();
   generation_ = max_gen + 1;
   restored_ = true;
-  take_all();
+  take_batches(state, n);
 }
 
 }  // namespace

@@ -530,7 +530,7 @@ __global__ void __launch_bounds__(THREADS, AB_INGEST_MIN_BLOCKS) ingest_kernel(c
 // sliding_aggregating_window.rs:725-733) into one pane block, by the ids BucketDict::place gave its keys.
 struct PartialParams {
   const uint32_t* ids;
-  const unsigned long long* state[MAX_ACC];  // state[0] = rows
+  const unsigned long long* state[MAX_ACC];  // state[0] = rows; null: each row counts one
   long long n;
   int n_acc;
   int acc_kind[MAX_ACC];
@@ -543,25 +543,8 @@ __global__ void ingest_partial_kernel(const __grid_constant__ PartialParams p) {
   long long stride = (long long)gridDim.x * blockDim.x;
   for (; i < p.n; i += stride) {
     const uint32_t id = p.ids[i];
-    for (int a = 0; a < p.n_acc; ++a) {
-      unsigned long long* dst = p.pane + (unsigned long long)a * p.id_cap + id;
-      unsigned long long v = p.state[a][i];
-      switch (p.acc_kind[a]) {
-        case ACC_ROWS:
-        case ACC_SUM_I64:
-          atomicAdd(dst, v);
-          break;
-        case ACC_SUM_F64:
-          atomicAdd(reinterpret_cast<double*>(dst), __longlong_as_double((long long)v));
-          break;
-        case ACC_MIN_I64:
-          atomicMin(reinterpret_cast<long long*>(dst), (long long)v);
-          break;
-        case ACC_MAX_I64:
-          atomicMax(reinterpret_cast<long long*>(dst), (long long)v);
-          break;
-      }
-    }
+    for (int a = 0; a < p.n_acc; ++a)
+      acc_atomic_merge(p.acc_kind[a], p.pane + (unsigned long long)a * p.id_cap + id, p.state[a] ? p.state[a][i] : 1ull);
   }
 }
 
@@ -603,15 +586,6 @@ struct EmitParams {
 
 constexpr int EMIT_THREADS = 256;
 
-__device__ __forceinline__ unsigned long long merge_acc(int kind, unsigned long long a, unsigned long long v) {
-  switch (kind) {
-    case ACC_SUM_F64:
-      return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) + __longlong_as_double((long long)v));
-    case ACC_MIN_I64: return (unsigned long long)min((long long)a, (long long)v);
-    case ACC_MAX_I64: return (unsigned long long)max((long long)a, (long long)v);
-    default: return a + v;  // ACC_ROWS, ACC_SUM_I64 (wrapping)
-  }
-}
 __device__ __forceinline__ unsigned long long unmerge_acc(int kind, unsigned long long a, unsigned long long v) {
   if (kind == ACC_SUM_F64)
     return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) - __longlong_as_double((long long)v));
@@ -685,8 +659,8 @@ __global__ void __launch_bounds__(EMIT_THREADS) emit_kernel(const __grid_constan
             {
               const ulonglong2 v = __ldcs(reinterpret_cast<const ulonglong2*>(pane + (unsigned long long)a * p.id_cap + id));
               const int kind = p.acc_kind[a];
-              acc0[a] = add ? merge_acc(kind, acc0[a], v.x) : unmerge_acc(kind, acc0[a], v.x);
-              acc1[a] = add ? merge_acc(kind, acc1[a], v.y) : unmerge_acc(kind, acc1[a], v.y);
+              acc0[a] = add ? acc_merge(kind, acc0[a], v.x) : unmerge_acc(kind, acc0[a], v.x);
+              acc1[a] = add ? acc_merge(kind, acc1[a], v.y) : unmerge_acc(kind, acc1[a], v.y);
             }
         }
         // a key that left the window restarts from exactly zero (no f64 drift carried over)
@@ -713,8 +687,8 @@ __global__ void __launch_bounds__(EMIT_THREADS) emit_kernel(const __grid_constan
             {
               const ulonglong2 v = __ldcs(reinterpret_cast<const ulonglong2*>(pane + (unsigned long long)a * p.id_cap + id));
               const int kind = p.acc_kind[a];
-              acc0[a] = merge_acc(kind, acc0[a], v.x);
-              acc1[a] = merge_acc(kind, acc1[a], v.y);
+              acc0[a] = acc_merge(kind, acc0[a], v.x);
+              acc1[a] = acc_merge(kind, acc1[a], v.y);
             }
         }
       }
@@ -740,47 +714,6 @@ __global__ void __launch_bounds__(EMIT_THREADS) emit_kernel(const __grid_constan
     if (v0) emit_row<NACC>(p, o0, acc0, (long long)keys.x);
     if (v1) emit_row<NACC>(p, o0 + (v0 ? 1u : 0u), acc1, (long long)keys.y);
     __syncthreads();
-  }
-}
-
-// checkpoint fold: frozen += active; active = identity  (see Pane::frozen)
-struct FoldParams {
-  unsigned long long* active;
-  unsigned long long* frozen;
-  unsigned long long id_cap;
-  uint32_t n_ids;
-  int n_acc;
-  int acc_kind[MAX_ACC];
-};
-__global__ void fold_kernel(const __grid_constant__ FoldParams p) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t stride = gridDim.x * blockDim.x;
-  for (; i < p.n_ids; i += stride) {
-    for (int a = 0; a < p.n_acc; ++a) {
-      unsigned long long* fa = p.frozen + (unsigned long long)a * p.id_cap + i;
-      unsigned long long* aa = p.active + (unsigned long long)a * p.id_cap + i;
-      unsigned long long f = *fa, v = *aa, ident = 0;
-      switch (p.acc_kind[a]) {
-        case ACC_ROWS:
-        case ACC_SUM_I64:
-          f += v;
-          break;
-        case ACC_SUM_F64:
-          f = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)f) +
-                                                       __longlong_as_double((long long)v));
-          break;
-        case ACC_MIN_I64:
-          f = (unsigned long long)min((long long)f, (long long)v);
-          ident = (unsigned long long)LLONG_MAX;
-          break;
-        case ACC_MAX_I64:
-          f = (unsigned long long)max((long long)f, (long long)v);
-          ident = (unsigned long long)LLONG_MIN;
-          break;
-      }
-      *fa = f;
-      *aa = ident;
-    }
   }
 }
 
@@ -2191,47 +2124,17 @@ void WindowAggOp::export_window(OutSet* os, int64_t n, BatchesPriv* out_host) {
   if (!async_out_) AB_CUDA(cudaStreamSynchronize(stream_));
 }
 
-// Partial-state batch in `partial_schema`: [key?, state cols..., _timestamp = pane start]
-// (arroyo-planner/src/builder.rs:163-192).  COUNT -> count; SUM -> sum; AVG -> (count u64, sum f64).
+// Partial-state batch in `partial_schema` (AggPlan::state_layout), `_timestamp` = pane start.
 void WindowAggOp::export_partial(OutSet* os, int64_t n, BatchesPriv* out) {
-  std::vector<OutColumn> cols;
-  std::vector<size_t> fix_f64;  // AVG state kept as an exact integer sum: the partial schema wants Float64
-  if (plan_.keyed) {
-    OutColumn k;
-    k.name = "key";
-    k.format = key_format_;
-    k.data = d2h_pinned(os->key.p, (size_t)n * 8, stream_, &st_.d2h_bytes);
-    cols.push_back(k);
-  }
-  for (int g = 0; g < plan_.n_aggs; ++g) {
-    auto add = [&](const char* nm, const char* fmt, const void* dev) {
-      OutColumn c;
-      c.name = std::string("agg") + std::to_string(g) + nm;
-      c.format = fmt;
-      c.data = d2h_pinned(dev, (size_t)n * 8, stream_, &st_.d2h_bytes);
-      cols.push_back(c);
-    };
-    switch (plan_.agg_kind[g]) {
-      case ARROYO_B200_AGG_COUNT_STAR: add("[count]", "l", os->state[0].p); break;
-      case ARROYO_B200_AGG_SUM_I64: add("[sum]", "l", os->state[plan_.agg_acc[g]].p); break;
-      case ARROYO_B200_AGG_AVG_I64:
-        add("[count]", "L", os->state[0].p);
-        add("[sum]", "g", os->state[plan_.agg_acc[g]].p);
-        if (plan_.acc_kind[plan_.agg_acc[g]] == ACC_SUM_I64) fix_f64.push_back(cols.size() - 1);
-        break;
-      case ARROYO_B200_AGG_MIN_I64: add("[min]", plan_.agg_format[g].c_str(), os->state[plan_.agg_acc[g]].p); break;
-      case ARROYO_B200_AGG_MAX_I64: add("[max]", plan_.agg_format[g].c_str(), os->state[plan_.agg_acc[g]].p); break;
-    }
-  }
-  OutColumn t;
-  t.name = "_timestamp";
-  t.format = "tsn:";
-  t.data = d2h_pinned(os->ts.p, (size_t)n * 8, stream_, &st_.d2h_bytes);
-  cols.push_back(t);
+  const std::vector<StateCol> layout = plan_.state_layout(false);
+  std::vector<OutColumn> cols = state_columns(layout, n, plan_.keyed ? os->key.p : nullptr, key_format_, os->state,
+                                              os->ts.p, stream_, &st_.d2h_bytes);
   AB_CUDA(cudaStreamSynchronize(stream_));
-  for (size_t ci : fix_f64) {
-    long long* raw = (long long*)cols[ci].data;
-    double* d = (double*)cols[ci].data;
+  // AVG state kept as an exact integer sum: the partial schema wants Float64
+  for (size_t j = 0; j < layout.size(); ++j) {
+    if (layout[j].role != S_ACC || plan_.acc_kind[layout[j].acc] != ACC_SUM_I64 || strcmp(layout[j].format, "g")) continue;
+    long long* raw = (long long*)cols[(plan_.keyed ? 1 : 0) + j].data;
+    double* d = (double*)raw;
     for (int64_t i = 0; i < n; ++i) d[i] = (double)raw[i];
   }
   out->arrays.emplace_back();
@@ -2502,14 +2405,14 @@ void WindowAggOp::handle_checkpoint(int64_t wm, BatchesPriv* out) {
     p.delta_exported = true;
     if (!p.frozen) p.frozen = acquire_block();
     FoldParams fp{};
-    fp.active = p.dev;
-    fp.frozen = p.frozen;
-    fp.id_cap = dict_.id_cap();
-    fp.n_ids = dict_.n_ids();
+    fp.base = p.frozen;
+    fp.delta = p.dev;
+    fp.cap = dict_.id_cap();
+    fp.n = dict_.n_ids();
     fp.n_acc = plan_.n_acc;
     for (int a = 0; a < plan_.n_acc; ++a) fp.acc_kind[a] = plan_.acc_kind[a];
     int grid = (int)std::min<uint32_t>((dict_.n_ids() + 255) / 256, (uint32_t)num_sms_ * 8);
-    fold_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(fp);
+    acc_fold_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(fp);
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
   }
@@ -2532,28 +2435,20 @@ void WindowAggOp::handle_checkpoint(int64_t wm, BatchesPriv* out) {
   collect_emit_times();
 }
 
-// Restore (tumbling :228-248, sliding :556-595): partial batches go back into pane blocks.
+// Restore (tumbling :228-248, sliding :556-595): partial batches go back into pane blocks, one batch at a time (a
+// batch holds one pane), once every batch has been checked.
 void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t watermark, int64_t table_min) {
   set_device();
+  const StateBatches sb(plan_, false, state, schemas, n);
   const bool has_wm = watermark != INT64_MIN;
   if (has_wm) late_bin_ = std::max<int64_t>(late_bin_, bin_start(watermark, slide_));
   if (sliding_) sliding_planner_->restore_begin(has_wm, watermark);
-  // expected partial layout
-  int n_state_cols = 0;
-  for (int g = 0; g < plan_.n_aggs; ++g) n_state_cols += plan_.agg_kind[g] == ARROYO_B200_AGG_AVG_I64 ? 2 : 1;
-  const int expect_cols = (plan_.keyed ? 1 : 0) + n_state_cols + 1;
-  std::vector<DevBuf> keep;
   for (int64_t bi = 0; bi < n; ++bi) {
-    int64_t rows = 0;
-    std::vector<InColumn> cols = import_batch(&state[bi], &schemas[bi], &rows);
-    AB_REQUIRE((int)cols.size() == expect_cols, ARROYO_B200_INVALID_ARGUMENT,
-               "state batch does not match the partial schema");
-    if (rows == 0) {
-      if (state[bi].release) state[bi].release(&state[bi]);
-      continue;
-    }
+    const int64_t rows = sb.rows[bi];
+    if (rows == 0) continue;
+    const std::vector<InColumn>& cols = sb.cols[bi];
     if (plan_.keyed) key_format_ = cols[0].format;
-    const int64_t ts = (int64_t)cols.back().data[0];
+    const int64_t ts = (int64_t)cols[sb.ts_col].data[0];
     const int64_t bin = bin_start(ts, slide_);
     ensure_pane(bin);
     Pane& p = panes_.at(bin);
@@ -2569,58 +2464,26 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
     pp.n = rows;
     pp.n_acc = plan_.n_acc;
     for (int a = 0; a < plan_.n_acc; ++a) pp.acc_kind[a] = plan_.acc_kind[a];
-    auto up = [&](const uint64_t* h) -> const unsigned long long* {
-      keep.emplace_back((size_t)rows * 8);
-      AB_CUDA(cudaMemcpyAsync(keep.back().p, h, (size_t)rows * 8, cudaMemcpyHostToDevice, stream_));
-      return keep.back().as<unsigned long long>();
-    };
-    int ci = 0;
-    const long long* keys = plan_.keyed ? (const long long*)up(cols[ci++].data) : nullptr;
-    for (int a = 0; a < MAX_ACC; ++a) pp.state[a] = nullptr;
-    std::vector<std::pair<int, int>> avg_sum_cols;  // (agg, column of its f64 sum)
-    for (int g = 0; g < plan_.n_aggs; ++g) {
-      switch (plan_.agg_kind[g]) {
-        case ARROYO_B200_AGG_COUNT_STAR: {
-          const unsigned long long* c = up(cols[ci++].data);
-          if (!pp.state[0]) pp.state[0] = c;
-          break;
-        }
-        case ARROYO_B200_AGG_AVG_I64: {
-          const unsigned long long* c = up(cols[ci++].data);
-          if (!pp.state[0]) pp.state[0] = c;
-          avg_sum_cols.emplace_back(g, ci++);
-          break;
-        }
-        default:
-          pp.state[plan_.agg_acc[g]] = up(cols[ci++].data);
-          break;
-      }
-    }
-    std::vector<long long> conv;
-    for (auto& pr : avg_sum_cols) {
-      const int acc = plan_.agg_acc[pr.first];
-      if (plan_.acc_kind[acc] == ACC_SUM_F64) {
-        pp.state[acc] = up(cols[pr.second].data);
-      } else if (!pp.state[acc]) {
+    DevBuf d_key, d_acc[MAX_ACC];
+    std::vector<long long> conv[MAX_ACC];
+    const long long* keys =
+        plan_.keyed ? (const long long*)sb.upload(0, bi, bi + 1, d_key, stream_, &st_.h2d_bytes) : nullptr;
+    for (int a = 0; a < plan_.n_acc; ++a) {
+      const int c = sb.seed[a];
+      if (c < 0) continue;
+      if (plan_.acc_kind[a] == ACC_SUM_I64 && !strcmp(sb.layout[c - sb.kc].format, "g")) {
         // exact-sum AVG without a SUM over the same column: the checkpoint only has the f64 image of the sum
-        // (exact below 2^53); a SUM column, when present, already restored the integer accumulator above
-        conv.resize((size_t)rows);
-        const double* d = (const double*)cols[pr.second].data;
-        for (int64_t i = 0; i < rows; ++i) conv[(size_t)i] = (long long)__builtin_llround(d[i]);
-        keep.emplace_back((size_t)rows * 8);
-        AB_CUDA(cudaMemcpyAsync(keep.back().p, conv.data(), (size_t)rows * 8, cudaMemcpyHostToDevice, stream_));
-        AB_CUDA(cudaStreamSynchronize(stream_));
-        pp.state[acc] = keep.back().as<unsigned long long>();
+        // (exact below 2^53)
+        conv[a].resize((size_t)rows);
+        const double* d = (const double*)cols[c].data;
+        for (int64_t i = 0; i < rows; ++i) conv[a][(size_t)i] = (long long)__builtin_llround(d[i]);
+        d_acc[a].alloc((size_t)rows * 8);
+        AB_CUDA(cudaMemcpyAsync(d_acc[a].p, conv[a].data(), (size_t)rows * 8, cudaMemcpyHostToDevice, stream_));
+        st_.h2d_bytes += (uint64_t)rows * 8;
+        pp.state[a] = d_acc[a].as<unsigned long long>();
+      } else {
+        pp.state[a] = sb.upload(c, bi, bi + 1, d_acc[a], stream_, &st_.h2d_bytes);
       }
-    }
-    if (pp.state[0] == nullptr) {
-      // SUM / MIN / MAX-only plans carry no row count in their partial state; the rows accumulator is only the
-      // "this key is present in the pane" flag for them, so every restored state row counts as one
-      std::vector<unsigned long long> ones((size_t)rows, 1ull);
-      keep.emplace_back((size_t)rows * 8);
-      AB_CUDA(cudaMemcpyAsync(keep.back().p, ones.data(), (size_t)rows * 8, cudaMemcpyHostToDevice, stream_));
-      AB_CUDA(cudaStreamSynchronize(stream_));
-      pp.state[0] = keep.back().as<unsigned long long>();
     }
     // room for every key of the batch at the target bucket fill (most of them are usually known already)
     while (plan_.keyed && (uint64_t)total_keys_host_ + (uint64_t)rows > dict_.n_buckets() * (uint64_t)BD_MEAN) {
@@ -2628,25 +2491,26 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
       grow_ids();
     }
     // every key gets its id before anything is merged (a bucket out of ids grows the dictionary), then merge by id
-    uint32_t* ids = keep.emplace_back((size_t)rows * sizeof(uint32_t)).as<uint32_t>();
-    dict_.place(keys, rows, ids, [&] { grow_ids(); });
-    pp.ids = ids;
+    DevBuf ids((size_t)rows * sizeof(uint32_t));
+    dict_.place(keys, rows, ids.as<uint32_t>(), [&] { grow_ids(); });
+    pp.ids = ids.as<uint32_t>();
     pp.pane = panes_.at(bin).frozen;
     pp.id_cap = dict_.id_cap();
     int grid = (int)std::min<int64_t>((rows + 255) / 256, (int64_t)num_sms_ * 8);
     ingest_partial_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(pp);
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
+    // the batch's device copies and `conv` are done with once the stream has passed this read
     Counters c{};
     AB_CUDA(cudaMemcpyAsync(&c, book_.p, sizeof c, cudaMemcpyDeviceToHost, stream_));
     AB_CUDA(cudaStreamSynchronize(stream_));
     total_keys_host_ = c.n_keys;
     last_counters_ = c;
     max_bin_seen_ = std::max<int64_t>(max_bin_seen_, bin);
-    if (state[bi].release) state[bi].release(&state[bi]);
   }
   if (sliding_) sliding_planner_->restore_end(table_min != INT64_MIN, table_min);
   AB_CUDA(cudaStreamSynchronize(stream_));
+  take_batches(state, n);
 }
 
 void WindowAggOp::stats(ArroyoB200Stats* out) {

@@ -294,14 +294,17 @@ const char* arroyo_b200_op_name(const ArroyoB200Op* op);
  * batch by releasing it, which sets its `release` to NULL; a successful restore takes every array.
  * Whatever still has a non-null `release` after the call, successful or not, belongs to the caller,
  * and so do the schemas.
+ * Window, instant and updating aggregates: a batch whose column count, column types or key type
+ * (l, L or tsn:) is not the plan's layout of the table => ARROYO_B200_INVALID_ARGUMENT, with nothing
+ * changed and every batch left to the caller.
  * Updating aggregate (incremental_aggregator.rs:446-503): `state` holds every batch of table "a"
  * (UncachedKeyValueView::get_all, in any order, not de-duplicated), in the layout
  * arroyo_b200_op_checkpoint_state writes; both time arguments are ignored.  Per key the row with the
  * largest `_generation` wins, a tie going to the later row (batch order, then row order); it seeds the
  * accumulators and the values the next flush retracts.  The dictionary is sized from the row count and
  * grows when a bucket runs out of ids; keys that still cannot be placed => ARROYO_B200_RUNTIME.
- * ARROYO_B200_INVALID_ARGUMENT, with nothing changed: a column count or type that is not the plan's
- * layout, or an operator that has already taken rows or been restored.  Restored rows do not count in
+ * ARROYO_B200_INVALID_ARGUMENT, with nothing changed: an operator that has already taken rows or been
+ * restored.  Restored rows do not count in
  * `rows_in`; their keys count in `n_keys`.
  * A null `_timestamp` (and only there) marks a tombstone: when it wins, its key stays absent (see
  * arroyo_b200_op_set_clock).  With a ttl, restored keys are stamped with the clock at this call.

@@ -68,6 +68,9 @@ def _new(kind):
         cfg = O.WindowAggConfig(width=4 * S, slide=S if kind == "sliding" else 0, key_names=["key"], aggs=AGGS,
                                 window_index=1)
         return cls(cfg, input_schema=SCHEMA)
+    if kind == "instant":
+        cfg = O.WindowAggConfig(width=0, key_names=["key"], aggs=AGGS, final_projection=False)
+        return native.InstantAggregatingWindowFunc(cfg, input_schema=SCHEMA)
     if kind == "session":
         return native.SessionAggregatingWindowFunc(O.SessionConfig(gap=S, key_names=["key"], aggs=AGGS, window_index=1),
                                                    input_schema=SCHEMA)
@@ -118,11 +121,32 @@ def test_on_start_takes_the_state_batches_it_restores(kind):
     op.close()
 
 
+def _broken(how, b):
+    """`b` with the wrong column count ("columns"), or with its first state column, an Int64 one in the layout of
+    tables "t" and "a", as Float64 ("type")."""
+    if how == "columns":
+        return b.drop_columns([b.schema.names[-2]])
+    col = b.column(1)
+    assert col.type == pa.int64()
+    return b.set_column(1, b.schema.field(1).with_type(pa.float64()), col.cast(pa.float64()))
+
+
+# "last": only the last batch has the wrong column count.  Table "s" of the session holds raw input rows, where a
+# Float64 value is an unsupported input type rather than a broken layout: it keeps the column-count case only.
+REFUSALS = [pytest.param(k, h, id=k if h == "columns" else f"{k}-{h}")
+            for k in ("tumbling", "sliding", "instant", "session", "updating")
+            for h in ("columns", "type", "last") if k != "session" or h == "columns"]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("kind", ["tumbling", "sliding", "session", "updating"])
-def test_a_refused_on_start_leaves_the_state_batches_to_the_caller(kind):
+@pytest.mark.parametrize("kind,how", REFUSALS)
+def test_a_refused_on_start_leaves_the_state_batches_to_the_caller(kind, how):
     batches, wm, t = _state(kind)
-    bad = [b.drop_columns([b.schema.names[-2]]) for b in batches]  # the wrong column count
+    assert len(batches) >= 2
+    if how == "last":
+        bad = batches[:-1] + [_broken("columns", batches[-1])]
+    else:
+        bad = [_broken(how, b) for b in batches]
     op = _new(kind)
     st, arrs, schs = _on_start(op, bad, wm, t)
     assert st == ffi.INVALID_ARGUMENT
@@ -130,7 +154,9 @@ def test_a_refused_on_start_leaves_the_state_batches_to_the_caller(kind):
     for s in arrs + schs:
         C.CFUNCTYPE(None, C.c_void_p)(s.release)(C.addressof(s))
         assert s.release is None
-    assert op.stats()["rows_in"] == 0
+    stats = op.stats()
+    assert stats["rows_in"] == 0
+    assert stats["n_keys"] == 0
     op.close()
 
 
