@@ -98,52 +98,6 @@ inline void require_aggregate_input_types(const std::vector<InColumn>& cols, int
   }
 }
 
-// The joins compare raw 64-bit key patterns, which is equality only for integer-like keys of one type: an Int64,
-// UInt64 or timestamp[ns] key, the same type on both sides (INTEGRATION.md §1).  A Float64 key (-0.0 = 0.0) or an
-// Int64 key against a UInt64 key is refused.  `seen_*`: the key format an earlier batch of this / the other side
-// carried ("" while unknown).
-inline int join_key_class(const std::string& f) {
-  if (f == "l") return 1;
-  if (f == "L") return 2;
-  if (f.compare(0, 4, "tsn:") == 0) return 3;
-  return 0;
-}
-inline void require_join_key_type(const std::string& f, const std::string& seen_this, const std::string& seen_other) {
-  const int k = join_key_class(f);
-  if (k == 0) throw Error(ARROYO_B200_UNSUPPORTED, "join key of type '" + f + "' (supported: l, L, tsn:)");
-  for (const std::string* s : {&seen_this, &seen_other})
-    if (!s->empty() && join_key_class(*s) != k)
-      throw Error(ARROYO_B200_UNSUPPORTED, "join key of type '" + f + "' after keys of type '" + *s + "'");
-}
-
-// One input of a join: its columns are the leading `_key_*` routing copies (`n_routing` of them), then the key, the
-// timestamp and the payload in any order.  The routing copies are stripped from the output like `unkeyed_batch`
-// does (arroyo-rpc/src/df.rs:359-367) and never reach the device.
-struct JoinSide {
-  int n_cols = 0, ts_col = 0, key_col = 0, n_routing = 0;
-  std::vector<int> payload;          // input column indices that appear in the output
-  std::vector<std::string> formats;  // Arrow format per input column
-  std::string key_format;            // the key's format once a host batch has shown it
-  std::vector<DevBuf> cols;          // device columns (the routing columns stay empty)
-};
-
-inline void init_join_side(JoinSide& s, int n_cols, int ts_col, int key_col, int n_routing) {
-  AB_REQUIRE(n_cols >= 2 && n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad join side n_cols");
-  AB_REQUIRE(ts_col >= 0 && ts_col < n_cols && key_col >= 0 && key_col < n_cols && n_routing >= 0 && n_routing < n_cols,
-             ARROYO_B200_INVALID_ARGUMENT, "bad join side columns");
-  AB_REQUIRE(key_col >= n_routing && ts_col >= n_routing, ARROYO_B200_INVALID_ARGUMENT,
-             "join key or timestamp column among the routing columns");
-  s.n_cols = n_cols;
-  s.ts_col = ts_col;
-  s.key_col = key_col;
-  s.n_routing = n_routing;
-  for (int i = n_routing; i < n_cols; ++i)
-    if (i != ts_col) s.payload.push_back(i);
-  s.formats.assign(n_cols, "l");
-  s.formats[ts_col] = "tsn:";
-  s.cols.resize(n_cols);
-}
-
 // ---- export -------------------------------------------------------------------------------
 struct OutColumn {
   std::string name;

@@ -22,13 +22,10 @@
 #include <algorithm>
 #include <climits>
 
-#include "op.h"
-#include "scan.cuh"
+#include "join_side.h"
 
 namespace ab {
 namespace {
-
-constexpr int JT = 256;
 
 __device__ __forceinline__ uint64_t pair_hash(long long key, long long ts) {
   return mix64((uint64_t)key ^ mix64((uint64_t)ts));
@@ -152,43 +149,6 @@ __global__ void append_unmatched_kernel(const unsigned char* __restrict__ elig, 
   }
 }
 
-struct GatherParams {
-  const int* idx;          // pair side to read
-  const long long* src;    // source column
-  long long* dst;
-  unsigned char* valid;    // optional validity bytes
-  long long n;
-};
-__global__ void gather_kernel(const __grid_constant__ GatherParams p) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < p.n; i += stride) {
-    int j = p.idx[i];
-    p.dst[i] = j >= 0 ? p.src[j] : 0;
-    if (p.valid) p.valid[i] = j >= 0 ? 1 : 0;
-  }
-}
-__global__ void gather_ts_kernel(const int* __restrict__ il, const int* __restrict__ ir, const long long* __restrict__ lts,
-                                 const long long* __restrict__ rts, long long* __restrict__ dst, long long n) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < n; i += stride) {
-    int a = il[i], b = ir[i];
-    long long ta = a >= 0 ? lts[a] : LLONG_MIN, tb = b >= 0 ? rts[b] : LLONG_MIN;
-    dst[i] = max(ta, tb);
-  }
-}
-// validity bytes -> Arrow validity bitmap (LSB first)
-__global__ void pack_bits_kernel(const unsigned char* __restrict__ bytes, long long n, unsigned int* __restrict__ words) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long n_pad = (n + 31) / 32 * 32;
-  long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < n_pad; i += stride) {
-    bool v = i < n && bytes[i];
-    unsigned int b = __ballot_sync(0xffffffffu, v);
-    if ((threadIdx.x & 31) == 0) words[i >> 5] = b;
-  }
-}
 // keep[i] = !elig[i] as counts for the compaction scan
 __global__ void keep_counts_kernel(const unsigned char* __restrict__ elig, long long n, unsigned int* __restrict__ cnt) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -205,12 +165,10 @@ __global__ void compact_kernel(const long long* __restrict__ src, const unsigned
 
 struct Side : JoinSide {
   std::vector<DevBuf> cols_alt;  // compaction target of `cols`
-  int64_t n = 0, cap = 0;
-  DevBuf elig, cnt, off;
-  int64_t scratch_cap = 0;
+  DevBuf elig, cnt, off;  // per-row scratch of the watermark, `cap` rows
 };
 
-class InstantJoinOp final : public OpBase {
+class InstantJoinOp final : public JoinOpBase {
  public:
   explicit InstantJoinOp(const ArroyoB200OpConfig& c);
   ~InstantJoinOp() override;
@@ -236,7 +194,6 @@ class InstantJoinOp final : public OpBase {
     AB_CUDA(cudaStreamSynchronize(stream_));
     inputs_.release(true);
   }
-  void stats(ArroyoB200Stats* out) override { *out = st_; }
 
  private:
   int join_type_;
@@ -244,18 +201,10 @@ class InstantJoinOp final : public OpBase {
   int64_t last_wm_ = INT64_MIN;
   DevBuf scalars_;  // [0] n_elig L, [1] n_elig R, [2] min_ts L, [3] min_ts R, [4] total, [5] cursor
   PinnedBuf h_scalars_;
-  DevBuf tab_, sums_, pair_l_, pair_r_, r_matched_;
-  int64_t pair_cap_ = 0;
-  std::vector<DevBuf> out_cols_;
-  std::vector<DevBuf> out_valid_;
-  DevBuf out_ts_;
+  DevBuf tab_, r_matched_;
   HeldInputs inputs_;  // host batches whose copies to the side columns may still run
-  ArroyoB200Stats st_{};
 
-  void reserve(Side& s, int64_t extra);
   void append(Side& s, const uint64_t* const* cols, int64_t n, bool host);
-  int grid_for(int64_t n) const { return (int)std::max<int64_t>(1, std::min<int64_t>((n + JT - 1) / JT, (int64_t)num_sms_ * 8)); }
-  void exclusive_scan(const unsigned int* cnt, int64_t n, unsigned long long* off, unsigned long long* total_dev);
   void compact(Side& s);
 };
 
@@ -274,59 +223,27 @@ InstantJoinOp::InstantJoinOp(const ArroyoB200OpConfig& c) {
 
 InstantJoinOp::~InstantJoinOp() { drain_stream(); }
 
-void InstantJoinOp::reserve(Side& s, int64_t extra) {
-  if (s.n + extra <= s.cap) return;
-  int64_t nc = std::max<int64_t>(s.cap * 2, 1 << 16);
-  while (nc < s.n + extra) nc *= 2;
-  // rows are numbered as int (pairs) and as row + 1 in 32 bits (table slots)
-  AB_REQUIRE(nc < (1ll << 31), ARROYO_B200_RUNTIME, "join side holds more than 2^31 rows");
-  for (int c = 0; c < s.n_cols; ++c) {
-    if (c < s.n_routing) continue;
-    DevBuf nb((size_t)nc * 8);
-    if (s.n) AB_CUDA(cudaMemcpyAsync(nb.p, s.cols[c].p, (size_t)s.n * 8, cudaMemcpyDeviceToDevice, stream_));
-    AB_CUDA(cudaStreamSynchronize(stream_));
-    s.cols[c] = std::move(nb);
-    s.cols_alt[c].release();
-  }
-  s.cap = nc;
-}
-
 void InstantJoinOp::append(Side& s, const uint64_t* const* cols, int64_t n, bool host) {
-  reserve(s, n);
-  for (int c = s.n_routing; c < s.n_cols; ++c)
-    AB_CUDA(cudaMemcpyAsync(s.cols[c].as<long long>() + s.n, cols[c], (size_t)n * 8,
-                            host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, stream_));
-  if (host) st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)(s.n_cols - s.n_routing);
-  s.n += n;
+  s.reserve(n, stream_, nullptr, &s.cols_alt);
+  s.append(cols, n, host, stream_, st_);
   st_.rows_in += (uint64_t)n;
 }
 
 void InstantJoinOp::process_batch(uint32_t index, uint32_t in_partitions, ArrowArray* batch, const ArrowSchema* schema) {
   set_device();
-  AB_REQUIRE(in_partitions >= 2 && in_partitions % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
-  const int sd = (int)(index / (in_partitions / 2));  // instant_join.rs:249-253
-  AB_REQUIRE(sd == 0 || sd == 1, ARROYO_B200_INVALID_ARGUMENT, "bad input index");
+  const int sd = side_of(index, in_partitions);
   Side& s = side_[sd];
-  int64_t n = 0;
-  std::vector<InColumn> cols = import_batch(batch, schema, &n);
-  AB_REQUIRE((int)cols.size() == s.n_cols, ARROYO_B200_INVALID_ARGUMENT, "join side has the wrong number of columns");
-  require_join_key_type(cols[s.key_col].format, s.key_format, side_[1 - sd].key_format);
-  AB_REQUIRE(n > 0, ARROYO_B200_PANIC, "should have max timestamp (empty batch; instant_join.rs:123)");
-  for (int c = 0; c < s.n_cols; ++c) s.formats[c] = cols[c].format;
-  s.key_format = cols[s.key_col].format;
-  const uint64_t* ptrs[ARROYO_B200_MAX_COLS];
-  for (int c = 0; c < s.n_cols; ++c) ptrs[c] = cols[c].data;
-  append(s, ptrs, n, true);
+  const JoinBatch b = s.import(batch, schema, s.key_format, side_[1 - sd]);
+  AB_REQUIRE(b.n > 0, ARROYO_B200_PANIC, "should have max timestamp (empty batch; instant_join.rs:123)");
+  s.take_formats(b.cols);
+  append(s, b.data, b.n, true);
   inputs_.hold(batch, stream_);
 }
 
 void InstantJoinOp::process_device_batch(uint32_t index, uint32_t in_partitions, const uint64_t* cols, int32_t n_cols,
                                          int64_t n_rows) {
   set_device();
-  AB_REQUIRE(in_partitions >= 2 && in_partitions % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
-  const int sd = (int)(index / (in_partitions / 2));
-  AB_REQUIRE(sd == 0 || sd == 1, ARROYO_B200_INVALID_ARGUMENT, "bad input index");
-  Side& s = side_[sd];
+  Side& s = side_[side_of(index, in_partitions)];
   AB_REQUIRE(n_cols == s.n_cols, ARROYO_B200_INVALID_ARGUMENT, "join side has the wrong number of columns");
   if (n_rows <= 0) return;
   const uint64_t* ptrs[ARROYO_B200_MAX_COLS];
@@ -334,22 +251,19 @@ void InstantJoinOp::process_device_batch(uint32_t index, uint32_t in_partitions,
   append(s, ptrs, n_rows, false);
 }
 
-void InstantJoinOp::exclusive_scan(const unsigned int* cnt, int64_t n, unsigned long long* off, unsigned long long* total_dev) {
-  device_exclusive_scan(cnt, n, off, total_dev, sums_, stream_);
-  st_.kernel_launches += 3;
-}
-
 // keep rows that did not take part in this watermark's join
 void InstantJoinOp::compact(Side& s) {
   if (s.n == 0) return;
-  keep_counts_kernel<<<grid_for(s.n), JT, 0, stream_>>>(s.elig.as<unsigned char>(), s.n, s.cnt.as<unsigned int>());
+  keep_counts_kernel<<<grid_for(s.n), JOIN_THREADS, 0, stream_>>>(s.elig.as<unsigned char>(), s.n, s.cnt.as<unsigned int>());
   AB_CUDA(cudaGetLastError());
   unsigned long long* total = scalars_.as<unsigned long long>() + 4;
-  exclusive_scan(s.cnt.as<unsigned int>(), s.n, s.off.as<unsigned long long>(), total);
+  device_exclusive_scan(s.cnt.as<unsigned int>(), s.n, s.off.as<unsigned long long>(), total, sums_, stream_);
+  st_.kernel_launches += 3;
   for (int c = s.n_routing; c < s.n_cols; ++c) {
     if (s.cols_alt[c].bytes < (size_t)s.cap * 8) s.cols_alt[c].alloc((size_t)s.cap * 8);
-    compact_kernel<<<grid_for(s.n), JT, 0, stream_>>>(s.cols[c].as<long long>(), s.elig.as<unsigned char>(),
-                                                     s.off.as<unsigned long long>(), s.n, s.cols_alt[c].as<long long>());
+    compact_kernel<<<grid_for(s.n), JOIN_THREADS, 0, stream_>>>(s.cols[c].as<long long>(), s.elig.as<unsigned char>(),
+                                                               s.off.as<unsigned long long>(), s.n,
+                                                               s.cols_alt[c].as<long long>());
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
   }
@@ -374,15 +288,12 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
   AB_CUDA(cudaMemcpyAsync(sc, init, sizeof init, cudaMemcpyHostToDevice, stream_));
   for (int sd = 0; sd < 2; ++sd) {
     Side& s = side_[sd];
-    if (s.scratch_cap < s.cap) {
-      s.elig.alloc((size_t)s.cap);
-      s.cnt.alloc((size_t)s.cap * 4);
-      s.off.alloc((size_t)s.cap * 8);
-      s.scratch_cap = s.cap;
-    }
+    grow(s.elig, (size_t)s.cap);
+    grow(s.cnt, (size_t)s.cap * 4);
+    grow(s.off, (size_t)s.cap * 8);
     if (s.n) {
-      mark_kernel<<<grid_for(s.n), JT, 0, stream_>>>(s.cols[s.ts_col].as<long long>(), s.n, wm, s.elig.as<unsigned char>(),
-                                                    sc + sd, (long long*)(sc + 2 + sd));
+      mark_kernel<<<grid_for(s.n), JOIN_THREADS, 0, stream_>>>(s.cols[s.ts_col].as<long long>(), s.n, wm,
+                                                              s.elig.as<unsigned char>(), sc + sd, (long long*)(sc + 2 + sd));
       AB_CUDA(cudaGetLastError());
       ++st_.kernel_launches;
     }
@@ -418,37 +329,32 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
   if (r_matched_.bytes < (size_t)std::max<int64_t>(Bs.n, 1)) r_matched_.alloc((size_t)std::max<int64_t>(Bs.cap, 1));
   if (Bs.n) AB_CUDA(cudaMemsetAsync(r_matched_.p, 0, (size_t)Bs.n, stream_));
   if (nb) {
-    build_kernel<<<grid_for(Bs.n), JT, 0, stream_>>>(Bs.cols[Bs.key_col].as<long long>(), Bs.cols[Bs.ts_col].as<long long>(),
-                                                    Bs.elig.as<unsigned char>(), Bs.n, tab_.as<JSlot>(), (uint32_t)(cap - 1));
+    build_kernel<<<grid_for(Bs.n), JOIN_THREADS, 0, stream_>>>(Bs.cols[Bs.key_col].as<long long>(),
+                                                              Bs.cols[Bs.ts_col].as<long long>(), Bs.elig.as<unsigned char>(),
+                                                              Bs.n, tab_.as<JSlot>(), (uint32_t)(cap - 1));
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
   }
   int64_t n_probe_out = 0;
   if (Ps.n) {
-    probe_kernel<0><<<grid_for(Ps.n), JT, 0, stream_>>>(
-        Ps.cols[Ps.key_col].as<long long>(), Ps.cols[Ps.ts_col].as<long long>(), Ps.elig.as<unsigned char>(), Ps.n,
-        Bs.cols[Bs.ts_col].as<long long>(), tab_.as<JSlot>(), (uint32_t)(cap - 1), keep_p ? 1 : 0,
-        Ps.cnt.as<unsigned int>(), nullptr, nullptr, nullptr, nullptr);
-    AB_CUDA(cudaGetLastError());
-    exclusive_scan(Ps.cnt.as<unsigned int>(), Ps.n, Ps.off.as<unsigned long long>(), sc + 4);
-    AB_CUDA(cudaMemcpyAsync(h_scalars_.as<unsigned long long>() + 4, sc + 4, 8, cudaMemcpyDeviceToHost, stream_));
-    AB_CUDA(cudaStreamSynchronize(stream_));
-    n_probe_out = (int64_t)h_scalars_.as<unsigned long long>()[4];
-    ++st_.kernel_launches;
+    n_probe_out = count_pairs(
+        [&] {
+          probe_kernel<0><<<grid_for(Ps.n), JOIN_THREADS, 0, stream_>>>(
+              Ps.cols[Ps.key_col].as<long long>(), Ps.cols[Ps.ts_col].as<long long>(), Ps.elig.as<unsigned char>(), Ps.n,
+              Bs.cols[Bs.ts_col].as<long long>(), tab_.as<JSlot>(), (uint32_t)(cap - 1), keep_p ? 1 : 0,
+              Ps.cnt.as<unsigned int>(), nullptr, nullptr, nullptr, nullptr);
+        },
+        Ps.cnt.as<unsigned int>(), Ps.n, Ps.off.as<unsigned long long>(), sc + 4, h_scalars_.as<unsigned long long>() + 4);
   }
   const int64_t max_out = n_probe_out + (keep_b ? nb : 0);
   AB_REQUIRE(max_out < (int64_t)INT_MAX, ARROYO_B200_RUNTIME, "join output too large for one watermark");
   int64_t n_out = n_probe_out;
   if (max_out > 0) {
-    if (pair_cap_ < max_out) {
-      pair_l_.alloc((size_t)max_out * 4);
-      pair_r_.alloc((size_t)max_out * 4);
-      pair_cap_ = max_out;
-    }
-    int* pair_p = bsd == 0 ? pair_r_.as<int>() : pair_l_.as<int>();
-    int* pair_b = bsd == 0 ? pair_l_.as<int>() : pair_r_.as<int>();
+    reserve_pairs(max_out);
+    int* pair_p = pairs_[1 - bsd].as<int>();
+    int* pair_b = pairs_[bsd].as<int>();
     if (n_probe_out) {
-      probe_kernel<1><<<grid_for(Ps.n), JT, 0, stream_>>>(
+      probe_kernel<1><<<grid_for(Ps.n), JOIN_THREADS, 0, stream_>>>(
           Ps.cols[Ps.key_col].as<long long>(), Ps.cols[Ps.ts_col].as<long long>(), Ps.elig.as<unsigned char>(), Ps.n,
           Bs.cols[Bs.ts_col].as<long long>(), tab_.as<JSlot>(), (uint32_t)(cap - 1), keep_p ? 1 : 0, nullptr,
           Ps.off.as<unsigned long long>(), pair_p, pair_b, r_matched_.as<unsigned char>());
@@ -458,8 +364,8 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
     if (keep_b && nb) {
       unsigned long long cur = (unsigned long long)n_probe_out;
       AB_CUDA(cudaMemcpyAsync(sc + 5, &cur, 8, cudaMemcpyHostToDevice, stream_));
-      append_unmatched_kernel<<<grid_for(Bs.n), JT, 0, stream_>>>(Bs.elig.as<unsigned char>(), r_matched_.as<unsigned char>(),
-                                                                 Bs.n, sc + 5, pair_p, pair_b);
+      append_unmatched_kernel<<<grid_for(Bs.n), JOIN_THREADS, 0, stream_>>>(
+          Bs.elig.as<unsigned char>(), r_matched_.as<unsigned char>(), Bs.n, sc + 5, pair_p, pair_b);
       AB_CUDA(cudaGetLastError());
       AB_CUDA(cudaMemcpyAsync(h_scalars_.as<unsigned long long>() + 5, sc + 5, 8, cudaMemcpyDeviceToHost, stream_));
       AB_CUDA(cudaStreamSynchronize(stream_));
@@ -468,90 +374,7 @@ void InstantJoinOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vec
     }
   }
 
-  if (n_out > 0) {
-    // gather [left payload..., right payload..., _timestamp]
-    const size_t n_oc = L.payload.size() + R.payload.size();
-    out_cols_.resize(n_oc);
-    out_valid_.resize(n_oc);
-    const bool l_nullable = keep_r, r_nullable = keep_l;
-    size_t oc = 0;
-    for (int sd = 0; sd < 2; ++sd) {
-      Side& s = side_[sd];
-      const bool nullable = sd == 0 ? l_nullable : r_nullable;
-      for (int c : s.payload) {
-        if (out_cols_[oc].bytes < (size_t)n_out * 8) out_cols_[oc].alloc((size_t)n_out * 8);
-        if (nullable && out_valid_[oc].bytes < (size_t)n_out + 64) out_valid_[oc].alloc((size_t)n_out + 64);
-        GatherParams gp{sd == 0 ? pair_l_.as<int>() : pair_r_.as<int>(), s.cols[c].as<long long>(),
-                        out_cols_[oc].as<long long>(), nullable ? out_valid_[oc].as<unsigned char>() : nullptr, n_out};
-        gather_kernel<<<grid_for(n_out), JT, 0, stream_>>>(gp);
-        AB_CUDA(cudaGetLastError());
-        ++st_.kernel_launches;
-        ++oc;
-      }
-    }
-    if (out_ts_.bytes < (size_t)n_out * 8) out_ts_.alloc((size_t)n_out * 8);
-    gather_ts_kernel<<<grid_for(n_out), JT, 0, stream_>>>(pair_l_.as<int>(), pair_r_.as<int>(), L.cols[L.ts_col].as<long long>(),
-                                                         R.cols[R.ts_col].as<long long>(), out_ts_.as<long long>(), n_out);
-    AB_CUDA(cudaGetLastError());
-    ++st_.kernel_launches;
-    st_.rows_out += (uint64_t)n_out;
-    ++st_.windows_out;
-
-    if (out_host) {
-      std::vector<OutColumn> cols;
-      oc = 0;
-      DevBuf bits;
-      for (int sd = 0; sd < 2; ++sd) {
-        Side& s = side_[sd];
-        const bool nullable = sd == 0 ? l_nullable : r_nullable;
-        for (int c : s.payload) {
-          OutColumn o;
-          o.name = std::string(sd == 0 ? "l" : "r") + std::to_string(c);
-          o.format = s.formats[c];
-          o.data = d2h_pinned(out_cols_[oc].p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
-          if (nullable) {
-            const size_t words = (size_t)((n_out + 31) / 32);
-            if (bits.bytes < words * 4) bits.alloc(words * 4 + 64);
-            pack_bits_kernel<<<grid_for(n_out), JT, 0, stream_>>>(out_valid_[oc].as<unsigned char>(), n_out, bits.as<unsigned int>());
-            AB_CUDA(cudaGetLastError());
-            o.validity = d2h_pinned(bits.p, words * 4, stream_, &st_.d2h_bytes);
-            AB_CUDA(cudaStreamSynchronize(stream_));  // `bits` is reused by the next column
-            const unsigned int* w = (const unsigned int*)o.validity;
-            int64_t set = 0;
-            for (size_t i = 0; i < words; ++i) set += __builtin_popcount(w[i]);
-            o.null_count = n_out - set;
-            o.nullable = true;
-            if (o.null_count == 0) {
-              PinnedPool::get().free(o.validity);
-              o.validity = nullptr;
-            }
-          }
-          cols.push_back(o);
-          ++oc;
-        }
-      }
-      OutColumn t;
-      t.name = "_timestamp";
-      t.format = "tsn:";
-      t.data = d2h_pinned(out_ts_.p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
-      cols.push_back(t);
-      AB_CUDA(cudaStreamSynchronize(stream_));
-      out_host->arrays.emplace_back();
-      out_host->schemas.emplace_back();
-      export_batch(cols, n_out, &out_host->arrays.back(), &out_host->schemas.back());
-    } else {
-      AB_REQUIRE(join_type_ == ARROYO_B200_JOIN_INNER, ARROYO_B200_UNSUPPORTED,
-                 "device-resident join output is only available for inner joins (no validity bitmaps)");
-      ArroyoB200DeviceBatch d{};
-      d.n_rows = n_out;
-      int c = 0;
-      for (size_t i = 0; i < n_oc; ++i) d.cols[c++] = (uint64_t)out_cols_[i].p;
-      d.cols[c++] = (uint64_t)out_ts_.p;
-      d.n_cols = c;
-      out_dev->push_back(d);
-      AB_CUDA(cudaStreamSynchronize(stream_));
-    }
-  }
+  if (n_out > 0) write_output(L, R, n_out, keep_r, keep_l, out_host, out_dev);
   // rows at or after the watermark stay for later
   compact(L);
   compact(R);

@@ -22,15 +22,12 @@
 // and never probed: the reference's `insert_internal` (expiring_time_key_map.rs:1008-1049) stores restored rows
 // without joining them, so no pair among them leaves again.
 #include <algorithm>
-#include <climits>
+#include <memory>
 
-#include "op.h"
-#include "scan.cuh"
+#include "join_side.h"
 
 namespace ab {
 namespace {
-
-constexpr int TJ = 256;
 
 struct alignas(16) MSlot {
   long long key;
@@ -114,32 +111,13 @@ __global__ void tj_rehash_kernel(const MSlot* __restrict__ old_tab, uint32_t old
   }
 }
 
-struct TGather {
-  const int* idx;
-  const long long* src;
-  long long* dst;
-  long long n;
-};
-__global__ void tj_gather_kernel(const __grid_constant__ TGather p) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < p.n; i += stride) p.dst[i] = p.src[p.idx[i]];
-}
-__global__ void tj_gather_ts_kernel(const int* __restrict__ il, const int* __restrict__ ir, const long long* __restrict__ lts,
-                                    const long long* __restrict__ rts, long long* __restrict__ dst, long long n) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < n; i += stride) dst[i] = max(lts[il[i]], rts[ir[i]]);
-}
-
 struct TSide : JoinSide {
   DevBuf next, tab;
-  int64_t n = 0, cap = 0;
   uint32_t tab_cap = 0;
   uint64_t keys_bound = 0;  // rows linked so far: an upper bound of the distinct keys
 };
 
-class TtlJoinOp final : public OpBase {
+class TtlJoinOp final : public JoinOpBase {
  public:
   explicit TtlJoinOp(const ArroyoB200OpConfig& c);
   ~TtlJoinOp() override;
@@ -149,12 +127,8 @@ class TtlJoinOp final : public OpBase {
   }
   void restore_side(uint32_t side, ArrowArray* batches, ArrowSchema* schemas, int64_t n) override;
   void process_batch(uint32_t index, uint32_t parts, ArrowArray* batch, const ArrowSchema* schema) override {
-    BatchesPriv sink;
-    process_batch_emit(index, parts, batch, schema, &sink);
-    for (auto& a : sink.arrays)
-      if (a.release) a.release(&a);
-    for (auto& s : sink.schemas)
-      if (s.release) s.release(&s);
+    std::unique_ptr<BatchesPriv, void (*)(BatchesPriv*)> sink(new BatchesPriv(), discard);
+    process_batch_emit(index, parts, batch, schema, sink.get());
   }
   void process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* batch, const ArrowSchema* schema, BatchesPriv* out) override;
   void process_device_batch(uint32_t, uint32_t, const uint64_t*, int32_t, int64_t) override {
@@ -167,19 +141,14 @@ class TtlJoinOp final : public OpBase {
     set_device();
     AB_CUDA(cudaStreamSynchronize(stream_));
   }
-  void stats(ArroyoB200Stats* out) override { *out = st_; }
 
  private:
   TSide side_[2];
-  DevBuf cnt_, off_, total_, sums_, pair_new_, pair_old_, out_ts_;
-  std::vector<DevBuf> out_cols_;
-  int64_t scratch_cap_ = 0, pair_cap_ = 0;
+  DevBuf cnt_, off_, total_;
   bool took_input_ = false;  // process_batch has accepted a batch: restore_side is refused from then on
-  ArroyoB200Stats st_{};
 
-  int grid_for(int64_t n) const { return (int)std::max<int64_t>(1, std::min<int64_t>((n + TJ - 1) / TJ, (int64_t)num_sms_ * 8)); }
-  void reserve(TSide& s, int64_t extra);
   void ensure_table(TSide& s, uint64_t more_rows);
+  void insert(TSide& s, const JoinBatch* in, int64_t n_batches, int64_t rows);
 };
 
 TtlJoinOp::TtlJoinOp(const ArroyoB200OpConfig& c) {
@@ -195,22 +164,6 @@ TtlJoinOp::TtlJoinOp(const ArroyoB200OpConfig& c) {
 
 TtlJoinOp::~TtlJoinOp() { drain_stream(); }
 
-void TtlJoinOp::reserve(TSide& s, int64_t extra) {
-  if (s.n + extra <= s.cap) return;
-  int64_t nc = std::max<int64_t>(s.cap * 2, 1 << 16);
-  while (nc < s.n + extra) nc *= 2;
-  AB_REQUIRE(nc < (1ll << 31), ARROYO_B200_RUNTIME, "join side holds more than 2^31 rows");
-  auto grow = [&](DevBuf& b, size_t elem) {
-    DevBuf nb((size_t)nc * elem);
-    if (s.n && b.p) AB_CUDA(cudaMemcpyAsync(nb.p, b.p, (size_t)s.n * elem, cudaMemcpyDeviceToDevice, stream_));
-    AB_CUDA(cudaStreamSynchronize(stream_));
-    b = std::move(nb);
-  };
-  for (int c = s.n_routing; c < s.n_cols; ++c) grow(s.cols[c], 8);
-  grow(s.next, 4);
-  s.cap = nc;
-}
-
 // the multimap stays at most half full of distinct keys (bounded by the rows linked so far)
 void TtlJoinOp::ensure_table(TSide& s, uint64_t more_rows) {
   const uint64_t need = (s.keys_bound + more_rows) * 2 + 1024;
@@ -221,7 +174,8 @@ void TtlJoinOp::ensure_table(TSide& s, uint64_t more_rows) {
   DevBuf nt((size_t)nc * sizeof(MSlot));
   AB_CUDA(cudaMemsetAsync(nt.p, 0, (size_t)nc * sizeof(MSlot), stream_));
   if (s.tab_cap) {
-    tj_rehash_kernel<<<grid_for(s.tab_cap), TJ, 0, stream_>>>(s.tab.as<MSlot>(), s.tab_cap, nt.as<MSlot>(), (uint32_t)(nc - 1));
+    tj_rehash_kernel<<<grid_for(s.tab_cap), JOIN_THREADS, 0, stream_>>>(s.tab.as<MSlot>(), s.tab_cap, nt.as<MSlot>(),
+                                                                       (uint32_t)(nc - 1));
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
   }
@@ -230,9 +184,24 @@ void TtlJoinOp::ensure_table(TSide& s, uint64_t more_rows) {
   s.tab_cap = (uint32_t)nc;
 }
 
+// Inserts accepted host batches of `rows` rows in all into side `s`'s key-time table (:52 / :83, insert_internal
+// :1008-1049): one reserve and one table sizing for all of them, their rows copied into consecutive arena ranges,
+// then linked into the multimap by one launch.
+void TtlJoinOp::insert(TSide& s, const JoinBatch* in, int64_t n_batches, int64_t rows) {
+  s.reserve(rows, stream_, &s.next);
+  ensure_table(s, (uint64_t)rows);
+  const int64_t first = s.n;
+  for (int64_t b = 0; b < n_batches; ++b)
+    if (in[b].n) s.append(in[b].data, in[b].n, true, stream_, st_);
+  tj_link_kernel<<<grid_for(rows), JOIN_THREADS, 0, stream_>>>(s.cols[s.key_col].as<long long>(), first, rows,
+                                                              s.tab.as<MSlot>(), s.tab_cap - 1, s.next.as<int>());
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  s.keys_bound += (uint64_t)rows;
+}
+
 // KeyTimeView::insert_internal (:1008-1049) for the batches of one side's table: every batch is checked before anything
-// changes, then the call's rows are copied into consecutive arena ranges and linked by one launch.  A restore that
-// succeeds takes every batch.
+// changes, then the call's rows are inserted without probing.  A restore that succeeds takes every batch.
 void TtlJoinOp::restore_side(uint32_t side, ArrowArray* batches, ArrowSchema* schemas, int64_t n) {
   AB_REQUIRE(side <= 1, ARROYO_B200_INVALID_ARGUMENT, "restore_side: side must be 0 (left) or 1 (right)");
   AB_REQUIRE(n >= 0 && (n == 0 || (batches != nullptr && schemas != nullptr)), ARROYO_B200_INVALID_ARGUMENT,
@@ -240,109 +209,61 @@ void TtlJoinOp::restore_side(uint32_t side, ArrowArray* batches, ArrowSchema* sc
   AB_REQUIRE(!took_input_, ARROYO_B200_INVALID_ARGUMENT,
              "JoinWithExpiration: restore_side after process_batch (restore before the first batch)");
   TSide& s = side_[side];
-  std::vector<std::vector<InColumn>> cols((size_t)n);
-  std::vector<int64_t> rows((size_t)n, 0);
-  std::string key_format = s.key_format;
+  std::vector<JoinBatch> in((size_t)n);
   int64_t total = 0;
   for (int64_t b = 0; b < n; ++b) {
-    cols[b] = import_batch(&batches[b], &schemas[b], &rows[b]);
-    AB_REQUIRE((int)cols[b].size() == s.n_cols, ARROYO_B200_INVALID_ARGUMENT,
-               "restore_side: batch does not have the side's number of columns");
-    require_join_key_type(cols[b][s.key_col].format, key_format, side_[1 - side].key_format);
-    key_format = cols[b][s.key_col].format;
-    total += rows[b];
+    in[b] = s.import(&batches[b], &schemas[b], b ? in[b - 1].cols[s.key_col].format : s.key_format, side_[1 - side],
+                     "restore_side: batch does not have the side's number of columns");
+    total += in[b].n;
   }
   set_device();
   if (total > 0) {
-    reserve(s, total);
-    ensure_table(s, (uint64_t)total);
-    long long at = s.n;
-    for (int64_t b = 0; b < n; ++b) {
-      for (int c = s.n_routing; c < s.n_cols; ++c)
-        if (rows[b])
-          AB_CUDA(cudaMemcpyAsync(s.cols[c].as<long long>() + at, cols[b][c].data, (size_t)rows[b] * 8,
-                                  cudaMemcpyHostToDevice, stream_));
-      at += rows[b];
-    }
-    st_.h2d_bytes += (uint64_t)total * 8 * (uint64_t)(s.n_cols - s.n_routing);
-    tj_link_kernel<<<grid_for(total), TJ, 0, stream_>>>(s.cols[s.key_col].as<long long>(), s.n, total, s.tab.as<MSlot>(),
-                                                      s.tab_cap - 1, s.next.as<int>());
-    AB_CUDA(cudaGetLastError());
-    ++st_.kernel_launches;
+    insert(s, in.data(), n, total);
     AB_CUDA(cudaStreamSynchronize(stream_));
-    s.n += total;
-    s.keys_bound += (uint64_t)total;
   }
-  if (n > 0) {
-    for (int c = 0; c < s.n_cols; ++c) s.formats[c] = cols[n - 1][c].format;
-    s.key_format = key_format;
-  }
+  if (n > 0) s.take_formats(in[n - 1].cols);
   for (int64_t b = 0; b < n; ++b)
     if (batches[b].release) batches[b].release(&batches[b]);
 }
 
 void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* batch, const ArrowSchema* schema, BatchesPriv* out) {
   set_device();
-  AB_REQUIRE(parts >= 2 && parts % 2 == 0, ARROYO_B200_INVALID_ARGUMENT, "join needs an even number of inputs");
-  const int sd = (int)(index / (parts / 2));
-  AB_REQUIRE(sd == 0 || sd == 1, ARROYO_B200_INVALID_ARGUMENT, "bad input index");
+  const int sd = side_of(index, parts);
   TSide& s = side_[sd];
   TSide& o = side_[1 - sd];
-  int64_t n = 0;
-  std::vector<InColumn> cols = import_batch(batch, schema, &n);
-  AB_REQUIRE((int)cols.size() == s.n_cols, ARROYO_B200_INVALID_ARGUMENT, "join side has the wrong number of columns");
-  require_join_key_type(cols[s.key_col].format, s.key_format, o.key_format);
-  for (int c = 0; c < s.n_cols; ++c) s.formats[c] = cols[c].format;
-  s.key_format = cols[s.key_col].format;
+  const JoinBatch b = s.import(batch, schema, s.key_format, o);
+  s.take_formats(b.cols);
   took_input_ = true;
-  st_.rows_in += (uint64_t)n;
+  st_.rows_in += (uint64_t)b.n;
+  const int64_t n = b.n;
   if (n == 0) {
     if (batch->release) batch->release(batch);
     batch->release = nullptr;
     return;
   }
   // 1. append + link (insert into this side's key-time table, :52 / :83)
-  reserve(s, n);
-  ensure_table(s, (uint64_t)n);
   const long long first = s.n;
-  for (int c = s.n_routing; c < s.n_cols; ++c)
-    AB_CUDA(cudaMemcpyAsync(s.cols[c].as<long long>() + first, cols[c].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
-  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)(s.n_cols - s.n_routing);
-  tj_link_kernel<<<grid_for(n), TJ, 0, stream_>>>(s.cols[s.key_col].as<long long>(), first, n, s.tab.as<MSlot>(), s.tab_cap - 1,
-                                                s.next.as<int>());
-  AB_CUDA(cudaGetLastError());
-  ++st_.kernel_launches;
+  insert(s, &b, 1, n);
   ++st_.ingest_launches;
-  s.n += n;
-  s.keys_bound += (uint64_t)n;
   // 2. the other side's rows of these keys (get_batch, :59-64 / :90-95) x the batch (compute_pair)
   int64_t n_out = 0;
   if (o.n > 0) {
-    if (n > scratch_cap_) {
-      scratch_cap_ = std::max<int64_t>(n, scratch_cap_ * 2);
-      cnt_.alloc((size_t)scratch_cap_ * 4);
-      off_.alloc((size_t)scratch_cap_ * 8);
-    }
+    grow(cnt_, (size_t)n * 4);
+    grow(off_, (size_t)n * 8);
     const long long* pkey = s.cols[s.key_col].as<long long>();
-    tj_probe_kernel<0><<<grid_for(n), TJ, 0, stream_>>>(pkey, first, n, o.tab.as<MSlot>(), o.tab_cap - 1, o.next.as<int>(),
-                                                       cnt_.as<unsigned int>(), nullptr, nullptr, nullptr);
-    AB_CUDA(cudaGetLastError());
-    device_exclusive_scan(cnt_.as<unsigned int>(), n, off_.as<unsigned long long>(), total_.as<unsigned long long>(), sums_, stream_);
     unsigned long long h_total = 0;
-    AB_CUDA(cudaMemcpyAsync(&h_total, total_.p, 8, cudaMemcpyDeviceToHost, stream_));
-    AB_CUDA(cudaStreamSynchronize(stream_));
-    st_.kernel_launches += 4;
-    n_out = (int64_t)h_total;
+    n_out = count_pairs(
+        [&] {
+          tj_probe_kernel<0><<<grid_for(n), JOIN_THREADS, 0, stream_>>>(pkey, first, n, o.tab.as<MSlot>(), o.tab_cap - 1,
+                                                                        o.next.as<int>(), cnt_.as<unsigned int>(), nullptr,
+                                                                        nullptr, nullptr);
+        },
+        cnt_.as<unsigned int>(), n, off_.as<unsigned long long>(), total_.as<unsigned long long>(), &h_total);
     if (n_out > 0) {
-      if (n_out > pair_cap_) {
-        pair_cap_ = std::max<int64_t>(n_out, pair_cap_ * 2);
-        pair_new_.alloc((size_t)pair_cap_ * 4);
-        pair_old_.alloc((size_t)pair_cap_ * 4);
-        out_ts_.alloc((size_t)pair_cap_ * 8);
-        out_cols_.clear();
-      }
-      tj_probe_kernel<1><<<grid_for(n), TJ, 0, stream_>>>(pkey, first, n, o.tab.as<MSlot>(), o.tab_cap - 1, o.next.as<int>(), nullptr,
-                                                         off_.as<unsigned long long>(), pair_new_.as<int>(), pair_old_.as<int>());
+      reserve_pairs(n_out);
+      tj_probe_kernel<1><<<grid_for(n), JOIN_THREADS, 0, stream_>>>(pkey, first, n, o.tab.as<MSlot>(), o.tab_cap - 1,
+                                                                    o.next.as<int>(), nullptr, off_.as<unsigned long long>(),
+                                                                    pairs_[sd].as<int>(), pairs_[1 - sd].as<int>());
       AB_CUDA(cudaGetLastError());
       ++st_.kernel_launches;
     }
@@ -351,49 +272,10 @@ void TtlJoinOp::process_batch_emit(uint32_t index, uint32_t parts, ArrowArray* b
   AB_CUDA(cudaStreamSynchronize(stream_));
   if (batch->release) batch->release(batch);
   batch->release = nullptr;
-  if (n_out == 0 || !out) return;
+  if (n_out == 0) return;
   // 3. output = [left payload..., right payload..., _timestamp = max(l, r)]
-  const int* il = sd == 0 ? pair_new_.as<int>() : pair_old_.as<int>();
-  const int* ir = sd == 0 ? pair_old_.as<int>() : pair_new_.as<int>();
-  const size_t n_oc = side_[0].payload.size() + side_[1].payload.size();
-  if (out_cols_.size() != n_oc) {
-    out_cols_.clear();
-    for (size_t i = 0; i < n_oc; ++i) out_cols_.emplace_back((size_t)pair_cap_ * 8);
-  }
-  std::vector<OutColumn> ocols;
-  size_t oc = 0;
-  for (int side = 0; side < 2; ++side) {
-    TSide& z = side_[side];
-    for (int c : z.payload) {
-      TGather g{side == 0 ? il : ir, z.cols[c].as<long long>(), out_cols_[oc].as<long long>(), n_out};
-      tj_gather_kernel<<<grid_for(n_out), TJ, 0, stream_>>>(g);
-      AB_CUDA(cudaGetLastError());
-      ++st_.kernel_launches;
-      OutColumn col;
-      col.name = (side == 0 ? "l" : "r") + std::to_string(c);
-      col.format = z.formats[c];
-      col.data = d2h_pinned(out_cols_[oc].p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
-      ocols.push_back(col);
-      ++oc;
-    }
-  }
-  tj_gather_ts_kernel<<<grid_for(n_out), TJ, 0, stream_>>>(il, ir, side_[0].cols[side_[0].ts_col].as<long long>(),
-                                                          side_[1].cols[side_[1].ts_col].as<long long>(), out_ts_.as<long long>(),
-                                                          n_out);
-  AB_CUDA(cudaGetLastError());
-  ++st_.kernel_launches;
+  write_output(side_[0], side_[1], n_out, false, false, out, nullptr);
   ++st_.emit_launches;
-  OutColumn t;
-  t.name = "_timestamp";
-  t.format = "tsn:";
-  t.data = d2h_pinned(out_ts_.p, (size_t)n_out * 8, stream_, &st_.d2h_bytes);
-  ocols.push_back(t);
-  AB_CUDA(cudaStreamSynchronize(stream_));
-  st_.rows_out += (uint64_t)n_out;
-  ++st_.windows_out;
-  out->arrays.emplace_back();
-  out->schemas.emplace_back();
-  export_batch(ocols, n_out, &out->arrays.back(), &out->schemas.back());
 }
 
 }  // namespace
