@@ -56,3 +56,16 @@ class JoinConfig:
     left_routing_keys: List[str] = field(default_factory=list)
     right_routing_keys: List[str] = field(default_factory=list)
     ttl: int = 0
+
+
+@dataclass
+class WindowFunctionConfig:
+    """WindowFunctionOperator (arroyo-worker/src/arrow/window_fn.rs): `function` (row_number | rank | dense_rank)
+    OVER (PARTITION BY window [, `partition_by`] ORDER BY `order_by`), the function column named `name`.  `order_by`
+    is a list of (column, descending).  `top_n` > 0 fuses the `WHERE name <= top_n` that follows the operator; 0 lets
+    every row through."""
+    function: str
+    partition_by: Optional[str]
+    order_by: List[tuple]
+    name: str
+    top_n: int = 0

@@ -151,6 +151,9 @@ int32_t arroyo_b200_op_create(const ArroyoB200OpConfig* config, ArroyoB200Op** o
       case ARROYO_B200_INSTANT_AGGREGATE:
         impl = make_instant_agg_op(*config);
         break;
+      case ARROYO_B200_WINDOW_FUNCTION:
+        impl = make_window_fn_op(*config);
+        break;
       default:
         set_err(err, err_len, "unknown operator kind");
         return ARROYO_B200_INVALID_ARGUMENT;

@@ -28,16 +28,81 @@ inline bool format_is_64bit(const char* f) {
   return false;
 }
 
+// A struct column of a batch imported with its structs flattened: its children are flat columns
+// [first, first + names.size()).
+struct Nest {
+  int first;
+  std::string name;
+  std::vector<std::string> names, formats;
+};
+
 // Validates a record batch exported as a struct array and returns its columns.  Nulls are refused, except in column
-// `nullable_col`, whose validity bitmap is then handed back.
+// `nullable_col`, whose validity bitmap is then handed back.  With `nests`, a struct column whose children are all
+// 64-bit takes their places among the columns and is recorded there (one level; the window function's input);
+// without it, as everywhere else, a struct column is refused.
 inline std::vector<InColumn> import_batch(const ArrowArray* a, const ArrowSchema* s, int64_t* n_rows,
-                                          int64_t nullable_col = -1) {
+                                          int64_t nullable_col = -1, std::vector<Nest>* nests = nullptr) {
   AB_REQUIRE(a && s, ARROYO_B200_INVALID_ARGUMENT, "null batch or schema");
   AB_REQUIRE(s->format && !strcmp(s->format, "+s"), ARROYO_B200_INVALID_ARGUMENT,
              "batch must be exported as a struct array (format +s)");
   AB_REQUIRE(a->n_children == s->n_children, ARROYO_B200_INVALID_ARGUMENT, "array/schema children mismatch");
   AB_REQUIRE(a->null_count <= 0 || a->n_buffers == 0 || a->buffers[0] == nullptr, ARROYO_B200_UNSUPPORTED,
              "null rows at the struct level are not supported");
+  if (nests) {
+    nests->clear();
+    // the struct array's children become the batch's: its offset adds to theirs (the batch's is kept separately)
+    std::vector<const ArrowArray*> arrays;
+    std::vector<const ArrowSchema*> schemas;
+    std::vector<int64_t> offsets;
+    std::vector<ArrowArray> flat_storage;
+    for (int64_t i = 0; i < a->n_children; ++i) {
+      const ArrowArray* c = a->children[i];
+      const ArrowSchema* cs = s->children[i];
+      AB_REQUIRE(c && cs, ARROYO_B200_INVALID_ARGUMENT, "null child");
+      if (!cs->format || strcmp(cs->format, "+s") != 0) {
+        arrays.push_back(c);
+        schemas.push_back(cs);
+        offsets.push_back(0);
+        continue;
+      }
+      AB_REQUIRE(c->n_children == cs->n_children && c->n_children > 0, ARROYO_B200_INVALID_ARGUMENT,
+                 "struct column: array/schema children mismatch");
+      AB_REQUIRE(c->length >= a->length + a->offset, ARROYO_B200_INVALID_ARGUMENT, "child shorter than batch");
+      AB_REQUIRE(c->null_count == 0 || c->n_buffers == 0 || c->buffers[0] == nullptr, ARROYO_B200_UNSUPPORTED,
+                 std::string("column ") + (cs->name ? cs->name : "?") + " has nulls: NULLs are outside the supported subset");
+      Nest n;
+      n.first = (int)arrays.size();
+      n.name = cs->name ? cs->name : "";
+      for (int64_t j = 0; j < c->n_children; ++j) {
+        AB_REQUIRE(c->children[j] && cs->children[j], ARROYO_B200_INVALID_ARGUMENT, "null child");
+        AB_REQUIRE(!cs->children[j]->format || strcmp(cs->children[j]->format, "+s") != 0, ARROYO_B200_UNSUPPORTED,
+                   "struct column nested in a struct column");
+        arrays.push_back(c->children[j]);
+        schemas.push_back(cs->children[j]);
+        offsets.push_back(c->offset);
+        n.names.push_back(cs->children[j]->name ? cs->children[j]->name : "");
+        n.formats.push_back(cs->children[j]->format ? cs->children[j]->format : "");
+      }
+      nests->push_back(n);
+    }
+    // the flattened batch, as a view: children with the struct's offset folded into their own
+    flat_storage.resize(arrays.size());
+    std::vector<ArrowArray*> ap(arrays.size());
+    std::vector<ArrowSchema*> sp(arrays.size());
+    for (size_t i = 0; i < arrays.size(); ++i) {
+      flat_storage[i] = *arrays[i];
+      flat_storage[i].offset += offsets[i];
+      flat_storage[i].length -= offsets[i];
+      ap[i] = &flat_storage[i];
+      sp[i] = const_cast<ArrowSchema*>(schemas[i]);
+    }
+    ArrowArray fa = *a;
+    ArrowSchema fs = *s;
+    fa.n_children = fs.n_children = (int64_t)arrays.size();
+    fa.children = ap.data();
+    fs.children = sp.data();
+    return import_batch(&fa, &fs, n_rows, nullable_col);
+  }
   std::vector<InColumn> cols;
   cols.reserve(a->n_children);
   for (int64_t i = 0; i < a->n_children; ++i) {

@@ -107,5 +107,6 @@ OpBase* make_session_op(const ArroyoB200OpConfig& cfg);
 OpBase* make_updating_agg_op(const ArroyoB200OpConfig& cfg);
 OpBase* make_ttl_join_op(const ArroyoB200OpConfig& cfg);
 OpBase* make_instant_agg_op(const ArroyoB200OpConfig& cfg);
+OpBase* make_window_fn_op(const ArroyoB200OpConfig& cfg);
 
 }  // namespace ab

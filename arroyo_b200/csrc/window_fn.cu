@@ -1,0 +1,884 @@
+// Window function on sm_90a (H100): the GPU side of `WindowFunctionOperator` (arroyo-worker/src/arrow/window_fn.rs),
+// for ROW_NUMBER / RANK / DENSE_RANK () OVER (PARTITION BY window [, key] ORDER BY k1 [DESC], ...), optionally fused
+// with the `WHERE fn <= N` that usually follows it (top N per window).  The planner (plan/window_fn.rs:101-105) drops
+// the `window` column from PARTITION BY: each upstream window stamps its rows with one `_timestamp`, so the rows are
+// bucketed by `_timestamp` ("instant") and the remaining PARTITION BY column, if any, splits each instant further.
+//
+//   store   every accepted row, SoA, one 64-bit array per flat input column; a row's index is its arrival sequence.
+//           The host doubles the store before a launch that could overfill it, from the rows it has handed over since
+//           it last read the row count;
+//   ingest  per launch: flag the rows that stay (ts >= the last watermark, filter_by_time in arroyo-rpc/src/df.rs:
+//           211-231; a negative ts is reported, the reference panics on it), device_exclusive_scan, append them in
+//           order behind the stored rows;
+//   emit    at watermark w every instant < w leaves (window_fn.rs:178-201): flag and compact the indices of the rows
+//           with ts < w, then stable LSD radix passes (CUB) starting from arrival order: the ORDER BY keys last to
+//           first, the partition key, `_timestamp`.  Each key is sorted in an unsigned order-preserving form (sign bit
+//           flipped for signed types, all bits complemented for DESC).  A rank pass flags segment starts (instant,
+//           partition) and peer starts (every sort key) and scans them, ballots within a warp and a two-level scan
+//           across 1024-row tiles: ROW_NUMBER = position in the segment + 1, RANK = position of the first peer + 1,
+//           DENSE_RANK = peer starts in the segment so far.  The fused filter, a compaction and a gather of every column
+//           write the output in sorted order; the rows that stay are compacted to the front of the store, in arrival
+//           order, so device memory tracks the open rows;
+//   state   table "input": a checkpoint writes the rows accepted since the previous one (one store index marks them,
+//           re-based when the store is compacted), one batch per instant, in the input layout.  on_start appends the
+//           restored rows first and does not late-filter them, as the reference re-feeds them (:130-145).
+// Rows that tie on every sort key leave in arrival order, restored rows first; DataFusion's sort promises no order
+// there, and RANK and DENSE_RANK do not depend on it.  Output rows of one emission leave in one batch (the reference
+// emits one batch per instant; the rows and their order are the same).  Device-resident output is refused.
+#include <algorithm>
+#include <climits>
+#include <functional>
+
+#include <cub/device/device_radix_sort.cuh>
+
+#include "op.h"
+#include "scan.cuh"
+
+namespace ab {
+namespace {
+
+constexpr int WF_THREADS = 256;
+constexpr int WF_TILE = 1024;  // rows per rank tile: one per thread, 32 warps
+constexpr unsigned FULL = 0xffffffffu;
+constexpr uint64_t WF_MAX_ROWS = 1ull << 31;
+constexpr int MAX_SORT_COLS = 2 + ARROYO_B200_MAX_ORDER_KEYS;  // _timestamp, the partition key, the ORDER BY keys
+
+struct WCounters {
+  unsigned long long n_store;  // rows in the store
+  unsigned long long late;
+  unsigned long long total;     // scan total
+  unsigned long long instants;  // instants of the last emission
+  unsigned int neg_ts;          // a row with a negative _timestamp arrived
+  unsigned int pad;
+};
+
+struct WCols {
+  unsigned long long* c[ARROYO_B200_MAX_COLS];
+};
+
+// flag[i] = row i of a launch stays: ts >= late_wm (LLONG_MIN: no watermark yet) and ts >= 0.  Counts late rows and
+// notes negative timestamps.  The loop bound is uniform per warp, so every lane reaches the warp reduction.
+__global__ void __launch_bounds__(WF_THREADS) wf_flag_kernel(const long long* __restrict__ ts, long long n,
+                                                             long long late_wm, unsigned int* __restrict__ flag,
+                                                             WCounters* counters) {
+  const unsigned lane = threadIdx.x & 31;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  unsigned int late = 0;
+  bool neg = false;
+  for (long long row0 = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); row0 < n; row0 += stride) {
+    const long long i = row0 + lane;
+    if (i >= n) continue;
+    const long long t = __ldcs(ts + i);
+    neg |= t < 0;
+    late += (t >= 0 && t < late_wm) ? 1u : 0u;
+    flag[i] = (t >= 0 && t >= late_wm) ? 1u : 0u;
+  }
+  const unsigned int wl = __reduce_add_sync(FULL, late);
+  if (lane == 0 && wl) atomicAdd(&counters->late, (unsigned long long)wl);
+  if (neg) counters->neg_ts = 1u;
+}
+
+// The flagged rows of a launch, appended in order behind the `*n_store` stored rows.
+struct WAppend {
+  const unsigned long long* in[ARROYO_B200_MAX_COLS];
+  WCols store;
+  int n_cols;
+  const unsigned int* flag;
+  const unsigned long long* off;
+  long long n;
+  const unsigned long long* n_store;
+};
+__global__ void __launch_bounds__(WF_THREADS) wf_append_kernel(const __grid_constant__ WAppend p) {
+  const unsigned long long base = *p.n_store;
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < p.n; i += stride) {
+    if (!p.flag[i]) continue;
+    const unsigned long long d = base + p.off[i];
+    for (int c = 0; c < p.n_cols; ++c) p.store.c[c][d] = __ldcs(p.in[c] + i);
+  }
+}
+
+// *n_store += the launch's scan total (a kernel of its own: every thread of the append reads the old count)
+__global__ void wf_advance_kernel(WCounters* c) { c->n_store += c->total; }
+__global__ void wf_set_rows_kernel(WCounters* c, unsigned long long n) { c->n_store = n; }
+
+// flag[i] = stored row i leaves at watermark w
+__global__ void wf_mark_kernel(const long long* __restrict__ ts, long long n, long long w, unsigned int* __restrict__ flag) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) flag[i] = ts[i] < w ? 1u : 0u;
+}
+
+// the flagged rows' store indices, compacted in arrival order
+__global__ void wf_select_kernel(const unsigned int* __restrict__ flag, const unsigned long long* __restrict__ off,
+                                 long long n, unsigned int* __restrict__ idx) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < n; i += stride)
+    if (flag[i]) idx[off[i]] = (unsigned int)i;
+}
+
+__global__ void wf_iota_kernel(unsigned int* __restrict__ idx, unsigned int first, long long n) {
+  long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; j < n; j += stride) idx[j] = first + (unsigned int)j;
+}
+
+// k[j] = the sort key of row idx[j] in its unsigned order-preserving form: col ^ flip
+__global__ void wf_key_kernel(const unsigned long long* __restrict__ col, const unsigned int* __restrict__ idx, long long n,
+                              unsigned long long flip, unsigned long long* __restrict__ k) {
+  long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; j < n; j += stride) k[j] = col[idx[j]] ^ flip;
+}
+
+// ---- ranks ------------------------------------------------------------------------------------------------------------
+// The scan that turns the segment and peer starts of the sorted rows into ranks.  An element is row j's
+// {seg = j + 1 if a segment starts there else 0, peer = the same for a peer group, dcnt = 1 if a peer group starts there};
+// over a range, seg / peer are the last starts in it and dcnt counts the peer starts from its last segment start on (all
+// of them when none starts in it).  A segment start is always a peer start.
+struct RankVal {
+  unsigned int seg, peer, dcnt;
+};
+__device__ __forceinline__ RankVal rv_combine(RankVal a, RankVal b) {
+  return {b.seg ? b.seg : a.seg, b.peer ? b.peer : a.peer, b.seg ? b.dcnt : a.dcnt + b.dcnt};
+}
+__device__ __forceinline__ RankVal rv_shfl_up(RankVal v, int o) {
+  return {__shfl_up_sync(FULL, v.seg, o), __shfl_up_sync(FULL, v.peer, o), __shfl_up_sync(FULL, v.dcnt, o)};
+}
+
+// Inclusive scan of one tile of WF_TILE rows (one per thread, `bits`: 2 = segment start, 4 = peer start), positions
+// from `j` of the calling thread; the tile's total goes to `*total`.  Within a warp the starts are two ballots: the last
+// start at or below a lane is the highest set bit of its ballot prefix.  Every thread of the block calls it.
+__device__ __forceinline__ RankVal tile_inclusive(unsigned int bits, long long j, RankVal* total) {
+  __shared__ RankVal s_warp[WF_TILE / 32];
+  const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const unsigned sb = __ballot_sync(FULL, bits & 2u), pb = __ballot_sync(FULL, bits & 4u);
+  const unsigned le = lane == 31 ? FULL : (2u << lane) - 1u;
+  const unsigned s = sb & le, p = pb & le;
+  const long long lane0 = j - (long long)lane;
+  RankVal v;
+  v.seg = s ? (unsigned int)(lane0 + (31 - __clz(s))) + 1u : 0u;
+  v.peer = p ? (unsigned int)(lane0 + (31 - __clz(p))) + 1u : 0u;
+  v.dcnt = s ? (unsigned int)__popc(p & ~((1u << (31 - __clz(s))) - 1u)) : (unsigned int)__popc(p);
+  if (lane == 31) s_warp[w] = v;
+  __syncthreads();
+  if (w == 0) {
+    RankVal x = s_warp[lane];
+    for (int o = 1; o < 32; o <<= 1) {
+      const RankVal y = rv_shfl_up(x, o);
+      if ((int)lane >= o) x = rv_combine(y, x);
+    }
+    s_warp[lane] = x;
+  }
+  __syncthreads();
+  if (w > 0) v = rv_combine(s_warp[w - 1], v);
+  *total = s_warp[WF_TILE / 32 - 1];
+  return v;
+}
+
+struct WRank {
+  const unsigned long long* col[MAX_SORT_COLS];  // _timestamp, the partition key (keyed), the ORDER BY keys
+  int n_col;
+  int keyed;
+  const unsigned int* idx;  // sorted
+  long long n;
+  unsigned char* bits;  // per sorted row: 1 = instant start, 2 = segment start, 4 = peer start
+  RankVal* tiles;       // per tile: its total, then (wf_rank_carry_kernel) the scan of the tiles before it
+  unsigned long long* instants;
+  int fn;
+  long long top_n;
+  unsigned long long* fn_out;
+  unsigned int* keep;  // the fused filter
+};
+
+// pass 1: the starts of each sorted row (against the row before it), the instants, and each tile's total
+__global__ void __launch_bounds__(WF_TILE) wf_rank_flags_kernel(const __grid_constant__ WRank p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  unsigned int bits = 0;
+  if (j < p.n) {
+    if (j == 0) {
+      bits = 7u;
+    } else {
+      const unsigned int a = p.idx[j], b = p.idx[j - 1];
+      const bool inst = p.col[0][a] != p.col[0][b];
+      bool seg = inst;
+      if (p.keyed) seg |= p.col[1][a] != p.col[1][b];
+      bool peer = seg;
+      for (int c = 1 + p.keyed; c < p.n_col; ++c) peer |= p.col[c][a] != p.col[c][b];
+      bits = (inst ? 1u : 0u) | (seg ? 2u : 0u) | (peer ? 4u : 0u);
+    }
+    p.bits[j] = (unsigned char)bits;
+  }
+  const int starts = __syncthreads_count(bits & 1u);
+  if (threadIdx.x == 0 && starts) atomicAdd(p.instants, (unsigned long long)starts);
+  RankVal total;
+  tile_inclusive(bits, j, &total);
+  if (threadIdx.x == 0) p.tiles[blockIdx.x] = total;
+}
+
+// pass 2, one block: tiles[t] becomes the exclusive scan of the totals of tiles [0, t), 1024 tiles per round
+__global__ void __launch_bounds__(1024) wf_rank_carry_kernel(RankVal* tiles, long long n_tiles) {
+  __shared__ RankVal s_warp[32];
+  __shared__ RankVal s_carry;
+  const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const RankVal zero = {0u, 0u, 0u};
+  if (threadIdx.x == 0) s_carry = zero;
+  __syncthreads();
+  for (long long base = 0; base < n_tiles; base += 1024) {
+    const long long i = base + threadIdx.x;
+    const RankVal v = i < n_tiles ? tiles[i] : zero;
+    RankVal x = v;
+    for (int o = 1; o < 32; o <<= 1) {
+      const RankVal y = rv_shfl_up(x, o);
+      if ((int)lane >= o) x = rv_combine(y, x);
+    }
+    RankVal ex = rv_shfl_up(x, 1);  // exclusive within the warp
+    if (lane == 0) ex = zero;
+    if (lane == 31) s_warp[w] = x;
+    __syncthreads();
+    if (w == 0) {
+      RankVal t = s_warp[lane];
+      for (int o = 1; o < 32; o <<= 1) {
+        const RankVal y = rv_shfl_up(t, o);
+        if ((int)lane >= o) t = rv_combine(y, t);
+      }
+      s_warp[lane] = t;  // inclusive over warps
+    }
+    __syncthreads();
+    const RankVal carry = s_carry;
+    RankVal before = w > 0 ? rv_combine(carry, s_warp[w - 1]) : carry;
+    if (i < n_tiles) tiles[i] = rv_combine(before, ex);
+    __syncthreads();
+    if (threadIdx.x == 0) s_carry = rv_combine(carry, s_warp[31]);
+    __syncthreads();
+  }
+}
+
+// pass 3: each sorted row's function value and whether the fused filter keeps it
+__global__ void __launch_bounds__(WF_TILE) wf_rank_apply_kernel(const __grid_constant__ WRank p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  const unsigned int bits = j < p.n ? p.bits[j] : 0u;
+  RankVal total;
+  const RankVal v = tile_inclusive(bits, j, &total);
+  if (j >= p.n) return;
+  const RankVal s = rv_combine(p.tiles[blockIdx.x], v);
+  unsigned long long f;
+  if (p.fn == ARROYO_B200_FN_ROW_NUMBER) f = (unsigned long long)(j + 2) - s.seg;
+  else if (p.fn == ARROYO_B200_FN_RANK) f = (unsigned long long)(s.peer - s.seg) + 1ull;
+  else f = s.dcnt;
+  p.fn_out[j] = f;
+  p.keep[j] = (p.top_n == 0 || f <= (unsigned long long)p.top_n) ? 1u : 0u;
+}
+
+// out[c][o] = store[c][idx[j]] for the kept rows (keep null: every row, o = j), and the function column
+struct WGather {
+  const unsigned long long* store[ARROYO_B200_MAX_COLS];
+  WCols out;
+  int n_cols;
+  const unsigned int* idx;
+  const unsigned int* keep;
+  const unsigned long long* off;
+  const unsigned long long* fn;
+  unsigned long long* fn_out;
+  long long n;
+};
+__global__ void __launch_bounds__(WF_THREADS) wf_gather_kernel(const __grid_constant__ WGather p) {
+  long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; j < p.n; j += stride) {
+    if (p.keep && !p.keep[j]) continue;
+    const unsigned long long o = p.keep ? p.off[j] : (unsigned long long)j;
+    const unsigned int src = p.idx[j];
+    for (int c = 0; c < p.n_cols; ++c) p.out.c[c][o] = p.store[c][src];
+    if (p.fn_out) p.fn_out[o] = p.fn[j];
+  }
+}
+
+// the rows that stay, moved to [0, n - leaving) of `to` in arrival order: new index = i - (rows leaving below it)
+struct WCompact {
+  const unsigned long long* from[ARROYO_B200_MAX_COLS];
+  WCols to;
+  int n_cols;
+  const unsigned int* flag;
+  const unsigned long long* off;
+  long long n;
+};
+__global__ void __launch_bounds__(WF_THREADS) wf_compact_kernel(const __grid_constant__ WCompact p) {
+  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < p.n; i += stride) {
+    if (p.flag[i]) continue;
+    const unsigned long long d = (unsigned long long)i - p.off[i];
+    for (int c = 0; c < p.n_cols; ++c) p.to.c[c][d] = p.from[c][i];
+  }
+}
+
+// room for `bytes`, kept across calls (grown by half again so that a slowly growing need does not reallocate each time)
+void reserve(DevBuf& b, size_t bytes) {
+  if (b.bytes < bytes) b.alloc(std::max(bytes, b.bytes + b.bytes / 2));
+}
+
+bool sortable_format(const std::string& f) { return f == "l" || f == "L" || f.compare(0, 4, "tsn:") == 0; }
+
+class WindowFnOp final : public OpBase {
+ public:
+  explicit WindowFnOp(const ArroyoB200OpConfig& c);
+  ~WindowFnOp() override { drain_stream(); }
+  void on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t watermark, int64_t table_min) override;
+  void process_batch(uint32_t, uint32_t, ArrowArray* batch, const ArrowSchema* schema) override;
+  void process_device_batch(uint32_t, uint32_t, const uint64_t* cols, int32_t n_cols, int64_t n_rows) override;
+  void handle_watermark(int64_t wm, BatchesPriv* out_host, std::vector<ArroyoB200DeviceBatch>* out_dev) override;
+  void handle_checkpoint(int64_t wm, BatchesPriv* out) override;
+  void on_close(int, BatchesPriv*) override { flush(); }
+  void flush() override {
+    set_device();
+    AB_CUDA(cudaStreamSynchronize(stream_));
+  }
+  void stats(ArroyoB200Stats* out) override {
+    set_device();
+    read_counters();
+    *out = st_;
+  }
+
+ private:
+  struct Store {
+    DevBuf col[ARROYO_B200_MAX_COLS];
+  };
+  // The input layout, flat: one entry per 64-bit column; `nests_` re-nests the struct columns of host batches.
+  struct Layout {
+    std::vector<std::string> names, formats;
+    std::vector<Nest> nests;
+  };
+  int n_cols_ = 0, ts_col_ = 0, key_col_ = -1, fn_ = 0;
+  int n_order_ = 0, order_col_[ARROYO_B200_MAX_ORDER_KEYS] = {}, order_desc_[ARROYO_B200_MAX_ORDER_KEYS] = {};
+  int64_t top_n_ = 0;
+  Layout layout_;
+  bool typed_ = false;  // layout_ comes from a host or state batch (else: Int64 columns, no structs)
+  int64_t late_wm_ = LLONG_MIN;
+  Store cur_, alt_;  // alt_: where the rows that stay after an emission go (allocated on first use)
+  uint64_t cap_ = 0;
+  uint64_t n_store_ = 0;   // as of the last read
+  uint64_t store_hi_ = 0;  // upper bound of the stored rows: n_store_ + rows handed over since
+  uint64_t ckpt_from_ = 0; // rows [ckpt_from_, n) arrived since the last checkpoint
+  DevBuf counters_, stage_;
+  uint64_t stage_cap_ = 0;
+  DevBuf flag_, off_, sums_, idx_[2], key_[2], cub_tmp_, bits_, tiles_, fnv_, keep_, off2_;
+  DevBuf out_[ARROYO_B200_MAX_COLS], out_fn_;
+  ArroyoB200Stats st_{};
+
+  int grid_for(uint64_t n) const {
+    return (int)std::max<uint64_t>(1, std::min<uint64_t>((n + WF_THREADS - 1) / WF_THREADS, (uint64_t)num_sms_ * 8));
+  }
+  WCounters* counters() const { return counters_.as<WCounters>(); }
+  const char* fn_name() const {
+    return fn_ == ARROYO_B200_FN_ROW_NUMBER ? "row_number" : fn_ == ARROYO_B200_FN_RANK ? "rank" : "dense_rank";
+  }
+  Layout layout_of(const std::vector<InColumn>& cols, const std::vector<Nest>& nests, const ArrowSchema* s) const;
+  void check_layout(const Layout& l, int bad_type_status) const;
+  void adopt(const Layout& l);
+  std::vector<OutColumn> host_columns(const std::function<void*(int)>& data) const;
+  void alloc_store(Store& s, uint64_t cap) const;
+  void reserve_rows(uint64_t more);
+  void read_counters();
+  const unsigned long long* const* stage(const std::vector<InColumn>& cols, int64_t n, const unsigned long long** ptrs);
+  void ingest(const unsigned long long* const* cols, int64_t n, long long late_wm);
+  unsigned int* sort_rows(uint64_t e, bool by_ts_only);
+  void emit(int64_t w, BatchesPriv* out);
+};
+
+WindowFnOp::WindowFnOp(const ArroyoB200OpConfig& c) {
+  cfg = c;
+  name = "window_function";
+  AB_REQUIRE(c.window_fn == ARROYO_B200_FN_ROW_NUMBER || c.window_fn == ARROYO_B200_FN_RANK ||
+                 c.window_fn == ARROYO_B200_FN_DENSE_RANK,
+             ARROYO_B200_INVALID_ARGUMENT, "window function: window_fn must be ROW_NUMBER (1), RANK (2) or DENSE_RANK (3)");
+  fn_ = c.window_fn;
+  AB_REQUIRE(c.n_cols >= 1 && c.n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad n_cols");
+  n_cols_ = c.n_cols;
+  AB_REQUIRE(c.timestamp_col >= 0 && c.timestamp_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT, "bad timestamp_col");
+  ts_col_ = c.timestamp_col;
+  AB_REQUIRE(c.n_key_cols >= 0, ARROYO_B200_INVALID_ARGUMENT, "bad n_key_cols");
+  AB_REQUIRE(c.n_key_cols <= 1, ARROYO_B200_UNSUPPORTED,
+             "window function: PARTITION BY over more than one column besides the window is not supported");
+  if (c.n_key_cols == 1) {
+    AB_REQUIRE(c.key_col >= 0 && c.key_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT, "bad key_col");
+    key_col_ = c.key_col;
+  }
+  AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= ARROYO_B200_MAX_ORDER_KEYS, ARROYO_B200_INVALID_ARGUMENT,
+             "window function: ORDER BY takes 1 to 4 keys (n_aggs)");
+  n_order_ = c.n_aggs;
+  for (int k = 0; k < n_order_; ++k) {
+    AB_REQUIRE(c.aggs[k].kind == ARROYO_B200_ORDER_ASC || c.aggs[k].kind == ARROYO_B200_ORDER_DESC,
+               ARROYO_B200_INVALID_ARGUMENT, "window function: an ORDER BY key's kind is ORDER_ASC (16) or ORDER_DESC (17)");
+    AB_REQUIRE(c.aggs[k].input_col >= 0 && c.aggs[k].input_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT,
+               "window function: ORDER BY column out of range");
+    order_col_[k] = c.aggs[k].input_col;
+    order_desc_[k] = c.aggs[k].kind == ARROYO_B200_ORDER_DESC;
+  }
+  AB_REQUIRE(c.slide_ns >= 0, ARROYO_B200_INVALID_ARGUMENT, "window function: top N (slide_ns) must be >= 0");
+  top_n_ = c.slide_ns;
+  for (int f = 0; f < n_cols_; ++f) {
+    layout_.names.push_back(f == ts_col_ ? "_timestamp" : "c" + std::to_string(f));
+    layout_.formats.push_back(f == ts_col_ ? "tsn:" : "l");
+  }
+  open_device(c);
+  counters_.alloc(sizeof(WCounters));
+  AB_CUDA(cudaMemsetAsync(counters_.p, 0, sizeof(WCounters), stream_));
+  cap_ = 1u << 16;
+  alloc_store(cur_, cap_);
+  AB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+// The flat layout of an imported batch: names and formats per flat column, and its struct columns.
+WindowFnOp::Layout WindowFnOp::layout_of(const std::vector<InColumn>& cols, const std::vector<Nest>& nests,
+                                         const ArrowSchema* s) const {
+  Layout l;
+  l.nests = nests;
+  for (int64_t i = 0; i < s->n_children; ++i) {
+    const ArrowSchema* cs = s->children[i];
+    if (cs->format && !strcmp(cs->format, "+s")) {
+      for (int64_t j = 0; j < cs->n_children; ++j) l.names.push_back(cs->children[j]->name ? cs->children[j]->name : "");
+    } else {
+      l.names.push_back(cs->name ? cs->name : "");
+    }
+  }
+  for (const InColumn& c : cols) l.formats.push_back(c.format);
+  return l;
+}
+
+// A batch's layout against the plan: its column count and the sort keys' types (`bad_type_status` when a key's type is
+// not l, L or tsn:), and, once the operator has its types, the same formats and struct columns.
+void WindowFnOp::check_layout(const Layout& l, int bad_type_status) const {
+  AB_REQUIRE((int)l.formats.size() == n_cols_, ARROYO_B200_INVALID_ARGUMENT,
+             "window function: batch has " + std::to_string(l.formats.size()) + " flat columns, the plan " +
+                 std::to_string(n_cols_));
+  if (key_col_ >= 0 && !sortable_format(l.formats[key_col_]))
+    throw Error(bad_type_status, "window function: PARTITION BY column of type '" + l.formats[key_col_] +
+                                     "' (supported: l, L, tsn:)");
+  for (int k = 0; k < n_order_; ++k)
+    if (!sortable_format(l.formats[order_col_[k]]))
+      throw Error(bad_type_status, "window function: ORDER BY column of type '" + l.formats[order_col_[k]] +
+                                       "' (supported: l, L, tsn:; Float64 ordering is not supported)");
+  if (!typed_) return;
+  bool same = l.formats == layout_.formats && l.nests.size() == layout_.nests.size();
+  for (size_t i = 0; same && i < l.nests.size(); ++i)
+    same = l.nests[i].first == layout_.nests[i].first && l.nests[i].names.size() == layout_.nests[i].names.size();
+  AB_REQUIRE(same, ARROYO_B200_INVALID_ARGUMENT,
+             "window function: batch layout (column types or struct columns) differs from the operator's input layout");
+}
+
+void WindowFnOp::adopt(const Layout& l) {
+  if (typed_) return;
+  layout_ = l;
+  typed_ = true;
+}
+
+// The columns of an output or state batch in the input layout, struct columns re-nested: `data(f)` gives flat column
+// f's pinned host buffer.
+std::vector<OutColumn> WindowFnOp::host_columns(const std::function<void*(int)>& data) const {
+  std::vector<OutColumn> cols;
+  auto column = [&](int f) {
+    OutColumn c;
+    c.name = layout_.names[f];
+    c.format = layout_.formats[f];
+    c.data = data(f);
+    return c;
+  };
+  for (int f = 0; f < n_cols_;) {
+    const Nest* nest = nullptr;
+    for (const Nest& x : layout_.nests)
+      if (x.first == f) nest = &x;
+    if (!nest) {
+      cols.push_back(column(f++));
+      continue;
+    }
+    OutColumn s;
+    s.name = nest->name;
+    s.format = "+s";
+    for (size_t k = 0; k < nest->names.size(); ++k) s.children.push_back(column(f + (int)k));
+    cols.push_back(s);
+    f += (int)nest->names.size();
+  }
+  return cols;
+}
+
+void WindowFnOp::alloc_store(Store& s, uint64_t cap) const {
+  for (int c = 0; c < n_cols_; ++c) s.col[c].alloc(cap * 8);
+}
+
+// Reads the counters (waits for the stream): the stored rows, the late rows, and a negative timestamp, on which the
+// reference panics.
+void WindowFnOp::read_counters() {
+  WCounters c{};
+  AB_CUDA(cudaMemcpyAsync(&c, counters_.p, sizeof c, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  n_store_ = store_hi_ = c.n_store;
+  st_.rows_late = c.late;
+  if (c.neg_ts) {
+    AB_CUDA(cudaMemsetAsync(&counters()->neg_ts, 0, 4, stream_));
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    throw Error(ARROYO_B200_PANIC, "batch holds a negative _timestamp (before the Unix epoch): the reference panics on it");
+  }
+}
+
+// Room for `more` rows: the bound is tightened from the device's count before the store doubles.  Past 2^31 rows the
+// call is refused before anything changes.
+void WindowFnOp::reserve_rows(uint64_t more) {
+  if (store_hi_ + more <= cap_) return;
+  read_counters();
+  AB_REQUIRE(n_store_ + more <= WF_MAX_ROWS, ARROYO_B200_RUNTIME, "window function: more than 2^31 buffered rows");
+  if (n_store_ + more <= cap_) return;
+  uint64_t nc = cap_ * 2;
+  while (nc < n_store_ + more) nc *= 2;
+  nc = std::min<uint64_t>(nc, WF_MAX_ROWS);
+  Store ns;
+  alloc_store(ns, nc);
+  for (int c = 0; c < n_cols_; ++c)
+    if (n_store_) AB_CUDA(cudaMemcpyAsync(ns.col[c].p, cur_.col[c].p, n_store_ * 8, cudaMemcpyDeviceToDevice, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  cur_ = std::move(ns);
+  alt_ = Store();
+  cap_ = nc;
+}
+
+// Copies the `n` rows of a host batch's flat columns to the device; `ptrs` receives the device columns.  The host batch
+// must outlive the copies.
+const unsigned long long* const* WindowFnOp::stage(const std::vector<InColumn>& cols, int64_t n,
+                                                   const unsigned long long** ptrs) {
+  if ((uint64_t)n > stage_cap_) {
+    AB_CUDA(cudaStreamSynchronize(stream_));
+    stage_cap_ = std::max<uint64_t>((uint64_t)n, stage_cap_ * 2);
+    stage_.alloc((size_t)n_cols_ * stage_cap_ * 8);
+  }
+  for (int c = 0; c < n_cols_; ++c) {
+    unsigned long long* d = stage_.as<unsigned long long>() + (size_t)c * stage_cap_;
+    AB_CUDA(cudaMemcpyAsync(d, cols[c].data, (size_t)n * 8, cudaMemcpyHostToDevice, stream_));
+    ptrs[c] = d;
+  }
+  st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)n_cols_;
+  return ptrs;
+}
+
+// Appends the rows of device columns `cols` with ts >= late_wm (and ts >= 0) to the store, in order.
+void WindowFnOp::ingest(const unsigned long long* const* cols, int64_t n, long long late_wm) {
+  reserve_rows((uint64_t)n);
+  reserve(flag_, (size_t)n * 4);
+  reserve(off_, (size_t)n * 8);
+  wf_flag_kernel<<<grid_for((uint64_t)n), WF_THREADS, 0, stream_>>>((const long long*)cols[ts_col_], n, late_wm,
+                                                                      flag_.as<unsigned int>(), counters());
+  AB_CUDA(cudaGetLastError());
+  device_exclusive_scan(flag_.as<unsigned int>(), n, off_.as<unsigned long long>(), &counters()->total, sums_, stream_);
+  WAppend p{};
+  for (int c = 0; c < n_cols_; ++c) {
+    p.in[c] = cols[c];
+    p.store.c[c] = cur_.col[c].as<unsigned long long>();
+  }
+  p.n_cols = n_cols_;
+  p.flag = flag_.as<unsigned int>();
+  p.off = off_.as<unsigned long long>();
+  p.n = n;
+  p.n_store = &counters()->n_store;
+  wf_append_kernel<<<grid_for((uint64_t)n), WF_THREADS, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  wf_advance_kernel<<<1, 1, 0, stream_>>>(counters());
+  AB_CUDA(cudaGetLastError());
+  st_.kernel_launches += 6;
+  ++st_.ingest_launches;
+  store_hi_ += (uint64_t)n;
+}
+
+void WindowFnOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const ArrowSchema* schema) {
+  set_device();
+  int64_t n = 0;
+  std::vector<Nest> nests;
+  const std::vector<InColumn> cols = import_batch(batch, schema, &n, -1, &nests);
+  const Layout l = layout_of(cols, nests, schema);
+  check_layout(l, ARROYO_B200_UNSUPPORTED);
+  adopt(l);
+  st_.rows_in += (uint64_t)n;
+  if (n > 0) {
+    const unsigned long long* ptrs[ARROYO_B200_MAX_COLS];
+    ingest(stage(cols, n, ptrs), n, late_wm_);
+    // the staging buffer is reused by the next batch, and a negative timestamp is reported with this batch
+    read_counters();
+  }
+  if (batch->release) batch->release(batch);
+  batch->release = nullptr;
+}
+
+void WindowFnOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols, int32_t n_cols, int64_t n_rows) {
+  set_device();
+  AB_REQUIRE(n_cols == n_cols_, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
+  if (n_rows <= 0) return;
+  st_.rows_in += (uint64_t)n_rows;
+  ingest((const unsigned long long* const*)cols, n_rows, late_wm_);
+}
+
+// Sorts the `e` store indices in idx_[0] and returns the buffer holding the sorted ones: stable LSD radix passes from
+// arrival order, the ORDER BY keys last to first, the partition key, then `_timestamp` (`by_ts_only`: that pass alone).
+unsigned int* WindowFnOp::sort_rows(uint64_t e, bool by_ts_only) {
+  reserve(idx_[1], e * 4);
+  reserve(key_[0], e * 8);
+  reserve(key_[1], e * 8);
+  struct Pass {
+    int col;
+    unsigned long long flip;
+    int end_bit;
+  };
+  std::vector<Pass> passes;
+  const unsigned long long sign = 1ull << 63;
+  auto flip_of = [&](int col, bool desc) {
+    const unsigned long long f = layout_.formats[col] == "L" ? 0ull : sign;
+    return desc ? ~f : f;
+  };
+  if (!by_ts_only) {
+    for (int k = n_order_ - 1; k >= 0; --k) passes.push_back({order_col_[k], flip_of(order_col_[k], order_desc_[k]), 64});
+    if (key_col_ >= 0) passes.push_back({key_col_, flip_of(key_col_, false), 64});
+  }
+  passes.push_back({ts_col_, 0ull, 63});  // timestamps are >= 0: bit 63 is never set
+  cub::DoubleBuffer<unsigned long long> keys(key_[0].as<unsigned long long>(), key_[1].as<unsigned long long>());
+  cub::DoubleBuffer<unsigned int> vals(idx_[0].as<unsigned int>(), idx_[1].as<unsigned int>());
+  size_t tmp = 0;
+  AB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, vals, (int64_t)e, 0, 64, stream_));
+  reserve(cub_tmp_, std::max<size_t>(tmp, 1));
+  for (const Pass& ps : passes) {
+    // the keys of the rows in their current order
+    wf_key_kernel<<<grid_for(e), WF_THREADS, 0, stream_>>>(cur_.col[ps.col].as<unsigned long long>(), vals.Current(),
+                                                           (long long)e, ps.flip, keys.Current());
+    AB_CUDA(cudaGetLastError());
+    tmp = cub_tmp_.bytes;
+    AB_CUDA(cub::DeviceRadixSort::SortPairs(cub_tmp_.p, tmp, keys, vals, (int64_t)e, 0, ps.end_bit, stream_));
+    st_.kernel_launches += 2;
+  }
+  return vals.Current();
+}
+
+// handle_watermark (:178-201): every instant below `wm` leaves, in ascending order, and its rows are freed.
+void WindowFnOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vector<ArroyoB200DeviceBatch>*) {
+  set_device();
+  AB_REQUIRE(out_host != nullptr, ARROYO_B200_UNSUPPORTED, "window function: device-resident output is not implemented");
+  read_counters();
+  if (n_store_ > 0 && wm != LLONG_MIN) emit(wm, out_host);
+  late_wm_ = std::max<int64_t>(late_wm_, wm);
+}
+
+void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
+  const uint64_t n = n_store_;
+  reserve(flag_, n * 4);
+  reserve(off_, n * 8);
+  wf_mark_kernel<<<grid_for(n), WF_THREADS, 0, stream_>>>(cur_.col[ts_col_].as<long long>(), (long long)n, w,
+                                                          flag_.as<unsigned int>());
+  AB_CUDA(cudaGetLastError());
+  device_exclusive_scan(flag_.as<unsigned int>(), (int64_t)n, off_.as<unsigned long long>(), &counters()->total, sums_,
+                        stream_);
+  st_.kernel_launches += 4;
+  unsigned long long e = 0, below = 0;  // rows leaving; of them, rows below the checkpoint boundary
+  AB_CUDA(cudaMemcpyAsync(&e, &counters()->total, 8, cudaMemcpyDeviceToHost, stream_));
+  if (ckpt_from_ < n)
+    AB_CUDA(cudaMemcpyAsync(&below, off_.as<unsigned long long>() + ckpt_from_, 8, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  if (e == 0) return;
+  if (ckpt_from_ >= n) below = e;
+
+  // the leaving rows, sorted
+  reserve(idx_[0], e * 4);
+  wf_select_kernel<<<grid_for(n), WF_THREADS, 0, stream_>>>(flag_.as<unsigned int>(), off_.as<unsigned long long>(),
+                                                            (long long)n, idx_[0].as<unsigned int>());
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  const unsigned int* idx = sort_rows(e, false);
+
+  // ranks and the fused filter
+  const uint64_t n_tiles = (e + WF_TILE - 1) / WF_TILE;
+  reserve(bits_, e);
+  reserve(tiles_, n_tiles * sizeof(RankVal));
+  reserve(fnv_, e * 8);
+  reserve(keep_, e * 4);
+  reserve(off2_, e * 8);
+  AB_CUDA(cudaMemsetAsync(&counters()->instants, 0, 8, stream_));
+  WRank r{};
+  r.col[0] = cur_.col[ts_col_].as<unsigned long long>();
+  r.n_col = 1;
+  if (key_col_ >= 0) r.col[r.n_col++] = cur_.col[key_col_].as<unsigned long long>();
+  for (int k = 0; k < n_order_; ++k) r.col[r.n_col++] = cur_.col[order_col_[k]].as<unsigned long long>();
+  r.keyed = key_col_ >= 0 ? 1 : 0;
+  r.idx = idx;
+  r.n = (long long)e;
+  r.bits = bits_.as<unsigned char>();
+  r.tiles = tiles_.as<RankVal>();
+  r.instants = &counters()->instants;
+  r.fn = fn_;
+  r.top_n = top_n_;
+  r.fn_out = fnv_.as<unsigned long long>();
+  r.keep = keep_.as<unsigned int>();
+  wf_rank_flags_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(r);
+  AB_CUDA(cudaGetLastError());
+  wf_rank_carry_kernel<<<1, 1024, 0, stream_>>>(r.tiles, (long long)n_tiles);
+  AB_CUDA(cudaGetLastError());
+  wf_rank_apply_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(r);
+  AB_CUDA(cudaGetLastError());
+  device_exclusive_scan(keep_.as<unsigned int>(), (int64_t)e, off2_.as<unsigned long long>(), &counters()->total, sums_,
+                        stream_);
+  st_.kernel_launches += 6;
+  unsigned long long m = 0, n_inst = 0;
+  AB_CUDA(cudaMemcpyAsync(&m, &counters()->total, 8, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaMemcpyAsync(&n_inst, &counters()->instants, 8, cudaMemcpyDeviceToHost, stream_));
+  AB_CUDA(cudaStreamSynchronize(stream_));
+
+  // the kept rows, in sorted order
+  if (m > 0) {
+    WGather g{};
+    for (int c = 0; c < n_cols_; ++c) {
+      reserve(out_[c], m * 8);
+      g.store[c] = cur_.col[c].as<unsigned long long>();
+      g.out.c[c] = out_[c].as<unsigned long long>();
+    }
+    reserve(out_fn_, m * 8);
+    g.n_cols = n_cols_;
+    g.idx = idx;
+    g.keep = keep_.as<unsigned int>();
+    g.off = off2_.as<unsigned long long>();
+    g.fn = fnv_.as<unsigned long long>();
+    g.fn_out = out_fn_.as<unsigned long long>();
+    g.n = (long long)e;
+    wf_gather_kernel<<<grid_for(e), WF_THREADS, 0, stream_>>>(g);
+    AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
+    ++st_.emit_launches;
+    std::vector<OutColumn> cols =
+        host_columns([&](int f) { return d2h_pinned(out_[f].p, (size_t)m * 8, stream_, &st_.d2h_bytes); });
+    OutColumn fc;
+    fc.name = fn_name();
+    fc.format = "L";
+    fc.data = d2h_pinned(out_fn_.p, (size_t)m * 8, stream_, &st_.d2h_bytes);
+    cols.push_back(fc);
+    out->arrays.emplace_back();
+    out->schemas.emplace_back();
+    export_batch(cols, (int64_t)m, &out->arrays.back(), &out->schemas.back());
+  }
+
+  // the rows that stay, to the front of the store
+  const uint64_t open = n - e;
+  if (open) {
+    if (!alt_.col[0].p) alloc_store(alt_, cap_);
+    WCompact p{};
+    for (int c = 0; c < n_cols_; ++c) {
+      p.from[c] = cur_.col[c].as<unsigned long long>();
+      p.to.c[c] = alt_.col[c].as<unsigned long long>();
+    }
+    p.n_cols = n_cols_;
+    p.flag = flag_.as<unsigned int>();
+    p.off = off_.as<unsigned long long>();
+    p.n = (long long)n;
+    wf_compact_kernel<<<grid_for(n), WF_THREADS, 0, stream_>>>(p);
+    AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
+    std::swap(cur_, alt_);
+  }
+  wf_set_rows_kernel<<<1, 1, 0, stream_>>>(counters(), open);
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  AB_CUDA(cudaStreamSynchronize(stream_));  // the batch's copies have completed
+  n_store_ = store_hi_ = open;
+  ckpt_from_ -= std::min<uint64_t>(ckpt_from_, below);
+  st_.rows_out += m;
+  st_.windows_out += n_inst;
+}
+
+// handle_checkpoint: table "input" gets the rows accepted since the previous checkpoint, one batch per instant in
+// ascending order, each in arrival order and in the input layout (the reference flushes the batches it inserted under
+// their instants since then).
+void WindowFnOp::handle_checkpoint(int64_t, BatchesPriv* out) {
+  set_device();
+  read_counters();
+  const uint64_t n = n_store_;
+  if (n <= ckpt_from_) return;
+  const uint64_t d = n - ckpt_from_;
+  reserve(idx_[0], d * 4);
+  wf_iota_kernel<<<grid_for(d), WF_THREADS, 0, stream_>>>(idx_[0].as<unsigned int>(), (unsigned int)ckpt_from_,
+                                                          (long long)d);
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  const unsigned int* idx = sort_rows(d, true);
+  WGather g{};
+  for (int c = 0; c < n_cols_; ++c) {
+    reserve(out_[c], d * 8);
+    g.store[c] = cur_.col[c].as<unsigned long long>();
+    g.out.c[c] = out_[c].as<unsigned long long>();
+  }
+  g.n_cols = n_cols_;
+  g.idx = idx;
+  g.n = (long long)d;
+  wf_gather_kernel<<<grid_for(d), WF_THREADS, 0, stream_>>>(g);
+  AB_CUDA(cudaGetLastError());
+  ++st_.kernel_launches;
+  // the columns once, on the host; each instant's rows are then a slice of them
+  std::vector<void*> flat(n_cols_);
+  for (int c = 0; c < n_cols_; ++c) flat[c] = d2h_pinned(out_[c].p, (size_t)d * 8, stream_, &st_.d2h_bytes);
+  AB_CUDA(cudaStreamSynchronize(stream_));
+  const uint64_t* ts = (const uint64_t*)flat[ts_col_];
+  for (uint64_t s = 0; s < d;) {
+    uint64_t e = s + 1;
+    while (e < d && ts[e] == ts[s]) ++e;
+    const std::vector<OutColumn> cols = host_columns([&](int f) {
+      void* p = PinnedPool::get().alloc((size_t)(e - s) * 8);
+      memcpy(p, (const uint64_t*)flat[f] + s, (size_t)(e - s) * 8);
+      return p;
+    });
+    out->arrays.emplace_back();
+    out->schemas.emplace_back();
+    export_batch(cols, (int64_t)(e - s), &out->arrays.back(), &out->schemas.back());
+    s = e;
+  }
+  for (void* p : flat) PinnedPool::get().free(p);
+  ckpt_from_ = n;
+}
+
+// on_start (:130-145): the batches of table "input", in any order, appended to the store ahead of any later row and not
+// late-filtered.  Every batch is checked against the input layout first: one that does not match => INVALID_ARGUMENT,
+// nothing changed.  The restored watermark is the late watermark.
+void WindowFnOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t watermark, int64_t) {
+  set_device();
+  if (n > 0) AB_REQUIRE(state != nullptr && schemas != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null state batches");
+  std::vector<std::vector<InColumn>> cols((size_t)std::max<int64_t>(n, 0));
+  std::vector<int64_t> rows(cols.size(), 0);
+  uint64_t total = 0;
+  Layout first;
+  for (size_t b = 0; b < cols.size(); ++b) {
+    std::vector<Nest> nests;
+    Layout l;
+    try {
+      cols[b] = import_batch(&state[b], &schemas[b], &rows[b], -1, &nests);
+      l = layout_of(cols[b], nests, &schemas[b]);
+      check_layout(l, ARROYO_B200_INVALID_ARGUMENT);
+    } catch (const Error& e) {
+      throw Error(ARROYO_B200_INVALID_ARGUMENT, std::string("state batch: ") + e.what());
+    }
+    if (b == 0) first = l;
+    AB_REQUIRE(l.formats == first.formats && l.nests.size() == first.nests.size(), ARROYO_B200_INVALID_ARGUMENT,
+               "state batch: layout differs from the first state batch's");
+    total += (uint64_t)rows[b];
+  }
+  if (total > 0) reserve_rows(total);  // may refuse: nothing has changed yet
+  if (n > 0) adopt(first);
+  if (total > 0) {
+    for (size_t b = 0; b < cols.size(); ++b) {
+      if (!rows[b]) continue;
+      const unsigned long long* ptrs[ARROYO_B200_MAX_COLS];
+      ingest(stage(cols[b], rows[b], ptrs), rows[b], LLONG_MIN);
+    }
+    read_counters();
+    ckpt_from_ = n_store_;  // the table already holds them
+  }
+  if (watermark != INT64_MIN) late_wm_ = std::max<int64_t>(late_wm_, watermark);
+  for (int64_t b = 0; b < n; ++b)
+    if (state[b].release) state[b].release(&state[b]);
+}
+
+}  // namespace
+
+OpBase* make_window_fn_op(const ArroyoB200OpConfig& cfg) { return new WindowFnOp(cfg); }
+
+}  // namespace ab

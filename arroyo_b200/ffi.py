@@ -14,6 +14,10 @@ MAX_COLS = 16
 OK, INVALID_ARGUMENT, UNSUPPORTED, RUNTIME, FATAL, PANIC = 0, 1, 2, 3, 4, 5
 TUMBLING_AGGREGATE, SLIDING_AGGREGATE, SESSION_AGGREGATE, INSTANT_JOIN, UPDATING_AGGREGATE, TTL_JOIN = 1, 2, 3, 4, 5, 6
 INSTANT_AGGREGATE = 7
+WINDOW_FUNCTION = 8
+FN_ROW_NUMBER, FN_RANK, FN_DENSE_RANK = 1, 2, 3
+ORDER_ASC, ORDER_DESC = 16, 17
+MAX_ORDER_KEYS = 4
 AGG_COUNT_STAR, AGG_SUM_I64, AGG_AVG_I64, AGG_MIN_I64, AGG_MAX_I64 = 1, 2, 3, 4, 5
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_FULL = 0, 1, 2, 3
 FLAG_PROFILE, FLAG_REMERGE_ONLY, FLAG_COMBINE, FLAG_AVG_F64, FLAG_NO_COMBINE, FLAG_ZERO_COPY = 1, 2, 4, 8, 16, 32
@@ -62,7 +66,7 @@ class OpConfig(C.Structure):
         ("join_type", C.c_int32), ("right_n_cols", C.c_int32), ("right_timestamp_col", C.c_int32),
         ("left_key_col", C.c_int32), ("right_key_col", C.c_int32),
         ("left_n_routing", C.c_int32), ("right_n_routing", C.c_int32),
-        ("partial_count_col_plus1", C.c_int32), ("reserved2", C.c_int32),
+        ("partial_count_col_plus1", C.c_int32), ("window_fn", C.c_int32),
         ("expected_keys", C.c_uint64), ("flags", C.c_uint32), ("reserved", C.c_uint32),
     ]
 

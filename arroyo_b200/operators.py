@@ -413,6 +413,108 @@ class InstantAggregatingWindowFunc(_WindowAggregate):
         return int(getattr(c, "nested_width", 0)) if c.final_projection else 0
 
 
+_WINDOW_FNS = {"row_number": ffi.FN_ROW_NUMBER, "rank": ffi.FN_RANK, "dense_rank": ffi.FN_DENSE_RANK}
+
+
+def flat_names(schema: pa.Schema) -> List[str]:
+    """The window function's flat columns: a struct column's children take its place as `<struct>_<child>`."""
+    names = []
+    for f in schema:
+        if pa.types.is_struct(f.type):
+            names += [f"{f.name}_{c.name}" for c in f.type]
+        else:
+            names.append(f.name)
+    return names
+
+
+class WindowFunction(_WindowAggregate):
+    """window_fn.rs: ROW_NUMBER / RANK / DENSE_RANK per instant (each upstream window stamps its rows with one
+    `_timestamp`) and partition key, with the fused `WHERE fn <= top_n`.  At watermark w every instant < w leaves in
+    one batch: the input columns, struct columns included, then the function column `config.name` (UInt64).  Columns
+    are named in the config by their flat names (`flat_names`).  Table "input" (retention 0) holds per instant the input
+    rows since the previous checkpoint.  Device-resident input is flat; a schema given at construction declares the
+    column types to the library, which device batches do not carry."""
+    kind = ffi.WINDOW_FUNCTION
+
+    def __init__(self, config, input_schema: Optional[pa.Schema] = None, **kw):
+        _NativeOperator.__init__(self, **kw)
+        self.config = config
+        self._names: Optional[List[str]] = None
+        if input_schema is not None:
+            self._build(input_schema.names, input_schema)
+
+    def name(self):
+        return "window_function"
+
+    def _build(self, names: List[str], schema: Optional[pa.Schema] = None):
+        c = self.config
+        if c.function not in _WINDOW_FNS:
+            raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, f"window function {c.function}")
+        flat = list(names) if schema is None else flat_names(schema)
+        cfg = ffi.OpConfig()
+        cfg.kind = self.kind
+        cfg.window_fn = _WINDOW_FNS[c.function]
+        cfg.n_cols = len(flat)
+        cfg.timestamp_col = flat.index(TIMESTAMP)
+        cfg.n_key_cols = 0 if c.partition_by is None else 1
+        cfg.key_col = 0 if c.partition_by is None else flat.index(c.partition_by)
+        if len(c.order_by) > ffi.MAX_ORDER_KEYS:
+            raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "more than 4 ORDER BY keys")
+        cfg.n_aggs = len(c.order_by)
+        for i, (col, desc) in enumerate(c.order_by):
+            cfg.aggs[i].kind = ffi.ORDER_DESC if desc else ffi.ORDER_ASC
+            cfg.aggs[i].input_col = flat.index(col)
+        cfg.slide_ns = int(c.top_n)
+        self._create(cfg)
+        self._names = list(names)
+        if schema is not None:
+            # a zero-row batch declares the column types (device batches carry none)
+            empty = pa.RecordBatch.from_arrays([pa.array([], f.type) for f in schema], schema=schema)
+            self._process_batch(self._lib.arroyo_b200_op_process_batch, 0, 1, empty)
+
+    def _ensure(self, schema: pa.Schema):
+        if not self.created:
+            self._build(schema.names, schema)
+
+    def output_names(self) -> List[str]:
+        return list(self._names) + [self.config.name]
+
+    def state_names(self) -> List[str]:
+        return list(self._names)
+
+    def tables(self):
+        return {"input": 0}
+
+    def on_start(self, ctx: OperatorContext):
+        wm = ctx.last_present_watermark()
+        batches = [b for _, b in ctx.table("input", 0).all_batches_for_watermark(wm)]
+        if not batches and not self.created:
+            return
+        if not self.created:
+            self._ensure(batches[0].schema)
+        self._on_start(batches, ffi.INT64_MIN if wm is None else clamp_watermark(wm), ffi.INT64_MIN)
+
+    def process_batch(self, batch: pa.RecordBatch, ctx: OperatorContext, collector: Collector):
+        self._ensure(batch.schema)
+        self._process_batch(self._lib.arroyo_b200_op_process_batch, 0, 1, batch)
+
+    def run_batches(self, exported: "ExportedBatches", watermarks, collector: Collector, first: int = 0,
+                    count: Optional[int] = None, async_emit: bool = True):
+        if not self.created:
+            raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "run_batches needs input_schema at construction")
+        super().run_batches(exported, watermarks, collector, first, count, async_emit)
+
+    def handle_checkpoint(self, barrier, ctx: OperatorContext, collector: Collector):
+        if not self.created:
+            return
+        out = ffi.Batches()
+        _check(self._lib, self._h, self._lib.arroyo_b200_op_handle_checkpoint(self._h, ffi.INT64_MIN, C.byref(out)))
+        table = ctx.table("input", 0)
+        names = self.state_names()
+        for b in import_batches(self._lib, out):
+            b = pa.RecordBatch.from_arrays(b.columns, names=names)
+            table.insert(b.column(names.index(TIMESTAMP)).cast(pa.int64())[0].as_py(), b)
+
 
 class SessionAggregatingWindowFunc(_NativeOperator):
     """arroyo-worker/src/arrow/session_aggregating_window.rs.  Output = [key cols...] with the window struct

@@ -99,7 +99,7 @@ typedef enum ArroyoB200OpKind {
                                        * INSTANT_JOIN; matches leave from arroyo_b200_op_process_batch_emit).  The shim
                                        * writes the key-time tables "left" / "right" from the input batches; a restart
                                        * hands them back through arroyo_b200_op_restore_side                           */
-  ARROYO_B200_INSTANT_AGGREGATE = 7   /* OperatorName::TumblingWindowAggregate with width_micros == 0: the instant window
+  ARROYO_B200_INSTANT_AGGREGATE = 7,  /* OperatorName::TumblingWindowAggregate with width_micros == 0: the instant window
                                        * the planner puts after an upstream window (extension/aggregate.rs:233-289).  The
                                        * bin is _timestamp itself; at watermark w every instant < w leaves in ascending
                                        * order.  Output [key?, aggregates..., _timestamp = instant], or with
@@ -107,7 +107,54 @@ typedef enum ArroyoB200OpKind {
                                        * inserted at window_index.  Checkpoints write table "t" (partial_schema, one
                                        * batch per instant, the rows since the previous checkpoint).  Host output only:
                                        * handle_watermark_device* => ARROYO_B200_UNSUPPORTED                           */
+  ARROYO_B200_WINDOW_FUNCTION = 8     /* OperatorName::WindowFunction: WindowFunctionOperator, arroyo-worker/src/arrow/
+                                       * window_fn.rs -- ROW_NUMBER / RANK / DENSE_RANK () OVER (PARTITION BY window
+                                       * [, key] ORDER BY ...), optionally fused with the filter `fn <= N` after it.
+                                       * Config:
+                                       *  - window_fn: ArroyoB200WindowFn; anything else => INVALID_ARGUMENT;
+                                       *  - n_key_cols / key_col: the PARTITION BY column besides the window (the planner
+                                       *    drops `window`, each upstream window stamping its rows with one _timestamp,
+                                       *    plan/window_fn.rs:101-105): 0 or 1, of type l, L or tsn:; 2 or more =>
+                                       *    UNSUPPORTED;
+                                       *  - n_aggs / aggs[]: the ORDER BY list, 1 to 4 entries {ARROYO_B200_ORDER_ASC |
+                                       *    _DESC, input_col} of type l, L or tsn: (a g column => UNSUPPORTED, as
+                                       *    DataFusion's float ordering and peers are not pinned here); 0 or more than 4
+                                       *    entries, or another kind code => INVALID_ARGUMENT;
+                                       *  - slide_ns: N of a fused `WHERE fn <= N` (`fn = 1` is the same as `<= 1` for all
+                                       *    three functions); 0 = every row leaves; < 0 => INVALID_ARGUMENT;
+                                       *  - n_cols / timestamp_col / key_col / input_col count FLAT columns: a host batch's
+                                       *    struct columns (the upstream window{start, end}, children all 64-bit) are
+                                       *    flattened in place, one level, for this kind only.
+                                       * Columns pass through as raw 64 bits.  Device batches carry no types: the column
+                                       * types are those of the first host or state batch (a zero-row host batch may
+                                       * declare them), Int64 until then; a later batch of other types =>
+                                       * INVALID_ARGUMENT.
+                                       * Rows: _timestamp < the last watermark => late, dropped (filter_by_time keeps
+                                       * ts >= w, arroyo-rpc/src/df.rs:211-231); a negative _timestamp => PANIC.
+                                       * Watermark w: every instant < w leaves in ascending order (window_fn.rs:178-201),
+                                       * in ONE batch per emission, rows ordered by (instant, partition key ASC, ORDER BY
+                                       * keys); ties on every key by arrival order, restored rows first (DataFusion's sort
+                                       * promises no order there; RANK and DENSE_RANK do not depend on it).  Output = the
+                                       * input columns (struct columns re-nested as the host batches had them) then the
+                                       * function as UInt64 (L).  Host output only: handle_watermark_device* =>
+                                       * UNSUPPORTED.
+                                       * Checkpoints write table "input" (retention 0): per open instant one batch of the
+                                       * rows accepted since the previous checkpoint, in the input layout, in arrival
+                                       * order.  on_start takes such batches in any order, does not late-filter them,
+                                       * and the restored watermark becomes the late watermark.  More than 2^31 buffered
+                                       * rows => RUNTIME, nothing changed.  Stats: rows_in, rows_late, rows_out (after
+                                       * the fused filter), windows_out (instants emitted).                             */
 } ArroyoB200OpKind;
+
+/* WINDOW_FUNCTION: the function (config field `window_fn`) and the ORDER BY directions (`aggs[].kind`) */
+typedef enum ArroyoB200WindowFn {
+  ARROYO_B200_FN_ROW_NUMBER = 1,
+  ARROYO_B200_FN_RANK = 2,
+  ARROYO_B200_FN_DENSE_RANK = 3
+} ArroyoB200WindowFn;
+#define ARROYO_B200_ORDER_ASC 16
+#define ARROYO_B200_ORDER_DESC 17
+#define ARROYO_B200_MAX_ORDER_KEYS 4
 
 typedef enum ArroyoB200AggKind {
   ARROYO_B200_AGG_COUNT_STAR = 1, /* count(Int64(1)) -> Int64                          */
@@ -188,7 +235,7 @@ typedef struct ArroyoB200OpConfig {
    * 1 + the index of the input column that carries the row count.  SUM / MIN / MAX then merge the
    * upstream partial columns, COUNT(*) and AVG use the carried count. */
   int32_t partial_count_col_plus1;
-  int32_t reserved2;
+  int32_t window_fn;        /* WINDOW_FUNCTION: ArroyoB200WindowFn; every other kind ignores it */
 
   uint64_t expected_keys;   /* capacity hint for the key dictionary (0 = default)         */
   uint32_t flags;           /* ARROYO_B200_FLAG_*                                         */

@@ -1,0 +1,128 @@
+"""Emission time of the window function (WindowFunction) behind the sliding aggregate, timed on one GPU.
+
+The sliding aggregate has the benchmark's sliding shape (SUM and AVG of an Int64 value over 2^20 keys, 10 s window,
+1 s slide, one row per key per slide).  Each slide's window goes device-resident (handle_watermark_device) into two
+window functions, ROW_NUMBER() OVER (PARTITION BY window ORDER BY sum DESC, key DESC) with top_n = 1 and with
+top_n = 0 (every row leaves).  Per slide, after warm-up:
+
+  sliding_emit_ms   the sliding aggregate's device-resident emission of the slide
+  wf_top1_ms        the window function's process_device_batch + handle_watermark with top_n = 1, host output included
+  wf_all_ms         the same with top_n = 0 (2^20 rows leave to the host)
+
+Each is timed with CUDA events on the operators' stream around the calls (every handle_watermark ends in a stream
+synchronise); the medians are reported, with the sorted rows per second of each window function.  Prints one JSON
+line with the card's name and power limit.
+
+    python tools/window_fn_rates.py [--scale S] [--slides K]
+
+--scale S divides the key count by 2^S (a quick rehearsal of the script)."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+SEC = 1_000_000_000
+T0 = 1_700_000_000 * SEC
+TS = "_timestamp"
+
+
+def card():
+    import torch
+    name = torch.cuda.get_device_name(0)
+    try:
+        limit = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader"],
+                               capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        limit = "unknown"
+    return {"gpu": name, "power_limit": limit}
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--scale", type=int, default=0, help="divide the key count by 2^S (0..16)")
+    ap.add_argument("--slides", type=int, default=20, help="timed slides after the 12 warm-up slides")
+    a = ap.parse_args()
+    if not 0 <= a.scale <= 16 or a.slides < 1:
+        ap.error("--scale must be in [0, 16] and --slides >= 1")
+    import pyarrow as pa
+    import torch
+
+    import arroyo_b200 as ab
+    from arroyo_b200 import config, operators as native
+    if not torch.cuda.is_available():
+        raise SystemExit("window_fn_rates needs a CUDA device")
+    keys = 1 << (20 - a.scale)
+    stream = torch.cuda.Stream()
+    ts_t = pa.timestamp("ns")
+    s_cfg = config.WindowAggConfig(width=10 * SEC, slide=SEC, key_names=["key"],
+                                   aggs=[config.Agg("sum", "v", "s"), config.Agg("avg", "v", "av")], window_index=1)
+    sliding = native.SlidingAggregatingWindowFunc(
+        s_cfg, input_schema=pa.schema([("key", pa.int64()), ("v", pa.int64()), (TS, ts_t)]), expected_keys=keys,
+        stream=stream.cuda_stream)
+    w_schema = pa.schema([("key", pa.int64()), ("window_start", ts_t), ("window_end", ts_t), ("s", pa.int64()),
+                          ("av", pa.float64()), (TS, ts_t)])
+    fns = {}
+    for what, top_n in (("top1", 1), ("all", 0)):
+        w_cfg = config.WindowFunctionConfig("row_number", None, [("s", True), ("key", True)], "rn", top_n)
+        fns[what] = native.WindowFunction(w_cfg, input_schema=w_schema, stream=stream.cuda_stream)
+    ctxs = {w: ab.OperatorContext(1) for w in fns}
+    rng = np.random.default_rng(7)
+    warm = 12
+    times = {"sliding_emit_ms": [], "wf_top1_ms": [], "wf_all_ms": []}
+    rows_out = {"top1": 0, "all": 0}
+    window_rows = []
+
+    def timed(f):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        r = f()
+        e1.record(stream)
+        e1.synchronize()
+        return r, e0.elapsed_time(e1)
+
+    with torch.cuda.stream(stream):
+        for step in range(warm + a.slides):
+            k = torch.from_numpy(rng.permutation(keys).astype(np.int64)).cuda()
+            v = torch.from_numpy(rng.integers(-1000, 1000, keys).astype(np.int64)).cuda()
+            ts = torch.from_numpy(T0 + step * SEC + rng.integers(0, SEC, keys).astype(np.int64)).cuda()
+            stream.synchronize()
+            sliding.process_device_batch([k.data_ptr(), v.data_ptr(), ts.data_ptr()], keys)
+            wm = T0 + step * SEC
+            wins, t_s = timed(lambda: sliding.handle_watermark_device(wm))
+            n_rows = sum(n for n, _ in wins)
+            for what, op in fns.items():
+                def call():
+                    for n, ptrs in wins:
+                        op.process_device_batch(ptrs, n)
+                    col = ab.Collector()
+                    ctxs[what].watermarks.set(0, wm)
+                    op.handle_watermark(wm, ctxs[what], col)
+                    return sum(b.num_rows for b in col.batches)
+                out, t_w = timed(call)
+                if step >= warm:
+                    times[f"wf_{what}_ms"].append(t_w)
+                    rows_out[what] += out
+            if step >= warm:
+                times["sliding_emit_ms"].append(t_s)
+                window_rows.append(n_rows)
+    med = {k: float(np.median(v)) for k, v in times.items()}
+    rows = float(np.median(window_rows))
+    res = {**card(), "keys": keys, "slides": a.slides, "window_rows": int(rows),
+           **{k: round(v, 3) for k, v in med.items()},
+           "wf_top1_sorted_rows_per_s": round(rows / (med["wf_top1_ms"] / 1e3)),
+           "wf_all_sorted_rows_per_s": round(rows / (med["wf_all_ms"] / 1e3)),
+           "rows_out_top1": rows_out["top1"], "rows_out_all": rows_out["all"]}
+    print(json.dumps(res), flush=True)
+    sliding.close()
+    for op in fns.values():
+        op.close()
+
+
+if __name__ == "__main__":
+    main()
