@@ -60,12 +60,14 @@ class JoinConfig:
 
 @dataclass
 class WindowFunctionConfig:
-    """WindowFunctionOperator (arroyo-worker/src/arrow/window_fn.rs): `function` (row_number | rank | dense_rank)
-    OVER (PARTITION BY window [, `partition_by`] ORDER BY `order_by`), the function column named `name`.  `order_by`
-    is a list of (column, descending).  `top_n` > 0 fuses the `WHERE name <= top_n` that follows the operator; 0 lets
-    every row through."""
+    """WindowFunctionOperator (arroyo-worker/src/arrow/window_fn.rs): `function` (row_number | rank | dense_rank,
+    or the aggregate sum | count | avg | min | max of column `argument`, which count ignores) OVER (PARTITION BY
+    window [, `partition_by`] ORDER BY `order_by`), the function column named `name`.  `order_by` is a list of
+    (column, descending); it may be empty for an aggregate, whose frame is then the whole partition.  `top_n` > 0
+    fuses the `WHERE name <= top_n` that follows a ranking function; 0 lets every row through."""
     function: str
     partition_by: Optional[str]
     order_by: List[tuple]
     name: str
     top_n: int = 0
+    argument: Optional[str] = None

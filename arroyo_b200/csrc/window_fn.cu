@@ -1,6 +1,7 @@
 // Window function on sm_90a (H100): the GPU side of `WindowFunctionOperator` (arroyo-worker/src/arrow/window_fn.rs),
 // for ROW_NUMBER / RANK / DENSE_RANK () OVER (PARTITION BY window [, key] ORDER BY k1 [DESC], ...), optionally fused
-// with the `WHERE fn <= N` that usually follows it (top N per window).  The planner (plan/window_fn.rs:101-105) drops
+// with the `WHERE fn <= N` that usually follows it (top N per window), and for COUNT(*) / SUM / AVG / MIN / MAX (x)
+// OVER (PARTITION BY window [, key] [ORDER BY ...]) over the default frame.  The planner (plan/window_fn.rs:101-105) drops
 // the `window` column from PARTITION BY: each upstream window stamps its rows with one `_timestamp`, so the rows are
 // bucketed by `_timestamp` ("instant") and the remaining PARTITION BY column, if any, splits each instant further.
 //
@@ -16,8 +17,10 @@
 //           flipped for signed types, all bits complemented for DESC).  A rank pass flags segment starts (instant,
 //           partition) and peer starts (every sort key) and scans them, ballots within a warp and a two-level scan
 //           across 1024-row tiles: ROW_NUMBER = position in the segment + 1, RANK = position of the first peer + 1,
-//           DENSE_RANK = peer starts in the segment so far.  The fused filter, a compaction and a gather of every column
-//           write the output in sorted order; the rows that stay are compacted to the front of the store, in arrival
+//           DENSE_RANK = peer starts in the segment so far.  An aggregate adds a segmented scan of its argument with the
+//           same tiling, read at each peer group's last row (see "aggregates" below).  The fused filter, a compaction
+//           and a gather of every column write the output in sorted order; the rows that stay are compacted to the front
+//           of the store, in arrival
 //           order, so device memory tracks the open rows;
 //   state   table "input": a checkpoint writes the rows accepted since the previous one (one store index marks them,
 //           re-based when the store is compacted), one batch per instant, in the input layout.  on_start appends the
@@ -140,11 +143,12 @@ __global__ void wf_key_kernel(const unsigned long long* __restrict__ col, const 
 // of them when none starts in it).  A segment start is always a peer start.
 struct RankVal {
   unsigned int seg, peer, dcnt;
+  __device__ static RankVal zero() { return {0u, 0u, 0u}; }
 };
-__device__ __forceinline__ RankVal rv_combine(RankVal a, RankVal b) {
+__device__ __forceinline__ RankVal combine(RankVal a, RankVal b) {
   return {b.seg ? b.seg : a.seg, b.peer ? b.peer : a.peer, b.seg ? b.dcnt : a.dcnt + b.dcnt};
 }
-__device__ __forceinline__ RankVal rv_shfl_up(RankVal v, int o) {
+__device__ __forceinline__ RankVal shfl_up(RankVal v, int o) {
   return {__shfl_up_sync(FULL, v.seg, o), __shfl_up_sync(FULL, v.peer, o), __shfl_up_sync(FULL, v.dcnt, o)};
 }
 
@@ -167,13 +171,13 @@ __device__ __forceinline__ RankVal tile_inclusive(unsigned int bits, long long j
   if (w == 0) {
     RankVal x = s_warp[lane];
     for (int o = 1; o < 32; o <<= 1) {
-      const RankVal y = rv_shfl_up(x, o);
-      if ((int)lane >= o) x = rv_combine(y, x);
+      const RankVal y = shfl_up(x, o);
+      if ((int)lane >= o) x = combine(y, x);
     }
     s_warp[lane] = x;
   }
   __syncthreads();
-  if (w > 0) v = rv_combine(s_warp[w - 1], v);
+  if (w > 0) v = combine(s_warp[w - 1], v);
   *total = s_warp[WF_TILE / 32 - 1];
   return v;
 }
@@ -185,7 +189,7 @@ struct WRank {
   const unsigned int* idx;  // sorted
   long long n;
   unsigned char* bits;  // per sorted row: 1 = instant start, 2 = segment start, 4 = peer start
-  RankVal* tiles;       // per tile: its total, then (wf_rank_carry_kernel) the scan of the tiles before it
+  RankVal* tiles;       // per tile: its total, then (wf_carry_kernel) the scan of the tiles before it
   unsigned long long* instants;
   int fn;
   long long top_n;
@@ -218,40 +222,42 @@ __global__ void __launch_bounds__(WF_TILE) wf_rank_flags_kernel(const __grid_con
   if (threadIdx.x == 0) p.tiles[blockIdx.x] = total;
 }
 
-// pass 2, one block: tiles[t] becomes the exclusive scan of the totals of tiles [0, t), 1024 tiles per round
-__global__ void __launch_bounds__(1024) wf_rank_carry_kernel(RankVal* tiles, long long n_tiles) {
-  __shared__ RankVal s_warp[32];
-  __shared__ RankVal s_carry;
+// pass 2, one block: tiles[t] becomes the exclusive scan of the totals of tiles [0, t), 1024 tiles per round.  T is a
+// scan element with combine / shfl_up overloads and an identity T::zero() (RankVal, AggVal).
+template <class T>
+__global__ void __launch_bounds__(1024) wf_carry_kernel(T* tiles, long long n_tiles) {
+  __shared__ T s_warp[32];
+  __shared__ T s_carry;
   const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const RankVal zero = {0u, 0u, 0u};
+  const T zero = T::zero();
   if (threadIdx.x == 0) s_carry = zero;
   __syncthreads();
   for (long long base = 0; base < n_tiles; base += 1024) {
     const long long i = base + threadIdx.x;
-    const RankVal v = i < n_tiles ? tiles[i] : zero;
-    RankVal x = v;
+    const T v = i < n_tiles ? tiles[i] : zero;
+    T x = v;
     for (int o = 1; o < 32; o <<= 1) {
-      const RankVal y = rv_shfl_up(x, o);
-      if ((int)lane >= o) x = rv_combine(y, x);
+      const T y = shfl_up(x, o);
+      if ((int)lane >= o) x = combine(y, x);
     }
-    RankVal ex = rv_shfl_up(x, 1);  // exclusive within the warp
+    T ex = shfl_up(x, 1);  // exclusive within the warp
     if (lane == 0) ex = zero;
     if (lane == 31) s_warp[w] = x;
     __syncthreads();
     if (w == 0) {
-      RankVal t = s_warp[lane];
+      T t = s_warp[lane];
       for (int o = 1; o < 32; o <<= 1) {
-        const RankVal y = rv_shfl_up(t, o);
-        if ((int)lane >= o) t = rv_combine(y, t);
+        const T y = shfl_up(t, o);
+        if ((int)lane >= o) t = combine(y, t);
       }
       s_warp[lane] = t;  // inclusive over warps
     }
     __syncthreads();
-    const RankVal carry = s_carry;
-    RankVal before = w > 0 ? rv_combine(carry, s_warp[w - 1]) : carry;
-    if (i < n_tiles) tiles[i] = rv_combine(before, ex);
+    const T carry = s_carry;
+    T before = w > 0 ? combine(carry, s_warp[w - 1]) : carry;
+    if (i < n_tiles) tiles[i] = combine(before, ex);
     __syncthreads();
-    if (threadIdx.x == 0) s_carry = rv_combine(carry, s_warp[31]);
+    if (threadIdx.x == 0) s_carry = combine(carry, s_warp[31]);
     __syncthreads();
   }
 }
@@ -263,7 +269,7 @@ __global__ void __launch_bounds__(WF_TILE) wf_rank_apply_kernel(const __grid_con
   RankVal total;
   const RankVal v = tile_inclusive(bits, j, &total);
   if (j >= p.n) return;
-  const RankVal s = rv_combine(p.tiles[blockIdx.x], v);
+  const RankVal s = combine(p.tiles[blockIdx.x], v);
   unsigned long long f;
   if (p.fn == ARROYO_B200_FN_ROW_NUMBER) f = (unsigned long long)(j + 2) - s.seg;
   else if (p.fn == ARROYO_B200_FN_RANK) f = (unsigned long long)(s.peer - s.seg) + 1ull;
@@ -272,7 +278,158 @@ __global__ void __launch_bounds__(WF_TILE) wf_rank_apply_kernel(const __grid_con
   p.keep[j] = (p.top_n == 0 || f <= (unsigned long long)p.top_n) ? 1u : 0u;
 }
 
-// out[c][o] = store[c][idx[j]] for the kept rows (keep null: every row, o = j), and the function column
+// ---- aggregates -------------------------------------------------------------------------------------------------------
+// SUM / COUNT / AVG / MIN / MAX over the default frame: from the segment start through the row's last peer (without
+// ORDER BY every row of a segment is a peer).  A segmented inclusive scan of the argument over the sorted rows, reset at
+// segment starts, gives each peer group's last row its frame's value; that row writes it at the group's first row, and
+// the gather reads it there for every row of the group.  AggOp<K>: the scan's value, identity and operator, the
+// argument's value for a row, and the function value from the frame's scan value and row count (AVG: the f64 sum over
+// the count; COUNT scans ones).
+template <int K> struct AggOp;
+template <> struct AggOp<ARROYO_B200_AGG_COUNT_STAR> {
+  using V = unsigned long long;
+  __device__ static V identity() { return 0ull; }
+  __device__ static V op(V a, V b) { return a + b; }
+  __device__ static V load(const unsigned long long*, unsigned int) { return 1ull; }
+  __device__ static unsigned long long result(V v, unsigned long long) { return v; }
+};
+template <> struct AggOp<ARROYO_B200_AGG_SUM_I64> {
+  using V = unsigned long long;  // wrapping
+  __device__ static V identity() { return 0ull; }
+  __device__ static V op(V a, V b) { return a + b; }
+  __device__ static V load(const unsigned long long* arg, unsigned int i) { return arg[i]; }
+  __device__ static unsigned long long result(V v, unsigned long long) { return v; }
+};
+template <> struct AggOp<ARROYO_B200_AGG_MIN_I64> {
+  using V = long long;
+  __device__ static V identity() { return LLONG_MAX; }
+  __device__ static V op(V a, V b) { return a < b ? a : b; }
+  __device__ static V load(const unsigned long long* arg, unsigned int i) { return (long long)arg[i]; }
+  __device__ static unsigned long long result(V v, unsigned long long) { return (unsigned long long)v; }
+};
+template <> struct AggOp<ARROYO_B200_AGG_MAX_I64> {
+  using V = long long;
+  __device__ static V identity() { return LLONG_MIN; }
+  __device__ static V op(V a, V b) { return a > b ? a : b; }
+  __device__ static V load(const unsigned long long* arg, unsigned int i) { return (long long)arg[i]; }
+  __device__ static unsigned long long result(V v, unsigned long long) { return (unsigned long long)v; }
+};
+template <> struct AggOp<ARROYO_B200_AGG_AVG_I64> {
+  using V = double;
+  __device__ static V identity() { return 0.0; }
+  __device__ static V op(V a, V b) { return a + b; }
+  __device__ static V load(const unsigned long long* arg, unsigned int i) { return (double)(long long)arg[i]; }
+  __device__ static unsigned long long result(V v, unsigned long long n) {
+    return (unsigned long long)__double_as_longlong(v / (double)n);
+  }
+};
+
+// The scan element: seg = a segment starts in the range, v = the operator over the range's rows from its last segment
+// start on (all of them when none starts in it).
+template <int K>
+struct AggVal {
+  unsigned int seg;
+  typename AggOp<K>::V v;
+  __device__ static AggVal zero() { return {0u, AggOp<K>::identity()}; }
+};
+template <int K>
+__device__ __forceinline__ AggVal<K> combine(AggVal<K> a, AggVal<K> b) {
+  return {a.seg | b.seg, b.seg ? b.v : AggOp<K>::op(a.v, b.v)};
+}
+template <int K>
+__device__ __forceinline__ AggVal<K> shfl_up(AggVal<K> x, int o) {
+  return {__shfl_up_sync(FULL, x.seg, o), __shfl_up_sync(FULL, x.v, o)};  // a 64-bit v moves as two 32-bit shuffles
+}
+
+struct WAgg {
+  const unsigned long long* arg;  // the argument column (COUNT: unused)
+  const unsigned int* idx;        // sorted
+  const unsigned char* bits;      // wf_rank_flags_kernel's starts
+  long long n;
+  const RankVal* rank_tiles;      // after wf_carry_kernel<RankVal>
+  void* tiles;                    // AggVal<K> per tile: its total, then the scan of the tiles before it
+  unsigned long long* fv;         // at each peer group's first sorted row: the group's function value
+  unsigned int* at;               // per sorted row: its peer group's first sorted row
+};
+
+template <int K>
+__device__ __forceinline__ AggVal<K> agg_element(const WAgg& p, long long j, unsigned int bits) {
+  AggVal<K> x = AggVal<K>::zero();
+  if (j < p.n) {
+    x.seg = (bits >> 1) & 1u;
+    x.v = AggOp<K>::load(p.arg, p.idx[j]);
+  }
+  return x;
+}
+
+// Inclusive segmented scan of one tile of WF_TILE rows (one per thread); the tile's total goes to `*total`.  Every
+// thread of the block calls it.
+template <int K>
+__device__ __forceinline__ AggVal<K> agg_tile_inclusive(AggVal<K> x, AggVal<K>* total) {
+  __shared__ AggVal<K> s_warp[WF_TILE / 32];
+  const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int o = 1; o < 32; o <<= 1) {
+    const AggVal<K> y = shfl_up(x, o);
+    if ((int)lane >= o) x = combine(y, x);
+  }
+  if (lane == 31) s_warp[w] = x;
+  __syncthreads();
+  if (w == 0) {
+    AggVal<K> t = s_warp[lane];
+    for (int o = 1; o < 32; o <<= 1) {
+      const AggVal<K> y = shfl_up(t, o);
+      if ((int)lane >= o) t = combine(y, t);
+    }
+    s_warp[lane] = t;
+  }
+  __syncthreads();
+  if (w > 0) x = combine(s_warp[w - 1], x);
+  *total = s_warp[WF_TILE / 32 - 1];
+  return x;
+}
+
+// pass 1: each tile's total
+template <int K>
+__global__ void __launch_bounds__(WF_TILE) wf_agg_tiles_kernel(const __grid_constant__ WAgg p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  const unsigned int bits = j < p.n ? p.bits[j] : 0u;
+  AggVal<K> total;
+  agg_tile_inclusive<K>(agg_element<K>(p, j, bits), &total);
+  if (threadIdx.x == 0) static_cast<AggVal<K>*>(p.tiles)[blockIdx.x] = total;
+}
+
+// pass 3 (after wf_carry_kernel over the tiles): each row's peer group, and at each group's last row the frame's
+// value, written at the group's first row
+template <int K>
+__global__ void __launch_bounds__(WF_TILE) wf_agg_apply_kernel(const __grid_constant__ WAgg p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  const unsigned int bits = j < p.n ? p.bits[j] : 0u;
+  RankVal rt;
+  const RankVal rv = tile_inclusive(bits, j, &rt);
+  AggVal<K> at;
+  const AggVal<K> av = agg_tile_inclusive<K>(agg_element<K>(p, j, bits), &at);
+  if (j >= p.n) return;
+  const RankVal r = combine(p.rank_tiles[blockIdx.x], rv);
+  const AggVal<K> s = combine(static_cast<const AggVal<K>*>(p.tiles)[blockIdx.x], av);
+  const unsigned int first = r.peer - 1u;
+  p.at[j] = first;
+  if (j + 1 == p.n || (p.bits[j + 1] & 4u))
+    p.fv[first] = AggOp<K>::result(s.v, (unsigned long long)(j + 2) - r.seg);
+}
+
+template <int K>
+void launch_aggregate(const WAgg& p, uint64_t n_tiles, cudaStream_t stream) {
+  static_assert(sizeof(AggVal<K>) == 16, "WindowFnOp::aggregate sizes the tile totals for 16 bytes");
+  wf_agg_tiles_kernel<K><<<(unsigned)n_tiles, WF_TILE, 0, stream>>>(p);
+  AB_CUDA(cudaGetLastError());
+  wf_carry_kernel<AggVal<K>><<<1, 1024, 0, stream>>>(static_cast<AggVal<K>*>(p.tiles), (long long)n_tiles);
+  AB_CUDA(cudaGetLastError());
+  wf_agg_apply_kernel<K><<<(unsigned)n_tiles, WF_TILE, 0, stream>>>(p);
+  AB_CUDA(cudaGetLastError());
+}
+
+// out[c][o] = store[c][idx[j]] for the kept rows (keep null: every row, o = j), and the function column: fn[j], or
+// fn[at[j]] when `at` is given
 struct WGather {
   const unsigned long long* store[ARROYO_B200_MAX_COLS];
   WCols out;
@@ -281,6 +438,7 @@ struct WGather {
   const unsigned int* keep;
   const unsigned long long* off;
   const unsigned long long* fn;
+  const unsigned int* at;
   unsigned long long* fn_out;
   long long n;
 };
@@ -292,7 +450,7 @@ __global__ void __launch_bounds__(WF_THREADS) wf_gather_kernel(const __grid_cons
     const unsigned long long o = p.keep ? p.off[j] : (unsigned long long)j;
     const unsigned int src = p.idx[j];
     for (int c = 0; c < p.n_cols; ++c) p.out.c[c][o] = p.store[c][src];
-    if (p.fn_out) p.fn_out[o] = p.fn[j];
+    if (p.fn_out) p.fn_out[o] = p.fn[p.at ? p.at[j] : (unsigned int)j];
   }
 }
 
@@ -352,6 +510,7 @@ class WindowFnOp final : public OpBase {
     std::vector<Nest> nests;
   };
   int n_cols_ = 0, ts_col_ = 0, key_col_ = -1, fn_ = 0;
+  int agg_kind_ = 0, agg_col_ = -1;  // FN_AGGREGATE: the aggregate and its argument column (COUNT: none)
   int n_order_ = 0, order_col_[ARROYO_B200_MAX_ORDER_KEYS] = {}, order_desc_[ARROYO_B200_MAX_ORDER_KEYS] = {};
   int64_t top_n_ = 0;
   Layout layout_;
@@ -364,7 +523,7 @@ class WindowFnOp final : public OpBase {
   uint64_t ckpt_from_ = 0; // rows [ckpt_from_, n) arrived since the last checkpoint
   DevBuf counters_, stage_;
   uint64_t stage_cap_ = 0;
-  DevBuf flag_, off_, sums_, idx_[2], key_[2], cub_tmp_, bits_, tiles_, fnv_, keep_, off2_;
+  DevBuf flag_, off_, sums_, idx_[2], key_[2], cub_tmp_, bits_, tiles_, fnv_, keep_, off2_, agg_tiles_, at_;
   DevBuf out_[ARROYO_B200_MAX_COLS], out_fn_;
   ArroyoB200Stats st_{};
 
@@ -373,8 +532,20 @@ class WindowFnOp final : public OpBase {
   }
   WCounters* counters() const { return counters_.as<WCounters>(); }
   const char* fn_name() const {
+    if (fn_ == ARROYO_B200_FN_AGGREGATE)
+      return agg_kind_ == ARROYO_B200_AGG_COUNT_STAR ? "count"
+             : agg_kind_ == ARROYO_B200_AGG_SUM_I64  ? "sum"
+             : agg_kind_ == ARROYO_B200_AGG_AVG_I64  ? "avg"
+             : agg_kind_ == ARROYO_B200_AGG_MIN_I64  ? "min"
+                                                     : "max";
     return fn_ == ARROYO_B200_FN_ROW_NUMBER ? "row_number" : fn_ == ARROYO_B200_FN_RANK ? "rank" : "dense_rank";
   }
+  // ranks are UInt64; count / sum / min / max Int64, avg Float64
+  const char* fn_format() const {
+    if (fn_ != ARROYO_B200_FN_AGGREGATE) return "L";
+    return agg_kind_ == ARROYO_B200_AGG_AVG_I64 ? "g" : "l";
+  }
+  void aggregate(const WRank& r, uint64_t n_tiles);
   Layout layout_of(const std::vector<InColumn>& cols, const std::vector<Nest>& nests, const ArrowSchema* s) const;
   void check_layout(const Layout& l, int bad_type_status) const;
   void adopt(const Layout& l);
@@ -392,9 +563,11 @@ WindowFnOp::WindowFnOp(const ArroyoB200OpConfig& c) {
   cfg = c;
   name = "window_function";
   AB_REQUIRE(c.window_fn == ARROYO_B200_FN_ROW_NUMBER || c.window_fn == ARROYO_B200_FN_RANK ||
-                 c.window_fn == ARROYO_B200_FN_DENSE_RANK,
-             ARROYO_B200_INVALID_ARGUMENT, "window function: window_fn must be ROW_NUMBER (1), RANK (2) or DENSE_RANK (3)");
+                 c.window_fn == ARROYO_B200_FN_DENSE_RANK || c.window_fn == ARROYO_B200_FN_AGGREGATE,
+             ARROYO_B200_INVALID_ARGUMENT,
+             "window function: window_fn must be ROW_NUMBER (1), RANK (2), DENSE_RANK (3) or AGGREGATE (4)");
   fn_ = c.window_fn;
+  const bool agg = fn_ == ARROYO_B200_FN_AGGREGATE;
   AB_REQUIRE(c.n_cols >= 1 && c.n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad n_cols");
   n_cols_ = c.n_cols;
   AB_REQUIRE(c.timestamp_col >= 0 && c.timestamp_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT, "bad timestamp_col");
@@ -406,19 +579,40 @@ WindowFnOp::WindowFnOp(const ArroyoB200OpConfig& c) {
     AB_REQUIRE(c.key_col >= 0 && c.key_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT, "bad key_col");
     key_col_ = c.key_col;
   }
-  AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= ARROYO_B200_MAX_ORDER_KEYS, ARROYO_B200_INVALID_ARGUMENT,
-             "window function: ORDER BY takes 1 to 4 keys (n_aggs)");
-  n_order_ = c.n_aggs;
-  for (int k = 0; k < n_order_; ++k) {
-    AB_REQUIRE(c.aggs[k].kind == ARROYO_B200_ORDER_ASC || c.aggs[k].kind == ARROYO_B200_ORDER_DESC,
-               ARROYO_B200_INVALID_ARGUMENT, "window function: an ORDER BY key's kind is ORDER_ASC (16) or ORDER_DESC (17)");
-    AB_REQUIRE(c.aggs[k].input_col >= 0 && c.aggs[k].input_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT,
-               "window function: ORDER BY column out of range");
-    order_col_[k] = c.aggs[k].input_col;
-    order_desc_[k] = c.aggs[k].kind == ARROYO_B200_ORDER_DESC;
+  if (agg) {
+    // aggs[0] is the aggregate, aggs[1 ..] the ORDER BY keys
+    AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= 1 + ARROYO_B200_MAX_ORDER_KEYS, ARROYO_B200_INVALID_ARGUMENT,
+               "window function: an aggregate takes itself and 0 to 4 ORDER BY keys (n_aggs 1 to 5)");
+    agg_kind_ = c.aggs[0].kind;
+    AB_REQUIRE(agg_kind_ == ARROYO_B200_AGG_COUNT_STAR || agg_kind_ == ARROYO_B200_AGG_SUM_I64 ||
+                   agg_kind_ == ARROYO_B200_AGG_AVG_I64 || agg_kind_ == ARROYO_B200_AGG_MIN_I64 ||
+                   agg_kind_ == ARROYO_B200_AGG_MAX_I64,
+               ARROYO_B200_INVALID_ARGUMENT,
+               "window function: aggs[0] of an aggregate is COUNT_STAR, SUM_I64, AVG_I64, MIN_I64 or MAX_I64");
+    if (agg_kind_ != ARROYO_B200_AGG_COUNT_STAR) {
+      AB_REQUIRE(c.aggs[0].input_col >= 0 && c.aggs[0].input_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT,
+                 "window function: aggregate argument column out of range");
+      agg_col_ = c.aggs[0].input_col;
+    }
+    AB_REQUIRE(c.slide_ns == 0, ARROYO_B200_INVALID_ARGUMENT,
+               "window function: an aggregate takes no top N filter (slide_ns must be 0)");
+  } else {
+    AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= ARROYO_B200_MAX_ORDER_KEYS, ARROYO_B200_INVALID_ARGUMENT,
+               "window function: ORDER BY takes 1 to 4 keys (n_aggs)");
+    AB_REQUIRE(c.slide_ns >= 0, ARROYO_B200_INVALID_ARGUMENT, "window function: top N (slide_ns) must be >= 0");
+    top_n_ = c.slide_ns;
   }
-  AB_REQUIRE(c.slide_ns >= 0, ARROYO_B200_INVALID_ARGUMENT, "window function: top N (slide_ns) must be >= 0");
-  top_n_ = c.slide_ns;
+  const int first_key = agg ? 1 : 0;
+  n_order_ = c.n_aggs - first_key;
+  for (int k = 0; k < n_order_; ++k) {
+    const ArroyoB200Agg& a = c.aggs[first_key + k];
+    AB_REQUIRE(a.kind == ARROYO_B200_ORDER_ASC || a.kind == ARROYO_B200_ORDER_DESC, ARROYO_B200_INVALID_ARGUMENT,
+               "window function: an ORDER BY key's kind is ORDER_ASC (16) or ORDER_DESC (17)");
+    AB_REQUIRE(a.input_col >= 0 && a.input_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT,
+               "window function: ORDER BY column out of range");
+    order_col_[k] = a.input_col;
+    order_desc_[k] = a.kind == ARROYO_B200_ORDER_DESC;
+  }
   for (int f = 0; f < n_cols_; ++f) {
     layout_.names.push_back(f == ts_col_ ? "_timestamp" : "c" + std::to_string(f));
     layout_.formats.push_back(f == ts_col_ ? "tsn:" : "l");
@@ -448,12 +642,16 @@ WindowFnOp::Layout WindowFnOp::layout_of(const std::vector<InColumn>& cols, cons
   return l;
 }
 
-// A batch's layout against the plan: its column count and the sort keys' types (`bad_type_status` when a key's type is
-// not l, L or tsn:), and, once the operator has its types, the same formats and struct columns.
+// A batch's layout against the plan: its column count, the sort keys' types (`bad_type_status` when a key's type is
+// not l, L or tsn:) and the aggregate argument's (not l), and, once the operator has its types, the same formats and
+// struct columns.
 void WindowFnOp::check_layout(const Layout& l, int bad_type_status) const {
   AB_REQUIRE((int)l.formats.size() == n_cols_, ARROYO_B200_INVALID_ARGUMENT,
              "window function: batch has " + std::to_string(l.formats.size()) + " flat columns, the plan " +
                  std::to_string(n_cols_));
+  if (agg_col_ >= 0 && l.formats[agg_col_] != "l")
+    throw Error(bad_type_status, "window function: " + std::string(fn_name()) + " argument of type '" +
+                                     l.formats[agg_col_] + "' (supported: l)");
   if (key_col_ >= 0 && !sortable_format(l.formats[key_col_]))
     throw Error(bad_type_status, "window function: PARTITION BY column of type '" + l.formats[key_col_] +
                                      "' (supported: l, L, tsn:)");
@@ -690,13 +888,16 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
   ++st_.kernel_launches;
   const unsigned int* idx = sort_rows(e, false);
 
-  // ranks and the fused filter
+  // ranks and the fused filter, or the aggregate
+  const bool agg = fn_ == ARROYO_B200_FN_AGGREGATE;
   const uint64_t n_tiles = (e + WF_TILE - 1) / WF_TILE;
   reserve(bits_, e);
   reserve(tiles_, n_tiles * sizeof(RankVal));
   reserve(fnv_, e * 8);
-  reserve(keep_, e * 4);
-  reserve(off2_, e * 8);
+  if (!agg) {
+    reserve(keep_, e * 4);
+    reserve(off2_, e * 8);
+  }
   AB_CUDA(cudaMemsetAsync(&counters()->instants, 0, 8, stream_));
   WRank r{};
   r.col[0] = cur_.col[ts_col_].as<unsigned long long>();
@@ -715,15 +916,19 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
   r.keep = keep_.as<unsigned int>();
   wf_rank_flags_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(r);
   AB_CUDA(cudaGetLastError());
-  wf_rank_carry_kernel<<<1, 1024, 0, stream_>>>(r.tiles, (long long)n_tiles);
+  wf_carry_kernel<RankVal><<<1, 1024, 0, stream_>>>(r.tiles, (long long)n_tiles);
   AB_CUDA(cudaGetLastError());
-  wf_rank_apply_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(r);
-  AB_CUDA(cudaGetLastError());
-  device_exclusive_scan(keep_.as<unsigned int>(), (int64_t)e, off2_.as<unsigned long long>(), &counters()->total, sums_,
-                        stream_);
-  st_.kernel_launches += 6;
-  unsigned long long m = 0, n_inst = 0;
-  AB_CUDA(cudaMemcpyAsync(&m, &counters()->total, 8, cudaMemcpyDeviceToHost, stream_));
+  unsigned long long m = e, n_inst = 0;
+  if (agg) {
+    aggregate(r, n_tiles);  // every row leaves
+  } else {
+    wf_rank_apply_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(r);
+    AB_CUDA(cudaGetLastError());
+    device_exclusive_scan(keep_.as<unsigned int>(), (int64_t)e, off2_.as<unsigned long long>(), &counters()->total,
+                          sums_, stream_);
+    st_.kernel_launches += 6;
+    AB_CUDA(cudaMemcpyAsync(&m, &counters()->total, 8, cudaMemcpyDeviceToHost, stream_));
+  }
   AB_CUDA(cudaMemcpyAsync(&n_inst, &counters()->instants, 8, cudaMemcpyDeviceToHost, stream_));
   AB_CUDA(cudaStreamSynchronize(stream_));
 
@@ -738,9 +943,10 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
     reserve(out_fn_, m * 8);
     g.n_cols = n_cols_;
     g.idx = idx;
-    g.keep = keep_.as<unsigned int>();
-    g.off = off2_.as<unsigned long long>();
+    g.keep = agg ? nullptr : keep_.as<unsigned int>();
+    g.off = agg ? nullptr : off2_.as<unsigned long long>();
     g.fn = fnv_.as<unsigned long long>();
+    g.at = agg ? at_.as<unsigned int>() : nullptr;
     g.fn_out = out_fn_.as<unsigned long long>();
     g.n = (long long)e;
     wf_gather_kernel<<<grid_for(e), WF_THREADS, 0, stream_>>>(g);
@@ -751,7 +957,7 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
         host_columns([&](int f) { return d2h_pinned(out_[f].p, (size_t)m * 8, stream_, &st_.d2h_bytes); });
     OutColumn fc;
     fc.name = fn_name();
-    fc.format = "L";
+    fc.format = fn_format();
     fc.data = d2h_pinned(out_fn_.p, (size_t)m * 8, stream_, &st_.d2h_bytes);
     cols.push_back(fc);
     out->arrays.emplace_back();
@@ -785,6 +991,30 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
   ckpt_from_ -= std::min<uint64_t>(ckpt_from_, below);
   st_.rows_out += m;
   st_.windows_out += n_inst;
+}
+
+// The aggregate's segmented scan over the `r.n` sorted rows (after wf_rank_flags and the rank tiles' carry): fnv_ gets
+// each peer group's value at its first row, at_ each row's group.
+void WindowFnOp::aggregate(const WRank& r, uint64_t n_tiles) {
+  reserve(agg_tiles_, n_tiles * 16);  // sizeof(AggVal<K>) for every K
+  reserve(at_, (size_t)r.n * 4);
+  WAgg p{};
+  p.arg = agg_col_ >= 0 ? cur_.col[agg_col_].as<unsigned long long>() : nullptr;
+  p.idx = r.idx;
+  p.bits = r.bits;
+  p.n = r.n;
+  p.rank_tiles = r.tiles;
+  p.tiles = agg_tiles_.p;
+  p.fv = fnv_.as<unsigned long long>();
+  p.at = at_.as<unsigned int>();
+  switch (agg_kind_) {
+    case ARROYO_B200_AGG_COUNT_STAR: launch_aggregate<ARROYO_B200_AGG_COUNT_STAR>(p, n_tiles, stream_); break;
+    case ARROYO_B200_AGG_SUM_I64: launch_aggregate<ARROYO_B200_AGG_SUM_I64>(p, n_tiles, stream_); break;
+    case ARROYO_B200_AGG_AVG_I64: launch_aggregate<ARROYO_B200_AGG_AVG_I64>(p, n_tiles, stream_); break;
+    case ARROYO_B200_AGG_MIN_I64: launch_aggregate<ARROYO_B200_AGG_MIN_I64>(p, n_tiles, stream_); break;
+    default: launch_aggregate<ARROYO_B200_AGG_MAX_I64>(p, n_tiles, stream_); break;
+  }
+  st_.kernel_launches += 5;  // with wf_rank_flags and the rank tiles' carry
 }
 
 // handle_checkpoint: table "input" gets the rows accepted since the previous checkpoint, one batch per instant in

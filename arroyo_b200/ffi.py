@@ -15,7 +15,7 @@ OK, INVALID_ARGUMENT, UNSUPPORTED, RUNTIME, FATAL, PANIC = 0, 1, 2, 3, 4, 5
 TUMBLING_AGGREGATE, SLIDING_AGGREGATE, SESSION_AGGREGATE, INSTANT_JOIN, UPDATING_AGGREGATE, TTL_JOIN = 1, 2, 3, 4, 5, 6
 INSTANT_AGGREGATE = 7
 WINDOW_FUNCTION = 8
-FN_ROW_NUMBER, FN_RANK, FN_DENSE_RANK = 1, 2, 3
+FN_ROW_NUMBER, FN_RANK, FN_DENSE_RANK, FN_AGGREGATE = 1, 2, 3, 4
 ORDER_ASC, ORDER_DESC = 16, 17
 MAX_ORDER_KEYS = 4
 AGG_COUNT_STAR, AGG_SUM_I64, AGG_AVG_I64, AGG_MIN_I64, AGG_MAX_I64 = 1, 2, 3, 4, 5

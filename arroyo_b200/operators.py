@@ -414,6 +414,8 @@ class InstantAggregatingWindowFunc(_WindowAggregate):
 
 
 _WINDOW_FNS = {"row_number": ffi.FN_ROW_NUMBER, "rank": ffi.FN_RANK, "dense_rank": ffi.FN_DENSE_RANK}
+_WINDOW_AGGS = {"count": ffi.AGG_COUNT_STAR, "sum": ffi.AGG_SUM_I64, "avg": ffi.AGG_AVG_I64, "min": ffi.AGG_MIN_I64,
+                "max": ffi.AGG_MAX_I64}
 
 
 def flat_names(schema: pa.Schema) -> List[str]:
@@ -429,8 +431,10 @@ def flat_names(schema: pa.Schema) -> List[str]:
 
 class WindowFunction(_WindowAggregate):
     """window_fn.rs: ROW_NUMBER / RANK / DENSE_RANK per instant (each upstream window stamps its rows with one
-    `_timestamp`) and partition key, with the fused `WHERE fn <= top_n`.  At watermark w every instant < w leaves in
-    one batch: the input columns, struct columns included, then the function column `config.name` (UInt64).  Columns
+    `_timestamp`) and partition key, with the fused `WHERE fn <= top_n`, or COUNT / SUM / AVG / MIN / MAX of
+    `config.argument` over the default frame.  At watermark w every instant < w leaves in one batch: the input columns,
+    struct columns included, then the function column `config.name` (UInt64 for a rank, Float64 for avg, else
+    Int64).  Columns
     are named in the config by their flat names (`flat_names`).  Table "input" (retention 0) holds per instant the input
     rows since the previous checkpoint.  Device-resident input is flat; a schema given at construction declares the
     column types to the library, which device batches do not carry."""
@@ -448,22 +452,30 @@ class WindowFunction(_WindowAggregate):
 
     def _build(self, names: List[str], schema: Optional[pa.Schema] = None):
         c = self.config
-        if c.function not in _WINDOW_FNS:
+        agg = c.function in _WINDOW_AGGS
+        if c.function not in _WINDOW_FNS and not agg:
             raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, f"window function {c.function}")
+        if agg and c.top_n != 0:
+            raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, f"{c.function} takes no top N filter")
         flat = list(names) if schema is None else flat_names(schema)
         cfg = ffi.OpConfig()
         cfg.kind = self.kind
-        cfg.window_fn = _WINDOW_FNS[c.function]
+        cfg.window_fn = ffi.FN_AGGREGATE if agg else _WINDOW_FNS[c.function]
         cfg.n_cols = len(flat)
         cfg.timestamp_col = flat.index(TIMESTAMP)
         cfg.n_key_cols = 0 if c.partition_by is None else 1
         cfg.key_col = 0 if c.partition_by is None else flat.index(c.partition_by)
         if len(c.order_by) > ffi.MAX_ORDER_KEYS:
             raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, "more than 4 ORDER BY keys")
-        cfg.n_aggs = len(c.order_by)
+        first = 0
+        if agg:  # aggs[0] is the aggregate, the ORDER BY keys follow
+            cfg.aggs[0].kind = _WINDOW_AGGS[c.function]
+            cfg.aggs[0].input_col = 0 if c.function == "count" else flat.index(c.argument)
+            first = 1
+        cfg.n_aggs = first + len(c.order_by)
         for i, (col, desc) in enumerate(c.order_by):
-            cfg.aggs[i].kind = ffi.ORDER_DESC if desc else ffi.ORDER_ASC
-            cfg.aggs[i].input_col = flat.index(col)
+            cfg.aggs[first + i].kind = ffi.ORDER_DESC if desc else ffi.ORDER_ASC
+            cfg.aggs[first + i].input_col = flat.index(col)
         cfg.slide_ns = int(c.top_n)
         self._create(cfg)
         self._names = list(names)

@@ -109,19 +109,32 @@ typedef enum ArroyoB200OpKind {
                                        * handle_watermark_device* => ARROYO_B200_UNSUPPORTED                           */
   ARROYO_B200_WINDOW_FUNCTION = 8     /* OperatorName::WindowFunction: WindowFunctionOperator, arroyo-worker/src/arrow/
                                        * window_fn.rs -- ROW_NUMBER / RANK / DENSE_RANK () OVER (PARTITION BY window
-                                       * [, key] ORDER BY ...), optionally fused with the filter `fn <= N` after it.
+                                       * [, key] ORDER BY ...), optionally fused with the filter `fn <= N` after it, or
+                                       * COUNT(*) / SUM / AVG / MIN / MAX (x) OVER (PARTITION BY window [, key]
+                                       * [ORDER BY ...]) with the default frame.
                                        * Config:
                                        *  - window_fn: ArroyoB200WindowFn; anything else => INVALID_ARGUMENT;
                                        *  - n_key_cols / key_col: the PARTITION BY column besides the window (the planner
                                        *    drops `window`, each upstream window stamping its rows with one _timestamp,
                                        *    plan/window_fn.rs:101-105): 0 or 1, of type l, L or tsn:; 2 or more =>
                                        *    UNSUPPORTED;
-                                       *  - n_aggs / aggs[]: the ORDER BY list, 1 to 4 entries {ARROYO_B200_ORDER_ASC |
-                                       *    _DESC, input_col} of type l, L or tsn: (a g column => UNSUPPORTED, as
-                                       *    DataFusion's float ordering and peers are not pinned here); 0 or more than 4
-                                       *    entries, or another kind code => INVALID_ARGUMENT;
+                                       *  - n_aggs / aggs[] of a ranking function: the ORDER BY list, 1 to 4 entries
+                                       *    {ARROYO_B200_ORDER_ASC | _DESC, input_col} of type l, L or tsn: (a g column =>
+                                       *    UNSUPPORTED, as DataFusion's float ordering and peers are not pinned here); 0
+                                       *    or more than 4 entries, or another kind code => INVALID_ARGUMENT;
+                                       *  - n_aggs / aggs[] of ARROYO_B200_FN_AGGREGATE: aggs[0] = {kind, input_col}, kind
+                                       *    one of ARROYO_B200_AGG_COUNT_STAR, _SUM_I64, _AVG_I64, _MIN_I64, _MAX_I64
+                                       *    (input_col ignored for COUNT; its column of another type than l =>
+                                       *    UNSUPPORTED), then 0 to 4 ORDER BY entries as above; n_aggs 0 or more than 5,
+                                       *    or another kind code => INVALID_ARGUMENT.  The frame is DataFusion's default:
+                                       *    without ORDER BY the whole segment (instant, key), with ORDER BY `RANGE
+                                       *    BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW`, from the segment start through
+                                       *    the row's last peer (peers tie on every ORDER BY key).  count / sum (wrapping)
+                                       *    / min / max give Int64 (l); avg gives Float64 (g): the f64 sum of the values
+                                       *    over the frame's row count;
                                        *  - slide_ns: N of a fused `WHERE fn <= N` (`fn = 1` is the same as `<= 1` for all
-                                       *    three functions); 0 = every row leaves; < 0 => INVALID_ARGUMENT;
+                                       *    three ranking functions); 0 = every row leaves; < 0, or not 0 for
+                                       *    FN_AGGREGATE => INVALID_ARGUMENT;
                                        *  - n_cols / timestamp_col / key_col / input_col count FLAT columns: a host batch's
                                        *    struct columns (the upstream window{start, end}, children all 64-bit) are
                                        *    flattened in place, one level, for this kind only.
@@ -136,8 +149,9 @@ typedef enum ArroyoB200OpKind {
                                        * keys); ties on every key by arrival order, restored rows first (DataFusion's sort
                                        * promises no order there; RANK and DENSE_RANK do not depend on it).  Output = the
                                        * input columns (struct columns re-nested as the host batches had them) then the
-                                       * function as UInt64 (L).  Host output only: handle_watermark_device* =>
-                                       * UNSUPPORTED.
+                                       * function: UInt64 (L) for a ranking function, named row_number / rank /
+                                       * dense_rank, and count / sum / avg / min / max as above for an aggregate.  Host
+                                       * output only: handle_watermark_device* => UNSUPPORTED.
                                        * Checkpoints write table "input" (retention 0): per open instant one batch of the
                                        * rows accepted since the previous checkpoint, in the input layout, in arrival
                                        * order.  on_start takes such batches in any order, does not late-filter them,
@@ -150,7 +164,8 @@ typedef enum ArroyoB200OpKind {
 typedef enum ArroyoB200WindowFn {
   ARROYO_B200_FN_ROW_NUMBER = 1,
   ARROYO_B200_FN_RANK = 2,
-  ARROYO_B200_FN_DENSE_RANK = 3
+  ARROYO_B200_FN_DENSE_RANK = 3,
+  ARROYO_B200_FN_AGGREGATE = 4  /* the ArroyoB200AggKind in aggs[0] */
 } ArroyoB200WindowFn;
 #define ARROYO_B200_ORDER_ASC 16
 #define ARROYO_B200_ORDER_DESC 17

@@ -9,11 +9,18 @@ top_n = 0 (every row leaves).  Per slide, after warm-up:
   wf_top1_ms        the window function's process_device_batch + handle_watermark with top_n = 1, host output included
   wf_all_ms         the same with top_n = 0 (2^20 rows leave to the host)
 
+With --function F (an aggregate: sum, count, avg, min or max) two more window functions take the same windows in the
+same slides, F(s) OVER (PARTITION BY window) and the running F(s) OVER (PARTITION BY window ORDER BY s DESC), every
+row leaving to the host:
+
+  wf_F_window_ms    F over the whole window
+  wf_F_running_ms   F over the default frame of ORDER BY s DESC
+
 Each is timed with CUDA events on the operators' stream around the calls (every handle_watermark ends in a stream
 synchronise); the medians are reported, with the sorted rows per second of each window function.  Prints one JSON
 line with the card's name and power limit.
 
-    python tools/window_fn_rates.py [--scale S] [--slides K]
+    python tools/window_fn_rates.py [--scale S] [--slides K] [--function F]
 
 --scale S divides the key count by 2^S (a quick rehearsal of the script)."""
 import argparse
@@ -47,6 +54,8 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--scale", type=int, default=0, help="divide the key count by 2^S (0..16)")
     ap.add_argument("--slides", type=int, default=20, help="timed slides after the 12 warm-up slides")
+    ap.add_argument("--function", default="row_number", choices=["row_number", "sum", "count", "avg", "min", "max"],
+                    help="an aggregate also times F(s) OVER (PARTITION BY window [ORDER BY s DESC])")
     a = ap.parse_args()
     if not 0 <= a.scale <= 16 or a.slides < 1:
         ap.error("--scale must be in [0, 16] and --slides >= 1")
@@ -67,15 +76,17 @@ def main():
         stream=stream.cuda_stream)
     w_schema = pa.schema([("key", pa.int64()), ("window_start", ts_t), ("window_end", ts_t), ("s", pa.int64()),
                           ("av", pa.float64()), (TS, ts_t)])
-    fns = {}
-    for what, top_n in (("top1", 1), ("all", 0)):
-        w_cfg = config.WindowFunctionConfig("row_number", None, [("s", True), ("key", True)], "rn", top_n)
-        fns[what] = native.WindowFunction(w_cfg, input_schema=w_schema, stream=stream.cuda_stream)
+    cfgs = {what: config.WindowFunctionConfig("row_number", None, [("s", True), ("key", True)], "rn", top_n)
+            for what, top_n in (("top1", 1), ("all", 0))}
+    if a.function != "row_number":
+        for what, order_by in (("window", []), ("running", [("s", True)])):
+            cfgs[f"{a.function}_{what}"] = config.WindowFunctionConfig(a.function, None, order_by, "f", argument="s")
+    fns = {what: native.WindowFunction(c, input_schema=w_schema, stream=stream.cuda_stream) for what, c in cfgs.items()}
     ctxs = {w: ab.OperatorContext(1) for w in fns}
     rng = np.random.default_rng(7)
     warm = 12
-    times = {"sliding_emit_ms": [], "wf_top1_ms": [], "wf_all_ms": []}
-    rows_out = {"top1": 0, "all": 0}
+    times = {"sliding_emit_ms": [], **{f"wf_{w}_ms": [] for w in fns}}
+    rows_out = {w: 0 for w in fns}
     window_rows = []
 
     def timed(f):
@@ -115,9 +126,8 @@ def main():
     rows = float(np.median(window_rows))
     res = {**card(), "keys": keys, "slides": a.slides, "window_rows": int(rows),
            **{k: round(v, 3) for k, v in med.items()},
-           "wf_top1_sorted_rows_per_s": round(rows / (med["wf_top1_ms"] / 1e3)),
-           "wf_all_sorted_rows_per_s": round(rows / (med["wf_all_ms"] / 1e3)),
-           "rows_out_top1": rows_out["top1"], "rows_out_all": rows_out["all"]}
+           **{f"wf_{w}_sorted_rows_per_s": round(rows / (med[f"wf_{w}_ms"] / 1e3)) for w in fns},
+           **{f"rows_out_{w}": rows_out[w] for w in fns}}
     print(json.dumps(res), flush=True)
     sliding.close()
     for op in fns.values():
