@@ -11,7 +11,7 @@ LIB = os.path.join(HERE, "libarroyo_b200.so")
 SOURCES = ["abi.cu", "window_agg.cu", "shuffle.cu", "join.cu", "session.cu", "updating_agg.cu", "ttl_join.cu",
            "instant_agg.cu", "window_fn.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper)
-HEADERS = ["agg_plan.h", "common.cuh", "dict.cuh", "bdict.cuh", "ingest_two_pass.cuh", "scan.cuh", "planner.h", "arrow_io.h", "op.h", "join_side.h", os.path.join("..", "..", "include", "arroyo_b200.h")]
+HEADERS = ["agg_plan.h", "common.cuh", "dict.cuh", "bdict.cuh", "ingest_two_pass.cuh", "scan.cuh", "planner.h", "arrow_io.h", "op.h", "join_side.h", "validity.cuh", os.path.join("..", "..", "include", "arroyo_b200.h")]
 
 
 def nvcc_path() -> str:

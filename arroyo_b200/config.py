@@ -61,13 +61,18 @@ class JoinConfig:
 @dataclass
 class WindowFunctionConfig:
     """WindowFunctionOperator (arroyo-worker/src/arrow/window_fn.rs): `function` (row_number | rank | dense_rank,
-    or the aggregate sum | count | avg | min | max of column `argument`, which count ignores) OVER (PARTITION BY
+    the aggregate sum | count | avg | min | max of column `argument`, which count ignores, the value function lag |
+    lead | first_value | last_value | nth_value of column `argument`, or percent_rank | cume_dist) OVER (PARTITION BY
     window [, `partition_by`] ORDER BY `order_by`), the function column named `name`.  `order_by` is a list of
-    (column, descending); it may be empty for an aggregate, whose frame is then the whole partition.  `top_n` > 0
-    fuses the `WHERE name <= top_n` that follows a ranking function; 0 lets every row through."""
+    (column, descending); it may be empty for every function but the ranking ones, the frame then being the whole
+    partition.  `top_n` > 0 fuses the `WHERE name <= top_n` that follows a ranking function; 0 lets every row through.
+    `offset` is lag / lead's k (>= 0) or nth_value's n (>= 1); `default` is lag / lead's default, in the argument's
+    type (None: NULL)."""
     function: str
     partition_by: Optional[str]
     order_by: List[tuple]
     name: str
     top_n: int = 0
     argument: Optional[str] = None
+    offset: int = 1
+    default: Optional[object] = None

@@ -10,6 +10,7 @@
 
 #include "op.h"
 #include "scan.cuh"
+#include "validity.cuh"
 
 namespace ab {
 
@@ -42,18 +43,6 @@ static __global__ void gather_ts_kernel(const int* __restrict__ il, const int* _
     dst[i] = max(ta, tb);
   }
 }
-// validity bytes -> Arrow validity bitmap (LSB first)
-static __global__ void pack_bits_kernel(const unsigned char* __restrict__ bytes, long long n, unsigned int* __restrict__ words) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long n_pad = (n + 31) / 32 * 32;
-  long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < n_pad; i += stride) {
-    bool v = i < n && bytes[i];
-    unsigned int b = __ballot_sync(0xffffffffu, v);
-    if ((threadIdx.x & 31) == 0) words[i >> 5] = b;
-  }
-}
-
 // ---- join sides ---------------------------------------------------------------------------
 // The joins compare raw 64-bit key patterns, which is equality only for integer-like keys of one type: an Int64,
 // UInt64 or timestamp[ns] key, the same type on both sides (INTEGRATION.md §1).  A Float64 key (-0.0 = 0.0) or an
@@ -231,23 +220,9 @@ class JoinOpBase : public OpBase {
           o.format = side[sd]->formats[c];
           o.data = d2h_pinned(out_cols_[oc].p, (size_t)n * 8, stream_, &st_.d2h_bytes);
           if (nullable[sd]) {
-            const size_t words = (size_t)((n + 31) / 32);
-            grow(out_bits_, words * 4);
-            pack_bits_kernel<<<grid_for(n), JOIN_THREADS, 0, stream_>>>(out_valid_[oc].as<unsigned char>(), n,
-                                                                       out_bits_.as<unsigned int>());
-            AB_CUDA(cudaGetLastError());
-            ++st_.kernel_launches;
-            o.validity = d2h_pinned(out_bits_.p, words * 4, stream_, &st_.d2h_bytes);
-            AB_CUDA(cudaStreamSynchronize(stream_));  // `out_bits_` is reused by the next column
-            const unsigned int* w = (const unsigned int*)o.validity;
-            int64_t set = 0;
-            for (size_t i = 0; i < words; ++i) set += __builtin_popcount(w[i]);
-            o.null_count = n - set;
-            o.nullable = true;
-            if (o.null_count == 0) {
-              PinnedPool::get().free(o.validity);
-              o.validity = nullptr;
-            }
+            grow(out_bits_, (size_t)((n + 31) / 32) * 4);
+            export_validity(o, out_valid_[oc].as<unsigned char>(), n, out_bits_.as<unsigned int>(), grid_for(n),
+                            JOIN_THREADS, stream_, st_);
           }
           cols.push_back(o);
         }

@@ -1,9 +1,11 @@
 // Window function on sm_90a (H100): the GPU side of `WindowFunctionOperator` (arroyo-worker/src/arrow/window_fn.rs),
 // for ROW_NUMBER / RANK / DENSE_RANK () OVER (PARTITION BY window [, key] ORDER BY k1 [DESC], ...), optionally fused
-// with the `WHERE fn <= N` that usually follows it (top N per window), and for COUNT(*) / SUM / AVG / MIN / MAX (x)
-// OVER (PARTITION BY window [, key] [ORDER BY ...]) over the default frame.  The planner (plan/window_fn.rs:101-105) drops
-// the `window` column from PARTITION BY: each upstream window stamps its rows with one `_timestamp`, so the rows are
-// bucketed by `_timestamp` ("instant") and the remaining PARTITION BY column, if any, splits each instant further.
+// with the `WHERE fn <= N` that usually follows it (top N per window), for COUNT(*) / SUM / AVG / MIN / MAX (x)
+// OVER (PARTITION BY window [, key] [ORDER BY ...]) over the default frame, and for LAG / LEAD / FIRST_VALUE /
+// LAST_VALUE / NTH_VALUE (x, ...) and PERCENT_RANK / CUME_DIST () over the same partitions.  The planner
+// (plan/window_fn.rs:101-105) drops the `window` column from PARTITION BY: each upstream window stamps its rows with one
+// `_timestamp`, so the rows are bucketed by `_timestamp` ("instant") and the remaining PARTITION BY column, if any,
+// splits each instant further.
 //
 //   store   every accepted row, SoA, one 64-bit array per flat input column; a row's index is its arrival sequence.
 //           The host doubles the store before a launch that could overfill it, from the rows it has handed over since
@@ -18,10 +20,10 @@
 //           partition) and peer starts (every sort key) and scans them, ballots within a warp and a two-level scan
 //           across 1024-row tiles: ROW_NUMBER = position in the segment + 1, RANK = position of the first peer + 1,
 //           DENSE_RANK = peer starts in the segment so far.  An aggregate adds a segmented scan of its argument with the
-//           same tiling, read at each peer group's last row (see "aggregates" below).  The fused filter, a compaction
-//           and a gather of every column write the output in sorted order; the rows that stay are compacted to the front
-//           of the store, in arrival
-//           order, so device memory tracks the open rows;
+//           same tiling, read at each peer group's last row (see "aggregates" below); the other functions add index
+//           arithmetic on the rank scan and a read of the argument (see "value functions" below).  The fused filter, a
+//           compaction and a gather of every column write the output in sorted order; the rows that stay are compacted
+//           to the front of the store, in arrival order, so device memory tracks the open rows;
 //   state   table "input": a checkpoint writes the rows accepted since the previous one (one store index marks them,
 //           re-based when the store is compacted), one batch per instant, in the input layout.  on_start appends the
 //           restored rows first and does not late-filter them, as the reference re-feeds them (:130-145).
@@ -36,6 +38,7 @@
 
 #include "op.h"
 #include "scan.cuh"
+#include "validity.cuh"
 
 namespace ab {
 namespace {
@@ -428,8 +431,88 @@ void launch_aggregate(const WAgg& p, uint64_t n_tiles, cudaStream_t stream) {
   AB_CUDA(cudaGetLastError());
 }
 
+// ---- value functions --------------------------------------------------------------------------------------------------
+// LAG / LEAD / FIRST_VALUE / LAST_VALUE / NTH_VALUE, PERCENT_RANK and CUME_DIST are index arithmetic on the rank scan.
+// For sorted row j the scan gives its segment's first row s and its peer group's first row g; the bounds pass adds the
+// segment's last row e and the peer group's last row f (the default frame's end: without ORDER BY every row of a segment
+// is a peer, so f = e): the last row of each peer group writes its index at the group's first row, and the last row of
+// each segment does the same at the segment's first row.  The apply pass then reads the argument at the row the function
+// names, LAG j - k, LEAD j + k, FIRST_VALUE s, LAST_VALUE f, NTH_VALUE s + n - 1, or takes the default (LAG / LEAD) or
+// NULL when that row is outside [s, e] (NTH_VALUE: [s, f]).  PERCENT_RANK = (g - s) / (e - s), 0 when s = e, and
+// CUME_DIST = (f - s + 1) / (e - s + 1), both in f64.  The argument's 64 bits move unchanged.
+struct WValue {
+  const unsigned long long* arg;  // the argument column (PERCENT_RANK / CUME_DIST: unused)
+  const unsigned int* idx;        // sorted
+  const unsigned char* bits;      // wf_rank_flags_kernel's starts
+  long long n;
+  const RankVal* rank_tiles;      // after wf_carry_kernel<RankVal>
+  unsigned int* peer_last;        // at each peer group's first sorted row: the group's last sorted row
+  unsigned int* seg_last;         // at each segment's first sorted row: the segment's last sorted row
+  int fn;
+  unsigned long long offset;      // LAG / LEAD: k; NTH_VALUE: n - 1
+  unsigned long long dflt;        // LAG / LEAD: the default's bits (0 without one; a NULL row's value)
+  unsigned long long* fv;         // per sorted row: the function's value
+  unsigned char* valid;           // per sorted row: 0 = NULL; null when the function cannot give NULL
+};
+
+// Each row's segment and peer group first rows: the rank scan of its tile on top of the tiles before it.  Every thread
+// of the block calls it.
+__device__ __forceinline__ RankVal value_scan(const WValue& p, long long j, unsigned int bits) {
+  RankVal total;
+  const RankVal v = tile_inclusive(bits, j, &total);
+  return combine(p.rank_tiles[blockIdx.x], v);
+}
+
+// pass 1: the last row of each peer group and of each segment, at its first row
+__global__ void __launch_bounds__(WF_TILE) wf_bounds_kernel(const __grid_constant__ WValue p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  const unsigned int bits = j < p.n ? p.bits[j] : 0u;
+  const RankVal r = value_scan(p, j, bits);
+  if (j >= p.n) return;
+  const unsigned int next = j + 1 < p.n ? p.bits[j + 1] : 6u;  // past the last row: a segment (and peer) start
+  if (next & 4u) p.peer_last[r.peer - 1u] = (unsigned int)j;
+  if (next & 2u) p.seg_last[r.seg - 1u] = (unsigned int)j;
+}
+
+// pass 2: each sorted row's value and validity
+__global__ void __launch_bounds__(WF_TILE) wf_value_apply_kernel(const __grid_constant__ WValue p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  const unsigned int bits = j < p.n ? p.bits[j] : 0u;
+  const RankVal r = value_scan(p, j, bits);
+  if (j >= p.n) return;
+  const unsigned int row = (unsigned int)j, s = r.seg - 1u, g = r.peer - 1u;
+  const unsigned int f = p.peer_last[g], e = p.seg_last[s];
+  unsigned long long v;
+  bool ok = true;
+  if (p.fn == ARROYO_B200_FN_PERCENT_RANK) {
+    v = e == s ? 0ull : (unsigned long long)__double_as_longlong((double)(g - s) / (double)(e - s));
+  } else if (p.fn == ARROYO_B200_FN_CUME_DIST) {
+    v = (unsigned long long)__double_as_longlong((double)(f - s + 1u) / (double)(e - s + 1u));
+  } else {
+    // the offsets are compared before they are narrowed: k may be anything up to INT64_MAX
+    unsigned int src;
+    if (p.fn == ARROYO_B200_FN_LAG) {
+      ok = p.offset <= (unsigned long long)(row - s);
+      src = row - (unsigned int)p.offset;
+    } else if (p.fn == ARROYO_B200_FN_LEAD) {
+      ok = p.offset <= (unsigned long long)(e - row);
+      src = row + (unsigned int)p.offset;
+    } else if (p.fn == ARROYO_B200_FN_FIRST_VALUE) {
+      src = s;
+    } else if (p.fn == ARROYO_B200_FN_LAST_VALUE) {
+      src = f;
+    } else {
+      ok = p.offset <= (unsigned long long)(f - s);
+      src = s + (unsigned int)p.offset;
+    }
+    v = ok ? p.arg[p.idx[src]] : p.dflt;
+  }
+  p.fv[j] = v;
+  if (p.valid) p.valid[j] = ok ? 1u : 0u;
+}
+
 // out[c][o] = store[c][idx[j]] for the kept rows (keep null: every row, o = j), and the function column: fn[j], or
-// fn[at[j]] when `at` is given
+// fn[at[j]] when `at` is given, with its validity byte from `valid` when that is given
 struct WGather {
   const unsigned long long* store[ARROYO_B200_MAX_COLS];
   WCols out;
@@ -439,7 +522,9 @@ struct WGather {
   const unsigned long long* off;
   const unsigned long long* fn;
   const unsigned int* at;
+  const unsigned char* valid;
   unsigned long long* fn_out;
+  unsigned char* valid_out;
   long long n;
 };
 __global__ void __launch_bounds__(WF_THREADS) wf_gather_kernel(const __grid_constant__ WGather p) {
@@ -450,7 +535,11 @@ __global__ void __launch_bounds__(WF_THREADS) wf_gather_kernel(const __grid_cons
     const unsigned long long o = p.keep ? p.off[j] : (unsigned long long)j;
     const unsigned int src = p.idx[j];
     for (int c = 0; c < p.n_cols; ++c) p.out.c[c][o] = p.store[c][src];
-    if (p.fn_out) p.fn_out[o] = p.fn[p.at ? p.at[j] : (unsigned int)j];
+    if (p.fn_out) {
+      const unsigned int f = p.at ? p.at[j] : (unsigned int)j;
+      p.fn_out[o] = p.fn[f];
+      if (p.valid) p.valid_out[o] = p.valid[f];
+    }
   }
 }
 
@@ -510,9 +599,13 @@ class WindowFnOp final : public OpBase {
     std::vector<Nest> nests;
   };
   int n_cols_ = 0, ts_col_ = 0, key_col_ = -1, fn_ = 0;
-  int agg_kind_ = 0, agg_col_ = -1;  // FN_AGGREGATE: the aggregate and its argument column (COUNT: none)
+  int agg_kind_ = 0;  // FN_AGGREGATE: the aggregate
+  int arg_col_ = -1;  // the argument column of an aggregate (COUNT: none) or a value function
   int n_order_ = 0, order_col_[ARROYO_B200_MAX_ORDER_KEYS] = {}, order_desc_[ARROYO_B200_MAX_ORDER_KEYS] = {};
   int64_t top_n_ = 0;
+  uint64_t offset_ = 0;      // LAG / LEAD: k; NTH_VALUE: n - 1
+  uint64_t dflt_ = 0;        // LAG / LEAD: the default's bits
+  bool has_default_ = false;
   Layout layout_;
   bool typed_ = false;  // layout_ comes from a host or state batch (else: Int64 columns, no structs)
   int64_t late_wm_ = LLONG_MIN;
@@ -524,28 +617,43 @@ class WindowFnOp final : public OpBase {
   DevBuf counters_, stage_;
   uint64_t stage_cap_ = 0;
   DevBuf flag_, off_, sums_, idx_[2], key_[2], cub_tmp_, bits_, tiles_, fnv_, keep_, off2_, agg_tiles_, at_;
-  DevBuf out_[ARROYO_B200_MAX_COLS], out_fn_;
+  DevBuf seg_last_, valid_;  // value functions: each segment's last row at its first, each row's validity
+  DevBuf out_[ARROYO_B200_MAX_COLS], out_fn_, out_valid_, out_bits_;
   ArroyoB200Stats st_{};
 
   int grid_for(uint64_t n) const {
     return (int)std::max<uint64_t>(1, std::min<uint64_t>((n + WF_THREADS - 1) / WF_THREADS, (uint64_t)num_sms_ * 8));
   }
   WCounters* counters() const { return counters_.as<WCounters>(); }
+  bool ranking() const { return fn_ <= ARROYO_B200_FN_DENSE_RANK; }
+  bool value_fn() const { return fn_ >= ARROYO_B200_FN_LAG && fn_ <= ARROYO_B200_FN_NTH_VALUE; }
+  // LAG / LEAD / NTH_VALUE may give NULL; `null_rows()`: with these arguments some row can be NULL
+  bool nullable() const {
+    return fn_ == ARROYO_B200_FN_LAG || fn_ == ARROYO_B200_FN_LEAD || fn_ == ARROYO_B200_FN_NTH_VALUE;
+  }
+  bool null_rows() const { return nullable() && !has_default_; }
   const char* fn_name() const {
+    static const char* const names[] = {"",          "row_number", "rank",       "dense_rank",   "",
+                                        "lag",       "lead",       "first_value", "last_value",  "nth_value",
+                                        "percent_rank", "cume_dist"};
     if (fn_ == ARROYO_B200_FN_AGGREGATE)
       return agg_kind_ == ARROYO_B200_AGG_COUNT_STAR ? "count"
              : agg_kind_ == ARROYO_B200_AGG_SUM_I64  ? "sum"
              : agg_kind_ == ARROYO_B200_AGG_AVG_I64  ? "avg"
              : agg_kind_ == ARROYO_B200_AGG_MIN_I64  ? "min"
                                                      : "max";
-    return fn_ == ARROYO_B200_FN_ROW_NUMBER ? "row_number" : fn_ == ARROYO_B200_FN_RANK ? "rank" : "dense_rank";
+    return names[fn_];
   }
-  // ranks are UInt64; count / sum / min / max Int64, avg Float64
-  const char* fn_format() const {
-    if (fn_ != ARROYO_B200_FN_AGGREGATE) return "L";
+  // ranks are UInt64; count / sum / min / max Int64, avg Float64; a value function takes its argument's type,
+  // PERCENT_RANK / CUME_DIST are Float64
+  std::string fn_format() const {
+    if (ranking()) return "L";
+    if (value_fn()) return layout_.formats[arg_col_];
+    if (fn_ != ARROYO_B200_FN_AGGREGATE) return "g";
     return agg_kind_ == ARROYO_B200_AGG_AVG_I64 ? "g" : "l";
   }
   void aggregate(const WRank& r, uint64_t n_tiles);
+  void values(const WRank& r, uint64_t n_tiles);
   Layout layout_of(const std::vector<InColumn>& cols, const std::vector<Nest>& nests, const ArrowSchema* s) const;
   void check_layout(const Layout& l, int bad_type_status) const;
   void adopt(const Layout& l);
@@ -562,10 +670,10 @@ class WindowFnOp final : public OpBase {
 WindowFnOp::WindowFnOp(const ArroyoB200OpConfig& c) {
   cfg = c;
   name = "window_function";
-  AB_REQUIRE(c.window_fn == ARROYO_B200_FN_ROW_NUMBER || c.window_fn == ARROYO_B200_FN_RANK ||
-                 c.window_fn == ARROYO_B200_FN_DENSE_RANK || c.window_fn == ARROYO_B200_FN_AGGREGATE,
+  AB_REQUIRE(c.window_fn >= ARROYO_B200_FN_ROW_NUMBER && c.window_fn <= ARROYO_B200_FN_CUME_DIST,
              ARROYO_B200_INVALID_ARGUMENT,
-             "window function: window_fn must be ROW_NUMBER (1), RANK (2), DENSE_RANK (3) or AGGREGATE (4)");
+             "window function: window_fn must be ROW_NUMBER (1), RANK (2), DENSE_RANK (3), AGGREGATE (4), LAG (5), "
+             "LEAD (6), FIRST_VALUE (7), LAST_VALUE (8), NTH_VALUE (9), PERCENT_RANK (10) or CUME_DIST (11)");
   fn_ = c.window_fn;
   const bool agg = fn_ == ARROYO_B200_FN_AGGREGATE;
   AB_REQUIRE(c.n_cols >= 1 && c.n_cols <= ARROYO_B200_MAX_COLS, ARROYO_B200_INVALID_ARGUMENT, "bad n_cols");
@@ -592,17 +700,49 @@ WindowFnOp::WindowFnOp(const ArroyoB200OpConfig& c) {
     if (agg_kind_ != ARROYO_B200_AGG_COUNT_STAR) {
       AB_REQUIRE(c.aggs[0].input_col >= 0 && c.aggs[0].input_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT,
                  "window function: aggregate argument column out of range");
-      agg_col_ = c.aggs[0].input_col;
+      arg_col_ = c.aggs[0].input_col;
     }
     AB_REQUIRE(c.slide_ns == 0, ARROYO_B200_INVALID_ARGUMENT,
                "window function: an aggregate takes no top N filter (slide_ns must be 0)");
-  } else {
+  } else if (ranking()) {
     AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= ARROYO_B200_MAX_ORDER_KEYS, ARROYO_B200_INVALID_ARGUMENT,
                "window function: ORDER BY takes 1 to 4 keys (n_aggs)");
     AB_REQUIRE(c.slide_ns >= 0, ARROYO_B200_INVALID_ARGUMENT, "window function: top N (slide_ns) must be >= 0");
     top_n_ = c.slide_ns;
+  } else {
+    if (value_fn()) {
+      // aggs[0] is the argument, aggs[1 ..] the ORDER BY keys
+      AB_REQUIRE(c.n_aggs >= 1 && c.n_aggs <= 1 + ARROYO_B200_MAX_ORDER_KEYS, ARROYO_B200_INVALID_ARGUMENT,
+                 std::string("window function: ") + fn_name() +
+                     " takes its argument and 0 to 4 ORDER BY keys (n_aggs 1 to 5)");
+      AB_REQUIRE(c.aggs[0].kind == ARROYO_B200_FN_ARGUMENT, ARROYO_B200_INVALID_ARGUMENT,
+                 std::string("window function: aggs[0] of ") + fn_name() + " is {FN_ARGUMENT (18), argument column}");
+      AB_REQUIRE(c.aggs[0].input_col >= 0 && c.aggs[0].input_col < n_cols_, ARROYO_B200_INVALID_ARGUMENT,
+                 "window function: argument column out of range");
+      arg_col_ = c.aggs[0].input_col;
+    } else {
+      AB_REQUIRE(c.n_aggs >= 0 && c.n_aggs <= ARROYO_B200_MAX_ORDER_KEYS, ARROYO_B200_INVALID_ARGUMENT,
+                 std::string("window function: ") + fn_name() + " takes 0 to 4 ORDER BY keys (n_aggs)");
+    }
+    AB_REQUIRE(c.slide_ns == 0, ARROYO_B200_INVALID_ARGUMENT,
+               std::string("window function: ") + fn_name() + " takes no top N filter (slide_ns must be 0)");
+    const bool lag_lead = fn_ == ARROYO_B200_FN_LAG || fn_ == ARROYO_B200_FN_LEAD;
+    has_default_ = (c.flags & ARROYO_B200_FLAG_FN_DEFAULT) != 0;
+    AB_REQUIRE(!has_default_ || lag_lead, ARROYO_B200_INVALID_ARGUMENT,
+               std::string("window function: ") + fn_name() + " takes no default (ARROYO_B200_FLAG_FN_DEFAULT)");
+    if (has_default_) dflt_ = (uint64_t)c.gap_ns;
+    if (lag_lead) {
+      AB_REQUIRE(c.width_ns >= 0, ARROYO_B200_UNSUPPORTED,
+                 std::string("window function: ") + fn_name() + " with a negative offset is not supported");
+      offset_ = (uint64_t)c.width_ns;
+    } else if (fn_ == ARROYO_B200_FN_NTH_VALUE) {
+      AB_REQUIRE(c.width_ns >= 0, ARROYO_B200_UNSUPPORTED,
+                 "window function: nth_value with a negative n is not supported");
+      AB_REQUIRE(c.width_ns != 0, ARROYO_B200_INVALID_ARGUMENT, "window function: nth_value's n (width_ns) must be >= 1");
+      offset_ = (uint64_t)c.width_ns - 1;
+    }
   }
-  const int first_key = agg ? 1 : 0;
+  const int first_key = (agg || value_fn()) ? 1 : 0;
   n_order_ = c.n_aggs - first_key;
   for (int k = 0; k < n_order_; ++k) {
     const ArroyoB200Agg& a = c.aggs[first_key + k];
@@ -643,15 +783,20 @@ WindowFnOp::Layout WindowFnOp::layout_of(const std::vector<InColumn>& cols, cons
 }
 
 // A batch's layout against the plan: its column count, the sort keys' types (`bad_type_status` when a key's type is
-// not l, L or tsn:) and the aggregate argument's (not l), and, once the operator has its types, the same formats and
-// struct columns.
+// not l, L or tsn:) and the argument's (an aggregate's not l, a value function's not l, L, g or tsn:), and, once the
+// operator has its types, the same formats and struct columns.
 void WindowFnOp::check_layout(const Layout& l, int bad_type_status) const {
   AB_REQUIRE((int)l.formats.size() == n_cols_, ARROYO_B200_INVALID_ARGUMENT,
              "window function: batch has " + std::to_string(l.formats.size()) + " flat columns, the plan " +
                  std::to_string(n_cols_));
-  if (agg_col_ >= 0 && l.formats[agg_col_] != "l")
-    throw Error(bad_type_status, "window function: " + std::string(fn_name()) + " argument of type '" +
-                                     l.formats[agg_col_] + "' (supported: l)");
+  if (arg_col_ >= 0) {
+    // an aggregate sums or compares Int64 values; a value function moves any 64-bit column of the operator unchanged
+    const std::string& f = l.formats[arg_col_];
+    const bool agg = fn_ == ARROYO_B200_FN_AGGREGATE;
+    if (agg ? f != "l" : !(sortable_format(f) || f == "g"))
+      throw Error(bad_type_status, "window function: " + std::string(fn_name()) + " argument of type '" + f +
+                                       "' (supported: " + (agg ? "l" : "l, L, g, tsn:") + ")");
+  }
   if (key_col_ >= 0 && !sortable_format(l.formats[key_col_]))
     throw Error(bad_type_status, "window function: PARTITION BY column of type '" + l.formats[key_col_] +
                                      "' (supported: l, L, tsn:)");
@@ -888,13 +1033,13 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
   ++st_.kernel_launches;
   const unsigned int* idx = sort_rows(e, false);
 
-  // ranks and the fused filter, or the aggregate
-  const bool agg = fn_ == ARROYO_B200_FN_AGGREGATE;
+  // ranks and the fused filter, the aggregate, or a value function
+  const bool agg = fn_ == ARROYO_B200_FN_AGGREGATE, rank = ranking();
   const uint64_t n_tiles = (e + WF_TILE - 1) / WF_TILE;
   reserve(bits_, e);
   reserve(tiles_, n_tiles * sizeof(RankVal));
   reserve(fnv_, e * 8);
-  if (!agg) {
+  if (rank) {
     reserve(keep_, e * 4);
     reserve(off2_, e * 8);
   }
@@ -921,6 +1066,8 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
   unsigned long long m = e, n_inst = 0;
   if (agg) {
     aggregate(r, n_tiles);  // every row leaves
+  } else if (!rank) {
+    values(r, n_tiles);  // every row leaves
   } else {
     wf_rank_apply_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(r);
     AB_CUDA(cudaGetLastError());
@@ -943,11 +1090,16 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
     reserve(out_fn_, m * 8);
     g.n_cols = n_cols_;
     g.idx = idx;
-    g.keep = agg ? nullptr : keep_.as<unsigned int>();
-    g.off = agg ? nullptr : off2_.as<unsigned long long>();
+    g.keep = rank ? keep_.as<unsigned int>() : nullptr;
+    g.off = rank ? off2_.as<unsigned long long>() : nullptr;
     g.fn = fnv_.as<unsigned long long>();
     g.at = agg ? at_.as<unsigned int>() : nullptr;
     g.fn_out = out_fn_.as<unsigned long long>();
+    if (null_rows()) {
+      reserve(out_valid_, m);
+      g.valid = valid_.as<unsigned char>();
+      g.valid_out = out_valid_.as<unsigned char>();
+    }
     g.n = (long long)e;
     wf_gather_kernel<<<grid_for(e), WF_THREADS, 0, stream_>>>(g);
     AB_CUDA(cudaGetLastError());
@@ -959,6 +1111,12 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
     fc.name = fn_name();
     fc.format = fn_format();
     fc.data = d2h_pinned(out_fn_.p, (size_t)m * 8, stream_, &st_.d2h_bytes);
+    fc.nullable = nullable();
+    if (g.valid) {
+      reserve(out_bits_, (size_t)((m + 31) / 32) * 4);
+      export_validity(fc, out_valid_.as<unsigned char>(), (int64_t)m, out_bits_.as<unsigned int>(), grid_for(m),
+                      WF_THREADS, stream_, st_);
+    }
     cols.push_back(fc);
     out->arrays.emplace_back();
     out->schemas.emplace_back();
@@ -999,7 +1157,7 @@ void WindowFnOp::aggregate(const WRank& r, uint64_t n_tiles) {
   reserve(agg_tiles_, n_tiles * 16);  // sizeof(AggVal<K>) for every K
   reserve(at_, (size_t)r.n * 4);
   WAgg p{};
-  p.arg = agg_col_ >= 0 ? cur_.col[agg_col_].as<unsigned long long>() : nullptr;
+  p.arg = arg_col_ >= 0 ? cur_.col[arg_col_].as<unsigned long long>() : nullptr;
   p.idx = r.idx;
   p.bits = r.bits;
   p.n = r.n;
@@ -1015,6 +1173,35 @@ void WindowFnOp::aggregate(const WRank& r, uint64_t n_tiles) {
     default: launch_aggregate<ARROYO_B200_AGG_MAX_I64>(p, n_tiles, stream_); break;
   }
   st_.kernel_launches += 5;  // with wf_rank_flags and the rank tiles' carry
+}
+
+// A value function, PERCENT_RANK or CUME_DIST over the `r.n` sorted rows (after wf_rank_flags and the rank tiles'
+// carry): fnv_ gets each row's value and, when the function can give NULL, valid_ its validity.  at_ holds each peer
+// group's last row, seg_last_ each segment's, at their first rows.
+void WindowFnOp::values(const WRank& r, uint64_t n_tiles) {
+  reserve(at_, (size_t)r.n * 4);
+  reserve(seg_last_, (size_t)r.n * 4);
+  WValue p{};
+  p.arg = arg_col_ >= 0 ? cur_.col[arg_col_].as<unsigned long long>() : nullptr;
+  p.idx = r.idx;
+  p.bits = r.bits;
+  p.n = r.n;
+  p.rank_tiles = r.tiles;
+  p.peer_last = at_.as<unsigned int>();
+  p.seg_last = seg_last_.as<unsigned int>();
+  p.fn = fn_;
+  p.offset = offset_;
+  p.dflt = dflt_;
+  p.fv = fnv_.as<unsigned long long>();
+  if (null_rows()) {
+    reserve(valid_, (size_t)r.n);
+    p.valid = valid_.as<unsigned char>();
+  }
+  wf_bounds_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  wf_value_apply_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(p);
+  AB_CUDA(cudaGetLastError());
+  st_.kernel_launches += 4;  // with wf_rank_flags and the rank tiles' carry
 }
 
 // handle_checkpoint: table "input" gets the rows accepted since the previous checkpoint, one batch per instant in

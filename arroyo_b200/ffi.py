@@ -16,7 +16,9 @@ TUMBLING_AGGREGATE, SLIDING_AGGREGATE, SESSION_AGGREGATE, INSTANT_JOIN, UPDATING
 INSTANT_AGGREGATE = 7
 WINDOW_FUNCTION = 8
 FN_ROW_NUMBER, FN_RANK, FN_DENSE_RANK, FN_AGGREGATE = 1, 2, 3, 4
+FN_LAG, FN_LEAD, FN_FIRST_VALUE, FN_LAST_VALUE, FN_NTH_VALUE, FN_PERCENT_RANK, FN_CUME_DIST = 5, 6, 7, 8, 9, 10, 11
 ORDER_ASC, ORDER_DESC = 16, 17
+FN_ARGUMENT = 18
 MAX_ORDER_KEYS = 4
 AGG_COUNT_STAR, AGG_SUM_I64, AGG_AVG_I64, AGG_MIN_I64, AGG_MAX_I64 = 1, 2, 3, 4, 5
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_FULL = 0, 1, 2, 3
@@ -25,6 +27,7 @@ FLAG_NO_DIRECT = 64  # accepted and ignored since round 2
 FLAG_NO_TWO_PASS = 128
 FLAG_TWO_PASS_ALWAYS = 256
 FLAG_UPDATING_INPUT = 512
+FLAG_FN_DEFAULT = 1024
 NO_WATERMARK = -(1 << 63)
 INT64_MIN = -(1 << 63)
 INT64_MAX = (1 << 63) - 1

@@ -7,6 +7,7 @@ handle_checkpoint(barrier, ctx, collector), on_close(final_message, ctx, collect
 Batches are pyarrow RecordBatches crossing the boundary through the Arrow C Data Interface."""
 import ctypes as C
 import functools
+import struct
 import time
 from typing import List, Optional
 
@@ -123,7 +124,7 @@ class _NativeOperator:
     def _create(self, cfg: ffi.OpConfig):
         cfg.device = self._device
         cfg.stream = self._stream
-        cfg.flags = self._flags
+        cfg.flags |= self._flags  # on top of the plan's own flags (WindowFunction's FLAG_FN_DEFAULT)
         cfg.expected_keys = self._expected_keys
         cfg.task_index = self._task_index
         cfg.parallelism = self._parallelism
@@ -416,25 +417,41 @@ class InstantAggregatingWindowFunc(_WindowAggregate):
 _WINDOW_FNS = {"row_number": ffi.FN_ROW_NUMBER, "rank": ffi.FN_RANK, "dense_rank": ffi.FN_DENSE_RANK}
 _WINDOW_AGGS = {"count": ffi.AGG_COUNT_STAR, "sum": ffi.AGG_SUM_I64, "avg": ffi.AGG_AVG_I64, "min": ffi.AGG_MIN_I64,
                 "max": ffi.AGG_MAX_I64}
+_WINDOW_VALUES = {"lag": ffi.FN_LAG, "lead": ffi.FN_LEAD, "first_value": ffi.FN_FIRST_VALUE,
+                  "last_value": ffi.FN_LAST_VALUE, "nth_value": ffi.FN_NTH_VALUE}
+_WINDOW_DISTS = {"percent_rank": ffi.FN_PERCENT_RANK, "cume_dist": ffi.FN_CUME_DIST}
 
 
 def flat_names(schema: pa.Schema) -> List[str]:
     """The window function's flat columns: a struct column's children take its place as `<struct>_<child>`."""
-    names = []
+    return [name for name, _ in _flat_fields(schema)]
+
+
+def _flat_fields(schema: pa.Schema):
+    fields = []
     for f in schema:
         if pa.types.is_struct(f.type):
-            names += [f"{f.name}_{c.name}" for c in f.type]
+            fields += [(f"{f.name}_{c.name}", c.type) for c in f.type]
         else:
-            names.append(f.name)
-    return names
+            fields.append((f.name, f.type))
+    return fields
+
+
+def _default_bits(value, arrow_type) -> int:
+    """LAG / LEAD's default as the signed 64 bits of the argument's type: a Float64's IEEE bits, else the integer
+    modulo 2^64."""
+    if arrow_type is not None and pa.types.is_floating(arrow_type):
+        return struct.unpack("<q", struct.pack("<d", float(value)))[0]
+    return ((int(value) + (1 << 63)) % (1 << 64)) - (1 << 63)
 
 
 class WindowFunction(_WindowAggregate):
     """window_fn.rs: ROW_NUMBER / RANK / DENSE_RANK per instant (each upstream window stamps its rows with one
-    `_timestamp`) and partition key, with the fused `WHERE fn <= top_n`, or COUNT / SUM / AVG / MIN / MAX of
-    `config.argument` over the default frame.  At watermark w every instant < w leaves in one batch: the input columns,
-    struct columns included, then the function column `config.name` (UInt64 for a rank, Float64 for avg, else
-    Int64).  Columns
+    `_timestamp`) and partition key, with the fused `WHERE fn <= top_n`, COUNT / SUM / AVG / MIN / MAX of
+    `config.argument` over the default frame, LAG / LEAD / FIRST_VALUE / LAST_VALUE / NTH_VALUE of `config.argument`,
+    or PERCENT_RANK / CUME_DIST.  At watermark w every instant < w leaves in one batch: the input columns, struct
+    columns included, then the function column `config.name` (UInt64 for a rank, Float64 for avg, percent_rank and
+    cume_dist, the argument's type for a value function, else Int64; lag / lead / nth_value are nullable).  Columns
     are named in the config by their flat names (`flat_names`).  Table "input" (retention 0) holds per instant the input
     rows since the previous checkpoint.  Device-resident input is flat; a schema given at construction declares the
     column types to the library, which device batches do not carry."""
@@ -452,15 +469,19 @@ class WindowFunction(_WindowAggregate):
 
     def _build(self, names: List[str], schema: Optional[pa.Schema] = None):
         c = self.config
-        agg = c.function in _WINDOW_AGGS
-        if c.function not in _WINDOW_FNS and not agg:
+        agg, value = c.function in _WINDOW_AGGS, c.function in _WINDOW_VALUES
+        codes = {**_WINDOW_FNS, **_WINDOW_VALUES, **_WINDOW_DISTS, **{f: ffi.FN_AGGREGATE for f in _WINDOW_AGGS}}
+        if c.function not in codes:
             raise ffi.UnsupportedPlan(ffi.UNSUPPORTED, f"window function {c.function}")
-        if agg and c.top_n != 0:
+        if c.function not in _WINDOW_FNS and c.top_n != 0:
             raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, f"{c.function} takes no top N filter")
-        flat = list(names) if schema is None else flat_names(schema)
+        if c.default is not None and c.function not in ("lag", "lead"):
+            raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, f"{c.function} takes no default")
+        fields = [(n, None) for n in names] if schema is None else _flat_fields(schema)
+        flat = [n for n, _ in fields]
         cfg = ffi.OpConfig()
         cfg.kind = self.kind
-        cfg.window_fn = ffi.FN_AGGREGATE if agg else _WINDOW_FNS[c.function]
+        cfg.window_fn = codes[c.function]
         cfg.n_cols = len(flat)
         cfg.timestamp_col = flat.index(TIMESTAMP)
         cfg.n_key_cols = 0 if c.partition_by is None else 1
@@ -472,6 +493,15 @@ class WindowFunction(_WindowAggregate):
             cfg.aggs[0].kind = _WINDOW_AGGS[c.function]
             cfg.aggs[0].input_col = 0 if c.function == "count" else flat.index(c.argument)
             first = 1
+        if value:  # aggs[0] is the argument, the ORDER BY keys follow
+            cfg.aggs[0].kind = ffi.FN_ARGUMENT
+            cfg.aggs[0].input_col = flat.index(c.argument)
+            first = 1
+            if c.function in ("lag", "lead", "nth_value"):
+                cfg.width_ns = int(c.offset)
+            if c.default is not None:
+                cfg.flags |= ffi.FLAG_FN_DEFAULT
+                cfg.gap_ns = _default_bits(c.default, fields[cfg.aggs[0].input_col][1])
         cfg.n_aggs = first + len(c.order_by)
         for i, (col, desc) in enumerate(c.order_by):
             cfg.aggs[first + i].kind = ffi.ORDER_DESC if desc else ffi.ORDER_ASC

@@ -109,9 +109,11 @@ typedef enum ArroyoB200OpKind {
                                        * handle_watermark_device* => ARROYO_B200_UNSUPPORTED                           */
   ARROYO_B200_WINDOW_FUNCTION = 8     /* OperatorName::WindowFunction: WindowFunctionOperator, arroyo-worker/src/arrow/
                                        * window_fn.rs -- ROW_NUMBER / RANK / DENSE_RANK () OVER (PARTITION BY window
-                                       * [, key] ORDER BY ...), optionally fused with the filter `fn <= N` after it, or
+                                       * [, key] ORDER BY ...), optionally fused with the filter `fn <= N` after it,
                                        * COUNT(*) / SUM / AVG / MIN / MAX (x) OVER (PARTITION BY window [, key]
-                                       * [ORDER BY ...]) with the default frame.
+                                       * [ORDER BY ...]) with the default frame, LAG / LEAD / FIRST_VALUE / LAST_VALUE /
+                                       * NTH_VALUE (x, ...) and PERCENT_RANK / CUME_DIST () OVER (PARTITION BY window
+                                       * [, key] [ORDER BY ...]).
                                        * Config:
                                        *  - window_fn: ArroyoB200WindowFn; anything else => INVALID_ARGUMENT;
                                        *  - n_key_cols / key_col: the PARTITION BY column besides the window (the planner
@@ -132,9 +134,33 @@ typedef enum ArroyoB200OpKind {
                                        *    the row's last peer (peers tie on every ORDER BY key).  count / sum (wrapping)
                                        *    / min / max give Int64 (l); avg gives Float64 (g): the f64 sum of the values
                                        *    over the frame's row count;
+                                       *  - n_aggs / aggs[] of a value function (FN_LAG .. FN_NTH_VALUE): aggs[0] =
+                                       *    {ARROYO_B200_FN_ARGUMENT, x}, x any flat column of type l, L, g or tsn: (a
+                                       *    window struct child included; another type => UNSUPPORTED), then 0 to 4
+                                       *    ORDER BY entries as above; aggs[0] of another kind, or n_aggs 0 or more than
+                                       *    5 => INVALID_ARGUMENT.  PERCENT_RANK / CUME_DIST: aggs[] is the ORDER BY list,
+                                       *    0 to 4 entries.  For a row j of a segment (instant, key) spanning sorted rows
+                                       *    [s, e], with f = the last row of j's peer group (the default frame's end; e
+                                       *    without ORDER BY, where every row of the segment is a peer):
+                                       *      LAG(x, k, d)    x at j - k if j - k >= s, else d        x's type, nullable
+                                       *      LEAD(x, k, d)   x at j + k if j + k <= e, else d        x's type, nullable
+                                       *      FIRST_VALUE(x)  x at s                                  x's type
+                                       *      LAST_VALUE(x)   x at f                                  x's type
+                                       *      NTH_VALUE(x, n) x at s + n - 1 if that is <= f, else NULL  x's type, nullable
+                                       *      PERCENT_RANK()  (rank - 1) / (e - s), 0 when s = e      Float64 (g)
+                                       *      CUME_DIST()     (f - s + 1) / (e - s + 1)               Float64 (g)
+                                       *    The value functions move x's 64 bits unchanged (NaN payloads and -0.0
+                                       *    included); LAG / LEAD ignore the frame.  width_ns is LAG / LEAD's k (>= 0)
+                                       *    or NTH_VALUE's n (>= 1); every other function ignores it.  k < 0 or n < 0 =>
+                                       *    UNSUPPORTED (DataFusion's reversed offsets are not pinned here), n = 0 =>
+                                       *    INVALID_ARGUMENT.  With flags & ARROYO_B200_FLAG_FN_DEFAULT, LAG / LEAD's
+                                       *    default d is the 64 bits in gap_ns, in x's type; without it d is NULL.  The
+                                       *    flag on FN_FIRST_VALUE .. FN_CUME_DIST => INVALID_ARGUMENT (the ranking
+                                       *    functions and the aggregates ignore flags, as before).  A nullable column
+                                       *    carries an Arrow validity bitmap only when one of its rows is NULL;
                                        *  - slide_ns: N of a fused `WHERE fn <= N` (`fn = 1` is the same as `<= 1` for all
-                                       *    three ranking functions); 0 = every row leaves; < 0, or not 0 for
-                                       *    FN_AGGREGATE => INVALID_ARGUMENT;
+                                       *    three ranking functions); 0 = every row leaves; < 0, or not 0 for any other
+                                       *    function => INVALID_ARGUMENT;
                                        *  - n_cols / timestamp_col / key_col / input_col count FLAT columns: a host batch's
                                        *    struct columns (the upstream window{start, end}, children all 64-bit) are
                                        *    flattened in place, one level, for this kind only.
@@ -150,8 +176,9 @@ typedef enum ArroyoB200OpKind {
                                        * promises no order there; RANK and DENSE_RANK do not depend on it).  Output = the
                                        * input columns (struct columns re-nested as the host batches had them) then the
                                        * function: UInt64 (L) for a ranking function, named row_number / rank /
-                                       * dense_rank, and count / sum / avg / min / max as above for an aggregate.  Host
-                                       * output only: handle_watermark_device* => UNSUPPORTED.
+                                       * dense_rank, count / sum / avg / min / max as above for an aggregate, and lag /
+                                       * lead / first_value / last_value / nth_value / percent_rank / cume_dist as
+                                       * above.  Host output only: handle_watermark_device* => UNSUPPORTED.
                                        * Checkpoints write table "input" (retention 0): per open instant one batch of the
                                        * rows accepted since the previous checkpoint, in the input layout, in arrival
                                        * order.  on_start takes such batches in any order, does not late-filter them,
@@ -165,10 +192,18 @@ typedef enum ArroyoB200WindowFn {
   ARROYO_B200_FN_ROW_NUMBER = 1,
   ARROYO_B200_FN_RANK = 2,
   ARROYO_B200_FN_DENSE_RANK = 3,
-  ARROYO_B200_FN_AGGREGATE = 4  /* the ArroyoB200AggKind in aggs[0] */
+  ARROYO_B200_FN_AGGREGATE = 4,   /* the ArroyoB200AggKind in aggs[0] */
+  ARROYO_B200_FN_LAG = 5,         /* value functions (5-9): aggs[0] = {ARROYO_B200_FN_ARGUMENT, x} */
+  ARROYO_B200_FN_LEAD = 6,
+  ARROYO_B200_FN_FIRST_VALUE = 7,
+  ARROYO_B200_FN_LAST_VALUE = 8,
+  ARROYO_B200_FN_NTH_VALUE = 9,
+  ARROYO_B200_FN_PERCENT_RANK = 10,
+  ARROYO_B200_FN_CUME_DIST = 11
 } ArroyoB200WindowFn;
 #define ARROYO_B200_ORDER_ASC 16
 #define ARROYO_B200_ORDER_DESC 17
+#define ARROYO_B200_FN_ARGUMENT 18 /* aggs[0].kind of a value function: input_col is its argument x */
 #define ARROYO_B200_MAX_ORDER_KEYS 4
 
 typedef enum ArroyoB200AggKind {
@@ -278,6 +313,7 @@ typedef struct ArroyoB200OpConfig {
 #define ARROYO_B200_FLAG_TWO_PASS_ALWAYS 256u /* two-pass ingest for every eligible launch, however small  */
                                           /* (by default launches under 2^19 rows use the one-pass kernel: */
                                           /* the per-bucket set-up does not pay for them; test knob)       */
+#define ARROYO_B200_FLAG_FN_DEFAULT 1024u /* WINDOW_FUNCTION, LAG / LEAD: gap_ns holds the default's 64 bits */
 
 typedef struct ArroyoB200Op ArroyoB200Op;
 

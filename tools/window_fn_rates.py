@@ -9,18 +9,23 @@ top_n = 0 (every row leaves).  Per slide, after warm-up:
   wf_top1_ms        the window function's process_device_batch + handle_watermark with top_n = 1, host output included
   wf_all_ms         the same with top_n = 0 (2^20 rows leave to the host)
 
-With --function F (an aggregate: sum, count, avg, min or max) two more window functions take the same windows in the
-same slides, F(s) OVER (PARTITION BY window) and the running F(s) OVER (PARTITION BY window ORDER BY s DESC), every
-row leaving to the host:
+With --function F [G ...] more window functions take the same windows in the same slides, every row leaving to the
+host.  An aggregate F (sum, count, avg, min or max) adds F(s) OVER (PARTITION BY window) and the running F(s) OVER
+(PARTITION BY window ORDER BY s DESC):
 
   wf_F_window_ms    F over the whole window
   wf_F_running_ms   F over the default frame of ORDER BY s DESC
+
+A value function F (lag, lead, first_value, last_value or nth_value) adds F(s) OVER (PARTITION BY window ORDER BY s
+DESC, key DESC), with lag / lead's offset 1 and nth_value's n 2, and percent_rank or cume_dist adds F() over the same:
+
+  wf_F_ms           F over the ordered window
 
 Each is timed with CUDA events on the operators' stream around the calls (every handle_watermark ends in a stream
 synchronise); the medians are reported, with the sorted rows per second of each window function.  Prints one JSON
 line with the card's name and power limit.
 
-    python tools/window_fn_rates.py [--scale S] [--slides K] [--function F]
+    python tools/window_fn_rates.py [--scale S] [--slides K] [--function F [G ...]]
 
 --scale S divides the key count by 2^S (a quick rehearsal of the script)."""
 import argparse
@@ -37,6 +42,8 @@ sys.path.insert(0, ROOT)
 SEC = 1_000_000_000
 T0 = 1_700_000_000 * SEC
 TS = "_timestamp"
+AGGREGATES = ["sum", "count", "avg", "min", "max"]
+ORDERED = ["lag", "lead", "first_value", "last_value", "nth_value", "percent_rank", "cume_dist"]
 
 
 def card():
@@ -54,8 +61,9 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--scale", type=int, default=0, help="divide the key count by 2^S (0..16)")
     ap.add_argument("--slides", type=int, default=20, help="timed slides after the 12 warm-up slides")
-    ap.add_argument("--function", default="row_number", choices=["row_number", "sum", "count", "avg", "min", "max"],
-                    help="an aggregate also times F(s) OVER (PARTITION BY window [ORDER BY s DESC])")
+    ap.add_argument("--function", nargs="+", default=["row_number"], choices=["row_number", *AGGREGATES, *ORDERED],
+                    help="also time F(s) OVER (PARTITION BY window [ORDER BY s DESC]) for an aggregate, or F over "
+                         "(PARTITION BY window ORDER BY s DESC, key DESC) for the other functions")
     a = ap.parse_args()
     if not 0 <= a.scale <= 16 or a.slides < 1:
         ap.error("--scale must be in [0, 16] and --slides >= 1")
@@ -78,9 +86,14 @@ def main():
                           ("av", pa.float64()), (TS, ts_t)])
     cfgs = {what: config.WindowFunctionConfig("row_number", None, [("s", True), ("key", True)], "rn", top_n)
             for what, top_n in (("top1", 1), ("all", 0))}
-    if a.function != "row_number":
-        for what, order_by in (("window", []), ("running", [("s", True)])):
-            cfgs[f"{a.function}_{what}"] = config.WindowFunctionConfig(a.function, None, order_by, "f", argument="s")
+    for f in a.function:
+        if f in AGGREGATES:
+            for what, order_by in (("window", []), ("running", [("s", True)])):
+                cfgs[f"{f}_{what}"] = config.WindowFunctionConfig(f, None, order_by, "f", argument="s")
+        elif f in ORDERED:
+            cfgs[f] = config.WindowFunctionConfig(f, None, [("s", True), ("key", True)], "f",
+                                                  argument=None if f in ("percent_rank", "cume_dist") else "s",
+                                                  offset=2 if f == "nth_value" else 1)
     fns = {what: native.WindowFunction(c, input_schema=w_schema, stream=stream.cuda_stream) for what, c in cfgs.items()}
     ctxs = {w: ab.OperatorContext(1) for w in fns}
     rng = np.random.default_rng(7)
