@@ -7,8 +7,6 @@
 
 namespace ab {
 
-constexpr int MAX_PROBE = 4096;
-
 struct alignas(16) Slot {
   long long key;
   uint32_t id;
@@ -72,10 +70,12 @@ static __global__ void dict_rebuild_kernel(Slot* slots, uint32_t cap, const long
   }
 }
 
-// First sighting of a key: claim the empty slot found at `pos` (or keep walking if somebody else took it).
+// First sighting of a key: claim the empty slot found at `pos` (or keep walking if somebody else took it).  The walk
+// may visit every slot: the table is kept below 0.3 load (dict_slots_for), so it always ends at the key or at an empty
+// slot, however long the key's chain is.  ID_OVERFLOW: the ids are used up, or (never, below full) no slot was found.
 static __device__ __noinline__ uint32_t dict_insert(const DictView& d, long long key, uint32_t pos) {
 #pragma unroll 1
-  for (int probe = 0; probe < MAX_PROBE; ++probe) {
+  for (uint32_t probe = 0; probe < d.cap; ++probe) {
     Slot* sp = d.slots + pos;
     ulonglong2 raw = __ldcg(reinterpret_cast<const ulonglong2*>(sp));
     long long k = (long long)raw.x;

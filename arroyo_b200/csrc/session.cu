@@ -76,7 +76,7 @@ struct SessCtx {
   int keyed;
 };
 
-enum : unsigned long long { ERR_POOL = 1, ERR_ADD_FLUSHED = 2, ERR_BEFORE_START = 4, ERR_OUT = 8, ERR_LOOP = 16 };
+enum : unsigned long long { ERR_POOL = 1, ERR_ADD_FLUSHED = 2, ERR_BEFORE_START = 4, ERR_OUT = 8, ERR_LOOP = 16, ERR_DICT = 32 };
 // Every device loop over the linked lists is bounded: a corrupted list must surface as an error, never as a hang.  The
 // bound is what a sound list can take: a list holds at most node_cap nodes; a fill visits each node at most twice
 // (pop_first's walk, then add_batch) and allocates its remainders from the same pool; and every session a watermark
@@ -394,8 +394,8 @@ __global__ void __launch_bounds__(ST) prep_kernel(const __grid_constant__ PrepPa
       const long long key = __ldcs(p.key + i);
       if (key == EMPTY_KEY) *p.min_key_seen = 1u;
       id = key == EMPTY_KEY ? 0u : dict_insert(p.dict, key, dict_home((uint64_t)key, p.dict.cap));
-      if (id >= ID_OVERFLOW) {
-        atomicOr(p.ctr + 5, (unsigned long long)ERR_POOL);
+      if (id >= ID_OVERFLOW) {  // the host sized ids and slots for every row of the launch: the batch fails, loudly
+        atomicOr(p.ctr + 5, (unsigned long long)ERR_DICT);
         keep = false;
       }
     }
@@ -926,6 +926,7 @@ void SessionOp::check_err() {
   if (e & ERR_ADD_FLUSHED)
     throw Error(ARROYO_B200_RUNTIME, "should not have flushed batches when adding a batch (session_aggregating_window.rs:672-675)");
   if (e & ERR_LOOP) throw Error(ARROYO_B200_RUNTIME, "session operator: per-key list walk exceeded its bound (corrupted state)");
+  if (e & ERR_DICT) throw Error(ARROYO_B200_RUNTIME, "session operator: a new key found no id or slot in the key dictionary");
   throw Error(ARROYO_B200_RUNTIME, "session operator pool / output capacity exceeded");
 }
 
