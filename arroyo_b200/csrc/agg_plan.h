@@ -2,11 +2,14 @@
 // accumulators it keeps per key and how each aggregate is computed from them.
 //
 // Accumulators are 64-bit words in a per-key SoA block.  Accumulator 0 counts rows; every other one folds one value
-// column with one kind, and aggregates of the same (kind, column) share it.
+// column with one kind, and aggregates of the same (kind, column) share it.  What each kind does on the device (its
+// identity, the accumulator form of an input value, sequential and global merge, unmerge, AVG) is defined here and
+// nowhere else.
 #pragma once
 
 #include <climits>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "arrow_io.h"
@@ -34,6 +37,12 @@ __host__ __device__ __forceinline__ unsigned long long acc_identity(int kind) {
   return v;
 }
 
+// The accumulator-domain form of an Int64 input value `x` for an accumulator of `kind`: the bits of (double)x for
+// ACC_SUM_F64, x itself for every other kind.
+__device__ __forceinline__ unsigned long long acc_of_value(int kind, long long x) {
+  return kind == ACC_SUM_F64 ? (unsigned long long)__double_as_longlong((double)x) : (unsigned long long)x;
+}
+
 // What folding `b` into `a` gives for an accumulator of `kind` (ACC_ROWS and ACC_SUM_I64 add, wrapping).
 __device__ __forceinline__ unsigned long long acc_merge(int kind, unsigned long long a, unsigned long long b) {
   switch (kind) {
@@ -45,13 +54,48 @@ __device__ __forceinline__ unsigned long long acc_merge(int kind, unsigned long 
   }
 }
 
-// acc_merge of `v` into `*dst`, as one atomic.
-__device__ __forceinline__ void acc_atomic_merge(int kind, unsigned long long* dst, unsigned long long v) {
+// f(k) with `kind` as the compile-time constant k (std::integral_constant), which the functions above take as a kind:
+// a loop over many values in f then folds with that kind's code alone instead of branching on the kind per value.
+// ACC_ROWS is passed as ACC_SUM_I64, which folds the same way.
+template <class F>
+__device__ __forceinline__ auto acc_with_kind(int kind, F f) {
   switch (kind) {
-    case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), __longlong_as_double((long long)v)); break;
-    case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(dst), (long long)v); break;
-    case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(dst), (long long)v); break;
-    default: atomicAdd(dst, v); break;
+    case ACC_SUM_F64: return f(std::integral_constant<int, ACC_SUM_F64>{});
+    case ACC_MIN_I64: return f(std::integral_constant<int, ACC_MIN_I64>{});
+    case ACC_MAX_I64: return f(std::integral_constant<int, ACC_MAX_I64>{});
+    default: return f(std::integral_constant<int, ACC_SUM_I64>{});
+  }
+}
+
+// What taking `b` back out of `a` gives: the inverse of acc_merge.  Defined only for the invertible kinds ACC_ROWS,
+// ACC_SUM_I64 (exact, wrapping) and ACC_SUM_F64 (up to rounding); MIN and MAX cannot be unmerged.
+__device__ __forceinline__ unsigned long long acc_unmerge(int kind, unsigned long long a, unsigned long long b) {
+  if (kind == ACC_SUM_F64)
+    return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) - __longlong_as_double((long long)b));
+  return a - b;
+}
+
+// Fire-and-forget global reductions (RED: no value comes back).  On a pointer loaded from memory, as accumulator
+// blocks often are, the compiler only knows a generic address, and atomicAdd and friends compile to a generic ATOM
+// with a shared-memory fallback; the explicit global address space makes every merge a RED.
+__device__ __forceinline__ void red_add_u64(unsigned long long* dst, unsigned long long v) {
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(__cvta_generic_to_global(dst)), "l"(v) : "memory");
+}
+
+// acc_merge of `v`, already in the accumulator's domain, into the accumulator `*dst` in global memory, as one RED.
+__device__ __forceinline__ void acc_red(int kind, unsigned long long* dst, unsigned long long v) {
+  switch (kind) {
+    case ACC_SUM_F64:
+      asm volatile("red.global.add.f64 [%0], %1;" ::"l"(__cvta_generic_to_global(dst)),
+                   "d"(__longlong_as_double((long long)v)) : "memory");
+      break;
+    case ACC_MIN_I64:
+      asm volatile("red.global.min.s64 [%0], %1;" ::"l"(__cvta_generic_to_global(dst)), "l"((long long)v) : "memory");
+      break;
+    case ACC_MAX_I64:
+      asm volatile("red.global.max.s64 [%0], %1;" ::"l"(__cvta_generic_to_global(dst)), "l"((long long)v) : "memory");
+      break;
+    default: red_add_u64(dst, v); break;
   }
 }
 
@@ -77,12 +121,18 @@ static __global__ void acc_fold_kernel(const __grid_constant__ FoldParams p) {
   }
 }
 
-// Output value of an aggregate of `agg_kind` (ARROYO_B200_AGG_*) whose accumulator holds `acc`: COUNT(*) is the row
-// count, AVG the f64 sum over the rows, anything else the accumulator itself.
+// The f64 bits of AVG over `rows` rows from the sum accumulator `acc` of `kind`: the f64 sum (ACC_SUM_F64, DataFusion's
+// AVG state) or the exact integer sum converted once (ACC_SUM_I64), over the rows.
+__device__ __forceinline__ unsigned long long acc_mean(int kind, unsigned long long acc, unsigned long long rows) {
+  const double num = kind == ACC_SUM_F64 ? __longlong_as_double((long long)acc) : (double)(long long)acc;
+  return (unsigned long long)__double_as_longlong(num / (double)rows);
+}
+
+// Output value of an aggregate of `agg_kind` (ARROYO_B200_AGG_*) whose accumulator holds `acc`, in a plan whose AVG
+// accumulators are ACC_SUM_F64: COUNT(*) is the row count, AVG acc_mean, anything else the accumulator itself.
 __device__ __forceinline__ unsigned long long agg_finalise(int agg_kind, unsigned long long acc, unsigned long long rows) {
   if (agg_kind == ARROYO_B200_AGG_COUNT_STAR) return rows;
-  if (agg_kind == ARROYO_B200_AGG_AVG_I64)
-    return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)acc) / (double)rows);
+  if (agg_kind == ARROYO_B200_AGG_AVG_I64) return acc_mean(ACC_SUM_F64, acc, rows);
   return acc;
 }
 

@@ -151,8 +151,7 @@ __global__ void __launch_bounds__(IA_THREADS) ia_ingest_kernel(const __grid_cons
 #pragma unroll
     for (int a = 1; a < MAX_ACC; ++a) {
       if (a >= p.g.n_acc) break;
-      const long long x = live ? __ldcs(p.val[p.acc_val[a]] + i) : 0;
-      v[a] = p.g.acc_kind[a] == ACC_SUM_F64 ? (unsigned long long)__double_as_longlong((double)x) : (unsigned long long)x;
+      v[a] = acc_of_value(p.g.acc_kind[a], live ? __ldcs(p.val[p.acc_val[a]] + i) : 0);
     }
     // combine the peers' values: at each step a lane folds in the value of the next peer above it that is still in
     // play, then every peer of odd rank drops out; after at most five steps the lowest peer holds the whole set's
@@ -172,11 +171,11 @@ __global__ void __launch_bounds__(IA_THREADS) ia_ingest_kernel(const __grid_cons
       rank >>= 1;
     }
     if (live && (int)lane == leader) {
-      atomicAdd(p.g.delta + id, (unsigned long long)__popc(peers));
+      acc_red(ACC_ROWS, p.g.delta + id, (unsigned long long)__popc(peers));
 #pragma unroll
       for (int a = 1; a < MAX_ACC; ++a) {
         if (a >= p.g.n_acc) break;
-        acc_atomic_merge(p.g.acc_kind[a], p.g.delta + (unsigned long long)a * p.g.cap + id, v[a]);
+        acc_red(p.g.acc_kind[a], p.g.delta + (unsigned long long)a * p.g.cap + id, v[a]);
       }
     }
   }
@@ -323,10 +322,8 @@ __global__ void ia_restore_kernel(const __grid_constant__ IRestore p) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (; i < p.n; i += stride) {
     const uint32_t id = ia_find_or_insert(p.g, p.ts[i], p.keyed ? p.key[i] : 0);
-    for (int a = 0; a < p.g.n_acc; ++a) {
-      const unsigned long long v = p.state[a] ? p.state[a][i] : 1ull;
-      acc_atomic_merge(p.g.acc_kind[a], p.g.base + (unsigned long long)a * p.g.cap + id, v);
-    }
+    for (int a = 0; a < p.g.n_acc; ++a)
+      acc_red(p.g.acc_kind[a], p.g.base + (unsigned long long)a * p.g.cap + id, p.state[a] ? p.state[a][i] : 1ull);
   }
 }
 

@@ -130,17 +130,12 @@ __device__ void merge_rows(const SessCtx& c, uint32_t id, const RowsRef& r, int 
       continue;
     }
     const long long* src = r.val[c.acc_val[a]] + r.off;
-    unsigned long long cur = *dst;
-    for (int i = lo; i < hi; ++i) {
-      const long long v = src[i];
-      switch (kind) {
-        case ACC_SUM_I64: cur += (unsigned long long)v; break;
-        case ACC_SUM_F64: cur = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)cur) + (double)v); break;
-        case ACC_MIN_I64: cur = (unsigned long long)min((long long)cur, v); break;
-        case ACC_MAX_I64: cur = (unsigned long long)max((long long)cur, v); break;
-      }
-    }
-    *dst = cur;
+    // in row order, so an f64 sum rounds as the reference's sequential accumulator does
+    *dst = acc_with_kind(kind, [&](auto k) {
+      unsigned long long cur = *dst;
+      for (int i = lo; i < hi; ++i) cur = acc_merge(k, cur, acc_of_value(k, src[i]));
+      return cur;
+    });
   }
 }
 

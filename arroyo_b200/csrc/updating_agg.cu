@@ -116,20 +116,15 @@ __global__ void __launch_bounds__(256) upd_ingest_kernel(const __grid_constant__
       }
     }
     if (TTL && p.last[id] != p.now) p.last[id] = p.now;  // every writer stores the same value
-    atomicAdd(p.st.cur + id, 1ull);
+    acc_red(ACC_ROWS, p.st.cur + id, 1ull);
 #pragma unroll
     for (int a = 1; a < MAX_ACC; ++a) {
       if (a >= p.st.n_acc) break;
+      const int kind = p.st.acc_kind[a];
       const long long v = __ldcs(p.val[p.st.acc_val[a]] + i);
-      unsigned long long* dst = p.st.cur + (unsigned long long)a * p.st.id_cap + id;
-      switch (p.st.acc_kind[a]) {
-        case ACC_SUM_I64: atomicAdd(dst, (unsigned long long)v); break;
-        case ACC_SUM_F64: atomicAdd(reinterpret_cast<double*>(dst), (double)v); break;
-        case ACC_MIN_I64: atomicMin(reinterpret_cast<long long*>(dst), v); break;
-        case ACC_MAX_I64: atomicMax(reinterpret_cast<long long*>(dst), v); break;
-      }
+      acc_red(kind, p.st.cur + (unsigned long long)a * p.st.id_cap + id, acc_of_value(kind, v));
     }
-    atomicMax(p.st.cur_ts + id, __ldcs(p.ts + i));
+    acc_red(ACC_MAX_I64, reinterpret_cast<unsigned long long*>(p.st.cur_ts + id), (unsigned long long)__ldcs(p.ts + i));
     if (atomicExch(p.st.touched + id, 1u) == 0u) {
       p.st.list[atomicAdd(p.st.n_touched, 1u)] = id;
       if (TTL && p.st.prev[id] == 0) atomicAdd(p.n_live, 1u);  // prev rows == 0: no rows at the last flush

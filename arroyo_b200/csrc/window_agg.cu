@@ -133,22 +133,6 @@ __device__ __forceinline__ const long long* ldg_ptr(const long long* const* pp) 
 // -------------------------------------------------------------------------------------------
 // ingest: window-assign + keyed partial aggregate
 // -------------------------------------------------------------------------------------------
-// RED (fire-and-forget reduction, no return trip).  The pane pointers come out of memory, so the
-// compiler only knows them as generic addresses and would emit the slower generic ATOM: state the
-// address space explicitly.
-__device__ __forceinline__ void red_add_u64(unsigned long long* a, unsigned long long v) {
-  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(__cvta_generic_to_global(a)), "l"(v) : "memory");
-}
-__device__ __forceinline__ void red_add_f64(unsigned long long* a, double v) {
-  asm volatile("red.global.add.f64 [%0], %1;" ::"l"(__cvta_generic_to_global(a)), "d"(v) : "memory");
-}
-__device__ __forceinline__ void red_min_s64(unsigned long long* a, long long v) {
-  asm volatile("red.global.min.s64 [%0], %1;" ::"l"(__cvta_generic_to_global(a)), "l"(v) : "memory");
-}
-__device__ __forceinline__ void red_max_s64(unsigned long long* a, long long v) {
-  asm volatile("red.global.max.s64 [%0], %1;" ::"l"(__cvta_generic_to_global(a)), "l"(v) : "memory");
-}
-
 __device__ __forceinline__ long long ring_bin(const IngestParams& p, uint32_t slot) {
   return p.ring_inline ? p.ring_bins[slot] : __ldg(p.pane_bins + slot);
 }
@@ -192,16 +176,8 @@ __device__ __noinline__ void defer_row(const IngestParams& p, long long key, lon
 // straight-line code.
 constexpr int GENERIC_SIG = -1;
 constexpr int sig_of(int k1, int k2 = 0, int k3 = 0) { return k1 | (k2 << 3) | (k3 << 6); }
-
-__device__ __forceinline__ void red_kind(int kind, unsigned long long* dst, long long v) {
-  switch (kind) {
-    case ACC_SUM_I64: red_add_u64(dst, (unsigned long long)v); break;
-    case ACC_SUM_F64: red_add_f64(dst, (double)v); break;
-    case ACC_MIN_I64: red_min_s64(dst, v); break;
-    case ACC_MAX_I64: red_max_s64(dst, v); break;
-    default: break;
-  }
-}
+// The kind of accumulator `a` (1..3) in signature `sig`, 0 when there is none.
+constexpr int sig_kind(int sig, int a) { return (sig >> (3 * (a - 1))) & 7; }
 
 // How many original rows an input row stands for: 1, or the carried count of a partial-aggregate row.
 __device__ __forceinline__ unsigned long long rows_of(const IngestParams& p, const Vals& v) {
@@ -220,15 +196,17 @@ __device__ __forceinline__ void accumulate(const IngestParams& p, const Vals& v,
       if (a < p.n_acc) {
         const int x = p.acc_val[a];
         const long long val = x == 0 ? v.v0 : x == 1 ? v.v1 : x == 2 ? v.v2 : v.v3;
-        red_kind(p.acc_kind[a], pane + (unsigned long long)a * p.id_cap + id, val);
+        const int kind = p.acc_kind[a];
+        acc_red(kind, pane + (unsigned long long)a * p.id_cap + id, acc_of_value(kind, val));
       }
     }
   } else {
     // at most one value column: every accumulator reads v0
-    constexpr int k1 = SIG & 7, k2 = (SIG >> 3) & 7, k3 = (SIG >> 6) & 7;
-    if (k1) red_kind(k1, pane + p.id_cap + id, v.v0);
-    if (k2) red_kind(k2, pane + 2 * p.id_cap + id, v.v0);
-    if (k3) red_kind(k3, pane + 3 * p.id_cap + id, v.v0);
+#pragma unroll
+    for (int a = 1; a <= 3; ++a) {
+      const int kind = sig_kind(SIG, a);
+      if (kind) acc_red(kind, pane + a * p.id_cap + id, acc_of_value(kind, v.v0));
+    }
   }
 }
 
@@ -308,36 +286,20 @@ __device__ __forceinline__ uint32_t hot_resolve(const IngestParams& p, const Pan
   return id;
 }
 
-__device__ __forceinline__ long long shfl_ll(unsigned mask, long long v, int src) {
-  return (long long)__shfl_sync(mask, (unsigned long long)v, src);
-}
-
-// Combines one accumulator across the lanes of `peers` (same pane, same id); valid in the leader.
-__device__ __forceinline__ long long group_reduce(int kind, unsigned peers, long long v) {
-  long long r = v;
+// Combines one accumulator across the lanes of `peers` (same pane, same id), in lane order; valid in the leader.
+__device__ __forceinline__ unsigned long long group_reduce(int kind, unsigned peers, unsigned long long v) {
+  unsigned long long r = v;
   bool first = true;
   for (unsigned m = peers; m; m &= m - 1) {
-    const long long x = shfl_ll(peers, v, __ffs(m) - 1);
+    const unsigned long long x = __shfl_sync(peers, v, __ffs(m) - 1);
     if (first) {
       r = x;
       first = false;
       continue;
     }
-    switch (kind) {
-      case ACC_SUM_I64: r = (long long)((unsigned long long)r + (unsigned long long)x); break;
-      case ACC_SUM_F64: r = __double_as_longlong(__longlong_as_double(r) + __longlong_as_double(x)); break;
-      case ACC_MIN_I64: r = min(r, x); break;
-      case ACC_MAX_I64: r = max(r, x); break;
-      default: break;
-    }
+    r = acc_merge(kind, r, x);
   }
   return r;
-}
-
-__device__ __forceinline__ void red_kind_combined(int kind, unsigned long long* dst, long long v) {
-  // v is already in the accumulator's domain (f64 bits for ACC_SUM_F64)
-  if (kind == ACC_SUM_F64) red_add_f64(dst, __longlong_as_double(v));
-  else red_kind(kind, dst, v);
 }
 
 // Convergent half: RED updates, after combining lanes of the warp that hit the same (pane, id).  Skewed
@@ -359,34 +321,35 @@ __device__ __forceinline__ void combine_accumulate(const IngestParams& p, const 
   if (p.rows_slot < 0) {
     if (fast && leader) red_add_u64(pane + id, (unsigned long long)__popc(peers));
   } else {
-    const long long r = group_reduce(ACC_SUM_I64, peers, (long long)rows_of(p, v));
-    if (fast && leader) red_add_u64(pane + id, (unsigned long long)r);
+    const unsigned long long r = group_reduce(ACC_ROWS, peers, rows_of(p, v));
+    if (fast && leader) red_add_u64(pane + id, r);
   }
   if (SIG == GENERIC_SIG) {
 #pragma unroll
     for (int a = 1; a < MAX_ACC; ++a) {
       if (a < p.n_acc) {
         const int x = p.acc_val[a];
-        long long val = x == 0 ? v.v0 : x == 1 ? v.v1 : x == 2 ? v.v2 : v.v3;
+        const long long val = x == 0 ? v.v0 : x == 1 ? v.v1 : x == 2 ? v.v2 : v.v3;
         const int kind = p.acc_kind[a];
-        if (kind == ACC_SUM_F64) val = __double_as_longlong((double)val);
-        const long long r = group_reduce(kind, peers, val);
-        if (fast && leader) red_kind_combined(kind, pane + (unsigned long long)a * p.id_cap + id, r);
+        const unsigned long long r = group_reduce(kind, peers, acc_of_value(kind, val));
+        if (fast && leader) acc_red(kind, pane + (unsigned long long)a * p.id_cap + id, r);
       }
     }
   } else {
-    constexpr int k1 = SIG & 7, k2 = (SIG >> 3) & 7, k3 = (SIG >> 6) & 7;
+    // Written out per accumulator: as a `#pragma unroll` loop (the form accumulate uses) this path compiles to
+    // longer code, with more warp shuffles and matches, than the straight-line form.
+    constexpr int k1 = sig_kind(SIG, 1), k2 = sig_kind(SIG, 2), k3 = sig_kind(SIG, 3);
     if (k1) {
-      const long long r = group_reduce(k1, peers, k1 == ACC_SUM_F64 ? __double_as_longlong((double)v.v0) : v.v0);
-      if (fast && leader) red_kind_combined(k1, pane + p.id_cap + id, r);
+      const unsigned long long r = group_reduce(k1, peers, acc_of_value(k1, v.v0));
+      if (fast && leader) acc_red(k1, pane + p.id_cap + id, r);
     }
     if (k2) {
-      const long long r = group_reduce(k2, peers, k2 == ACC_SUM_F64 ? __double_as_longlong((double)v.v0) : v.v0);
-      if (fast && leader) red_kind_combined(k2, pane + 2 * p.id_cap + id, r);
+      const unsigned long long r = group_reduce(k2, peers, acc_of_value(k2, v.v0));
+      if (fast && leader) acc_red(k2, pane + 2 * p.id_cap + id, r);
     }
     if (k3) {
-      const long long r = group_reduce(k3, peers, k3 == ACC_SUM_F64 ? __double_as_longlong((double)v.v0) : v.v0);
-      if (fast && leader) red_kind_combined(k3, pane + 3 * p.id_cap + id, r);
+      const unsigned long long r = group_reduce(k3, peers, acc_of_value(k3, v.v0));
+      if (fast && leader) acc_red(k3, pane + 3 * p.id_cap + id, r);
     }
   }
 }
@@ -544,7 +507,7 @@ __global__ void ingest_partial_kernel(const __grid_constant__ PartialParams p) {
   for (; i < p.n; i += stride) {
     const uint32_t id = p.ids[i];
     for (int a = 0; a < p.n_acc; ++a)
-      acc_atomic_merge(p.acc_kind[a], p.pane + (unsigned long long)a * p.id_cap + id, p.state[a] ? p.state[a][i] : 1ull);
+      acc_red(p.acc_kind[a], p.pane + (unsigned long long)a * p.id_cap + id, p.state[a] ? p.state[a][i] : 1ull);
   }
 }
 
@@ -586,12 +549,6 @@ struct EmitParams {
 
 constexpr int EMIT_THREADS = 256;
 
-__device__ __forceinline__ unsigned long long unmerge_acc(int kind, unsigned long long a, unsigned long long v) {
-  if (kind == ACC_SUM_F64)
-    return (unsigned long long)__double_as_longlong(__longlong_as_double((long long)a) - __longlong_as_double((long long)v));
-  return a - v;
-}
-
 // Finalises and writes one output row (K4 finalise + K5 projection).
 template <int NACC>
 __device__ __forceinline__ void emit_row(const EmitParams& p, unsigned int o, const unsigned long long (&acc)[NACC],
@@ -608,12 +565,8 @@ __device__ __forceinline__ void emit_row(const EmitParams& p, unsigned int o, co
 #pragma unroll
   for (int a = 0; a < NACC; ++a) {
     if (p.out_raw[a]) p.out_raw[a][o] = acc[a];
-    if (p.out_avg[a]) {
-      // f64 accumulator: sum of inputs cast to f64 (DataFusion's AVG state); integer accumulator: the exact
-      // sum, converted once (guarded against overflow on ingest)
-      const double num = p.acc_kind[a] == ACC_SUM_F64 ? __longlong_as_double((long long)acc[a]) : (double)(long long)acc[a];
-      p.out_avg[a][o] = (unsigned long long)__double_as_longlong(num / (double)rows);
-    }
+    // an integer sum accumulator is guarded against overflow on ingest
+    if (p.out_avg[a]) p.out_avg[a][o] = acc_mean(p.acc_kind[a], acc[a], rows);
   }
   if (p.out_wstart) {
     p.out_wstart[o] = p.wstart;
@@ -659,8 +612,8 @@ __global__ void __launch_bounds__(EMIT_THREADS) emit_kernel(const __grid_constan
             {
               const ulonglong2 v = __ldcs(reinterpret_cast<const ulonglong2*>(pane + (unsigned long long)a * p.id_cap + id));
               const int kind = p.acc_kind[a];
-              acc0[a] = add ? acc_merge(kind, acc0[a], v.x) : unmerge_acc(kind, acc0[a], v.x);
-              acc1[a] = add ? acc_merge(kind, acc1[a], v.y) : unmerge_acc(kind, acc1[a], v.y);
+              acc0[a] = add ? acc_merge(kind, acc0[a], v.x) : acc_unmerge(kind, acc0[a], v.x);
+              acc1[a] = add ? acc_merge(kind, acc1[a], v.y) : acc_unmerge(kind, acc1[a], v.y);
             }
         }
         // a key that left the window restarts from exactly zero (no f64 drift carried over)
@@ -1210,7 +1163,7 @@ void WindowAggOp::grow_ids() {
 __global__ void i64_to_f64_kernel(const unsigned long long* __restrict__ src, unsigned long long* __restrict__ dst, uint64_t n) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-  for (; i < n; i += stride) dst[i] = (unsigned long long)__double_as_longlong((double)(long long)src[i]);
+  for (; i < n; i += stride) dst[i] = acc_of_value(ACC_SUM_F64, (long long)src[i]);
 }
 
 // Leaves exact-sum AVG: every AVG gets its own f64 accumulator, seeded from the (still exact) integer sums.
