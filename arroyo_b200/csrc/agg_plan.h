@@ -269,11 +269,12 @@ struct StateBatches {
   // The column each accumulator is restored from; -1: none, which only the row count can lack (each row then counts
   // one).  The row count comes from COUNT(*)'s column, else the first count column; an accumulator from its first
   // column, but an Int64 one before a Float64 one: an exact-sum AVG shares its integer accumulator with a SUM over the
-  // same column, whose Int64 column restores it exactly.
+  // same column, and the window aggregate keeps that sharing on restore only where the two columns agree.
   int seed[MAX_ACC];
+  bool table_a = false;
 
-  StateBatches(const AggPlan& plan, bool table_a, const ArrowArray* state, const ArrowSchema* schemas, int64_t n)
-      : layout(plan.state_layout(table_a)), kc(plan.keyed ? 1 : 0) {
+  StateBatches(const AggPlan& plan, bool table_a_, const ArrowArray* state, const ArrowSchema* schemas, int64_t n)
+      : layout(plan.state_layout(table_a_)), kc(plan.keyed ? 1 : 0), table_a(table_a_) {
     if (n > 0) AB_REQUIRE(state != nullptr && schemas != nullptr, ARROYO_B200_INVALID_ARGUMENT, "null state batches");
     ts_col = kc + (int)layout.size() - (table_a ? 2 : 1);
     cols.resize((size_t)std::max<int64_t>(n, 0));
@@ -301,6 +302,13 @@ struct StateBatches {
       }
       total += rows[b];
     }
+    assign_seeds(plan);
+  }
+
+  // Fills `seed` for `plan`, which has the layout the batches were checked against: a plan that changed only which
+  // accumulator an aggregate reads (the window aggregate's AVG promotion) restores from the same columns.
+  void assign_seeds(const AggPlan& plan) {
+    layout = plan.state_layout(table_a);
     for (int a = 0; a < MAX_ACC; ++a) seed[a] = -1;
     for (size_t j = 0; j < layout.size(); ++j) {
       const StateCol& sc = layout[j];

@@ -728,7 +728,8 @@ class WindowAggOp final : public OpBase {
   // AVG(Int64) from the exact integer sum instead of a separate f64 RED per row (one scattered access
   // less per row).  Valid while no per-key sum can overflow i64: every guarded value is < 2^31 in
   // magnitude (checked per row on the device) and no window holds 2^32 rows (checked on the host);
-  // otherwise the operator promotes itself to f64 accumulators (promote_avg).  The result differs from
+  // otherwise the operator promotes itself to f64 accumulators (promote_avg).  A restore keeps exact mode
+  // only for state that could have come from such rows (restore_is_exact).  The result differs from
   // DataFusion's running f64 sum by at most n * 2^-53 relative (north-star tolerance: 1e-6).
   bool avg_exact_ = true;
   unsigned int guard_vals_ = 0;
@@ -869,6 +870,7 @@ class WindowAggOp final : public OpBase {
   void rebuild_blocks(Fill fill);
   void grow_ids();
   void promote_avg();
+  bool restore_is_exact(const StateBatches& sb) const;
   unsigned long long* acquire_block();
   void release_block(unsigned long long* blk);
   void init_block(unsigned long long* blk, uint64_t n_ids);
@@ -2388,11 +2390,50 @@ void WindowAggOp::handle_checkpoint(int64_t wm, BatchesPriv* out) {
   collect_emit_times();
 }
 
+// Whether exact-sum AVG (avg_exact_) stays valid with the state of `sb` merged in: the restored state must be what rows
+// that passed the ingest guard can give.  Every AVG's Float64 [sum] is then an integer below 2^53 in magnitude (so it is
+// the exact sum), at most 2^31 per row of its count, and equal to the Int64 [sum] of a SUM that shares its accumulator;
+// and no pane holds 2^31 rows (absorb's bound).  A table written after a promotion, or by the reference, may hold a
+// wrapped Int64 [sum] next to the f64 sum, f64 sums of 2^53 and more, or any count.
+bool WindowAggOp::restore_is_exact(const StateBatches& sb) const {
+  std::map<int64_t, uint64_t> pane_rows;
+  for (size_t bi = 0; bi < sb.cols.size(); ++bi) {
+    const int64_t rows = sb.rows[bi];
+    if (rows == 0) continue;
+    const std::vector<InColumn>& cols = sb.cols[bi];
+    const uint64_t* count = sb.seed[0] >= 0 ? cols[sb.seed[0]].data : nullptr;
+    uint64_t& in_pane = pane_rows[bin_start((int64_t)cols[sb.ts_col].data[0], slide_)];
+    for (int64_t i = 0; i < rows; ++i) {
+      const uint64_t c = count ? count[i] : 1;
+      if (c >= (1ull << 31) || (in_pane += c) >= (1ull << 31)) return false;
+    }
+    for (size_t j = 0; j < sb.layout.size(); ++j) {
+      const StateCol& sc = sb.layout[j];
+      if (sc.role != S_ACC || plan_.acc_kind[sc.acc] != ACC_SUM_I64 || strcmp(sc.format, "g")) continue;
+      const double* sum = (const double*)cols[sb.kc + j].data;
+      const int shared = sb.seed[sc.acc];
+      const long long* isum = strcmp(sb.layout[shared - sb.kc].format, "g") ? (const long long*)cols[shared].data : nullptr;
+      for (int64_t i = 0; i < rows; ++i) {
+        const double s = sum[i], c = count ? (double)count[i] : 1.0;
+        if (!(std::fabs(s) < 0x1p53) || s != std::trunc(s) || std::fabs(s) > c * 0x1p31) return false;
+        if (isum && isum[i] != (long long)s) return false;
+      }
+    }
+  }
+  return true;
+}
+
 // Restore (tumbling :228-248, sliding :556-595): partial batches go back into pane blocks, one batch at a time (a
-// batch holds one pane), once every batch has been checked.
+// batch holds one pane), once every batch has been checked.  An operator in exact-sum AVG mode first promotes itself
+// unless the state keeps that mode valid (restore_is_exact); each AVG's f64 accumulator then starts from its own
+// Float64 [sum], the reference's AVG state, and a SUM's from its Int64 [sum].
 void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, int64_t watermark, int64_t table_min) {
   set_device();
-  const StateBatches sb(plan_, false, state, schemas, n);
+  StateBatches sb(plan_, false, state, schemas, n);
+  if (avg_exact_ && !restore_is_exact(sb)) {
+    promote_avg();
+    sb.assign_seeds(plan_);
+  }
   const bool has_wm = watermark != INT64_MIN;
   if (has_wm) late_bin_ = std::max<int64_t>(late_bin_, bin_start(watermark, slide_));
   if (sliding_) sliding_planner_->restore_begin(has_wm, watermark);
@@ -2425,11 +2466,11 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
       const int c = sb.seed[a];
       if (c < 0) continue;
       if (plan_.acc_kind[a] == ACC_SUM_I64 && !strcmp(sb.layout[c - sb.kc].format, "g")) {
-        // exact-sum AVG without a SUM over the same column: the checkpoint only has the f64 image of the sum
-        // (exact below 2^53)
+        // exact-sum AVG without a SUM over the same column: the checkpoint only has the f64 image of the sum, an
+        // integer below 2^53 (restore_is_exact)
         conv[a].resize((size_t)rows);
         const double* d = (const double*)cols[c].data;
-        for (int64_t i = 0; i < rows; ++i) conv[a][(size_t)i] = (long long)__builtin_llround(d[i]);
+        for (int64_t i = 0; i < rows; ++i) conv[a][(size_t)i] = (long long)d[i];
         d_acc[a].alloc((size_t)rows * 8);
         AB_CUDA(cudaMemcpyAsync(d_acc[a].p, conv[a].data(), (size_t)rows * 8, cudaMemcpyHostToDevice, stream_));
         st_.h2d_bytes += (uint64_t)rows * 8;
@@ -2453,6 +2494,9 @@ void WindowAggOp::on_start(ArrowArray* state, ArrowSchema* schemas, int64_t n, i
     ingest_partial_kernel<<<std::max(grid, 1), 256, 0, stream_>>>(pp);
     AB_CUDA(cudaGetLastError());
     ++st_.kernel_launches;
+    // the restored rows count toward the exact-AVG row bounds like ingested ones (emit_window)
+    const uint64_t* count = sb.seed[0] >= 0 ? cols[sb.seed[0]].data : nullptr;
+    for (int64_t i = 0; i < rows; ++i) p.rows += count ? count[i] : 1;
     // the batch's device copies and `conv` are done with once the stream has passed this read
     Counters c{};
     AB_CUDA(cudaMemcpyAsync(&c, book_.p, sizeof c, cudaMemcpyDeviceToHost, stream_));
