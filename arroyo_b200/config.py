@@ -59,6 +59,16 @@ class JoinConfig:
 
 
 @dataclass
+class WindowFrame:
+    """A window function's explicit frame, `{ROWS | RANGE | GROUPS} BETWEEN start AND end`: `units` is rows, range or
+    groups; `start` and `end` are each "unbounded_preceding", "current_row" or "unbounded_following", or a pair
+    ("preceding" | "following", n) with n >= 0 (nanoseconds for RANGE over a timestamp key)."""
+    units: str
+    start: object
+    end: object
+
+
+@dataclass
 class WindowFunctionConfig:
     """WindowFunctionOperator (arroyo-worker/src/arrow/window_fn.rs): `function` (row_number | rank | dense_rank,
     the aggregate sum | count | avg | min | max of column `argument`, which count ignores, the value function lag |
@@ -67,7 +77,8 @@ class WindowFunctionConfig:
     (column, descending); it may be empty for every function but the ranking ones, the frame then being the whole
     partition.  `top_n` > 0 fuses the `WHERE name <= top_n` that follows a ranking function; 0 lets every row through.
     `offset` is lag / lead's k (>= 0) or nth_value's n (>= 1); `default` is lag / lead's default, in the argument's
-    type (None: NULL)."""
+    type (None: NULL).  `frame` is the frame of an aggregate or of first_value / last_value / nth_value (None: the
+    default frame)."""
     function: str
     partition_by: Optional[str]
     order_by: List[tuple]
@@ -76,3 +87,4 @@ class WindowFunctionConfig:
     argument: Optional[str] = None
     offset: int = 1
     default: Optional[object] = None
+    frame: Optional[WindowFrame] = None

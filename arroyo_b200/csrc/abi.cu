@@ -99,7 +99,8 @@ int64_t hand_out(OpBase* o, std::vector<ArroyoB200DeviceBatch>& v, ArroyoB200Dev
 
 extern "C" {
 
-int32_t arroyo_b200_abi_version(void) { return 1; }
+// 2: ArroyoB200OpConfig gained `frame` at its end (192 -> 224 bytes)
+int32_t arroyo_b200_abi_version(void) { return 2; }
 
 int32_t arroyo_b200_device_count(void) {
   int n = 0;

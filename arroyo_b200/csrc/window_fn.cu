@@ -1,8 +1,9 @@
 // Window function on sm_90a (H100): the GPU side of `WindowFunctionOperator` (arroyo-worker/src/arrow/window_fn.rs),
 // for ROW_NUMBER / RANK / DENSE_RANK () OVER (PARTITION BY window [, key] ORDER BY k1 [DESC], ...), optionally fused
 // with the `WHERE fn <= N` that usually follows it (top N per window), for COUNT(*) / SUM / AVG / MIN / MAX (x)
-// OVER (PARTITION BY window [, key] [ORDER BY ...]) over the default frame, and for LAG / LEAD / FIRST_VALUE /
-// LAST_VALUE / NTH_VALUE (x, ...) and PERCENT_RANK / CUME_DIST () over the same partitions.  The planner
+// OVER (PARTITION BY window [, key] [ORDER BY ...]) over the default frame or an explicit ROWS / RANGE / GROUPS frame,
+// and for LAG / LEAD / FIRST_VALUE / LAST_VALUE / NTH_VALUE (x, ...) and PERCENT_RANK / CUME_DIST () over the same
+// partitions (FIRST_VALUE / LAST_VALUE / NTH_VALUE over an explicit frame too).  The planner
 // (plan/window_fn.rs:101-105) drops the `window` column from PARTITION BY: each upstream window stamps its rows with one
 // `_timestamp`, so the rows are bucketed by `_timestamp` ("instant") and the remaining PARTITION BY column, if any,
 // splits each instant further.
@@ -511,6 +512,203 @@ __global__ void __launch_bounds__(WF_TILE) wf_value_apply_kernel(const __grid_co
   if (p.valid) p.valid[j] = ok ? 1u : 0u;
 }
 
+// ---- explicit frames --------------------------------------------------------------------------------------------------
+// An aggregate or FIRST_VALUE / LAST_VALUE / NTH_VALUE over `{ROWS | RANGE | GROUPS} BETWEEN start AND end`.  Sorted
+// row j of a segment [s, e] gets the half-open frame [lo, hi) of sorted rows, clipped to [s, e + 1); lo >= hi is an
+// empty frame.  Each bound is found from the rank scan (s, the peer group's first row g, the dense rank d) and
+// wf_bounds_kernel's e and peer-group ends:
+//   ROWS    row j - n / j / j + n (an end one past it);
+//   GROUPS  the first row of peer group d - n / d / d + n (an end: of the group after it), through a map from each
+//           segment's group ordinals to their first rows (wf_groups_kernel);
+//   RANGE   CURRENT ROW: g, or one past the peer group's last row; n PRECEDING / FOLLOWING: a binary search in [s, e + 1)
+//           of the one ORDER BY key in its sort's unsigned order-preserving form u, for u >= u(j) -/+ n (a start) or
+//           u > u(j) -/+ n (an end); a limit u(j) -/+ n outside [0, 2^64) is before or after every row.  That form has
+//           slope +-1, so under DESC "n PRECEDING" is keys up to x + n.
+// ROWS and GROUPS offsets are clamped to 2^32 before any arithmetic: a segment has fewer than 2^31 rows, so a larger n
+// reaches as far.  lo and hi are non-decreasing in j within a segment.  The values over [lo, hi):
+//   COUNT hi - lo; SUM / AVG differences of prefix sums over the sorted rows, kept exact as the low 32 bits and the
+//   high 32 bits (signed, biased by 2^31) of each value, so SUM wraps and AVG converts the exact sum to f64 once;
+//   MIN / MAX a range-extremum query: 32-row blocks with in-block prefix and suffix extremes, a sparse table over the
+//   block extremes, and a scan of at most 32 values when lo and hi - 1 share a block;
+//   FIRST_VALUE / LAST_VALUE / NTH_VALUE the argument at lo, hi - 1, lo + n - 1 (NULL past hi - 1).
+// Every function but COUNT is NULL on an empty frame.
+constexpr unsigned long long FRAME_OFFSET_CAP = 1ull << 32;
+
+struct WFrame {
+  WValue b;                  // the rank scan, wf_bounds_kernel's peer_last / seg_last, fn, NTH_VALUE's n - 1, fv, valid
+  int units, start_kind, end_kind;
+  unsigned long long start_off, end_off;
+  const unsigned long long* ukey;  // RANGE with an offset: per sorted row its ORDER BY key, unsigned order-preserving
+  unsigned int* gfirst;            // GROUPS: at s + d - 1 the first row of the segment's d-th peer group
+  unsigned int* gcount;            // GROUPS: at s the segment's number of peer groups
+  const unsigned long long* pre_lo;  // SUM / AVG: at j (0 .. n) the sums over sorted rows [0, j) of the values' low
+  const unsigned long long* pre_hi;  //   32 bits and of their high 32 bits + 2^31 (the signed high half, biased)
+  const long long* v;              // MIN / MAX: per sorted row the argument
+  const long long* in_pre;         //   per sorted row the extreme of its 32-row block's rows up to it
+  const long long* in_suf;         //   ... and from it on
+  const long long* table;          //   level k (k * n_blocks on): per block b the extreme of blocks [b, b + 2^k)
+  long long n_blocks;
+};
+
+// GROUPS: each segment's peer groups by ordinal, and its group count
+__global__ void __launch_bounds__(WF_TILE) wf_groups_kernel(const __grid_constant__ WFrame p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  const unsigned int bits = j < p.b.n ? p.b.bits[j] : 0u;
+  const RankVal r = value_scan(p.b, j, bits);
+  if (j >= p.b.n) return;
+  const unsigned int s = r.seg - 1u;
+  if (bits & 4u) p.gfirst[s + r.dcnt - 1u] = (unsigned int)j;
+  const unsigned int next = j + 1 < p.b.n ? p.b.bits[j + 1] : 6u;
+  if (next & 2u) p.gcount[s] = r.dcnt;
+}
+
+// the first row in [a, b) whose key is > t (`strict`) or >= t
+__device__ __forceinline__ unsigned int key_search(const unsigned long long* u, unsigned int a, unsigned int b,
+                                                   unsigned long long t, bool strict) {
+  while (a < b) {
+    const unsigned int m = a + (b - a) / 2;
+    const unsigned long long x = u[m];
+    if (strict ? x <= t : x < t) a = m + 1;
+    else b = m;
+  }
+  return a;
+}
+
+// One end of row j's frame, in [s, e + 1]: the start (`end` false) or one past the end.
+__device__ __forceinline__ unsigned int frame_edge(const WFrame& p, int kind, unsigned long long off, bool end,
+                                                   unsigned int j, unsigned int s, unsigned int e, const RankVal& r) {
+  if (kind == ARROYO_B200_BOUND_UNBOUNDED_PRECEDING) return s;
+  if (kind == ARROYO_B200_BOUND_UNBOUNDED_FOLLOWING) return e + 1u;
+  const bool cur = kind == ARROYO_B200_BOUND_CURRENT_ROW, back = kind == ARROYO_B200_BOUND_PRECEDING;
+  if (p.units == ARROYO_B200_FRAME_RANGE) {
+    const unsigned int g = r.peer - 1u;
+    if (cur) return end ? p.b.peer_last[g] + 1u : g;
+    // a limit past the key type's range lies before every row (PRECEDING) or after every row (FOLLOWING)
+    const unsigned long long u = p.ukey[j];
+    if (back ? u < off : off > ~u) return back ? s : e + 1u;
+    return key_search(p.ukey, s, e + 1u, back ? u - off : u + off, end);
+  }
+  const long long n = cur ? 0 : (long long)(off < FRAME_OFFSET_CAP ? off : FRAME_OFFSET_CAP);
+  const long long k = (back ? -n : n) + (end ? 1 : 0);
+  if (p.units == ARROYO_B200_FRAME_ROWS) {
+    const long long x = (long long)j + k;
+    return x < (long long)s ? s : x > (long long)e + 1 ? e + 1u : (unsigned int)x;
+  }
+  const long long d = (long long)r.dcnt + k;  // GROUPS: the ordinal of the peer group the edge starts
+  return d < 1 ? s : d > (long long)p.gcount[s] ? e + 1u : p.gfirst[s + (unsigned int)d - 1u];
+}
+
+// MIN / MAX of the sorted rows [a, b], a <= b
+template <int K>
+__device__ __forceinline__ long long range_extreme(const WFrame& p, unsigned int a, unsigned int b) {
+  const unsigned int ba = a >> 5, bb = b >> 5;
+  if (ba == bb) {
+    long long x = p.v[a];
+    for (unsigned int i = a + 1; i <= b; ++i) x = AggOp<K>::op(x, p.v[i]);
+    return x;
+  }
+  long long x = AggOp<K>::op(p.in_suf[a], p.in_pre[b]);
+  if (bb > ba + 1) {
+    const unsigned int l = ba + 1, h = bb - 1;
+    const int k = 31 - __clz(h - l + 1);
+    const long long* t = p.table + (long long)k * p.n_blocks;
+    x = AggOp<K>::op(x, AggOp<K>::op(t[l], t[h + 1 - (1u << k)]));
+  }
+  return x;
+}
+
+// each sorted row's frame and its value over it (F: an ArroyoB200AggKind, or FN_FIRST_VALUE .. FN_NTH_VALUE)
+template <int F>
+__global__ void __launch_bounds__(WF_TILE) wf_frame_apply_kernel(const __grid_constant__ WFrame p) {
+  const long long j = (long long)blockIdx.x * WF_TILE + threadIdx.x;
+  const unsigned int bits = j < p.b.n ? p.b.bits[j] : 0u;
+  const RankVal r = value_scan(p.b, j, bits);
+  if (j >= p.b.n) return;
+  const unsigned int row = (unsigned int)j, s = r.seg - 1u, e = p.b.seg_last[s];
+  const unsigned int lo = frame_edge(p, p.start_kind, p.start_off, false, row, s, e, r);
+  const unsigned int hi = frame_edge(p, p.end_kind, p.end_off, true, row, s, e, r);
+  bool ok = lo < hi;
+  unsigned long long v = 0;
+  if constexpr (F == ARROYO_B200_AGG_COUNT_STAR) {
+    v = ok ? hi - lo : 0u;
+    ok = true;
+  } else if constexpr (F == ARROYO_B200_AGG_SUM_I64 || F == ARROYO_B200_AGG_AVG_I64) {
+    if (ok) {
+      const unsigned long long sl = p.pre_lo[hi] - p.pre_lo[lo];
+      const long long sh = (long long)(p.pre_hi[hi] - p.pre_hi[lo] - ((unsigned long long)(hi - lo) << 31));
+      if constexpr (F == ARROYO_B200_AGG_SUM_I64) v = ((unsigned long long)sh << 32) + sl;
+      else v = (unsigned long long)__double_as_longlong((double)(((__int128)sh << 32) + (__int128)sl) / (double)(hi - lo));
+    }
+  } else if constexpr (F == ARROYO_B200_AGG_MIN_I64 || F == ARROYO_B200_AGG_MAX_I64) {
+    if (ok) v = (unsigned long long)range_extreme<F>(p, lo, hi - 1u);
+  } else {
+    unsigned int src = lo;  // FIRST_VALUE
+    if constexpr (F == ARROYO_B200_FN_LAST_VALUE) src = hi - 1u;
+    if constexpr (F == ARROYO_B200_FN_NTH_VALUE) {
+      ok = ok && p.b.offset < (unsigned long long)(hi - lo);  // compared before it is narrowed
+      src = lo + (unsigned int)p.b.offset;
+    }
+    if (ok) v = p.b.arg[p.b.idx[src]];
+  }
+  p.b.fv[j] = v;
+  if (p.b.valid) p.b.valid[j] = ok ? 1u : 0u;
+}
+
+// SUM / AVG: sorted row j's value as two 32-bit counts for device_exclusive_scan: lo[j] its low 32 bits, hi[j] its
+// high 32 bits + 2^31
+__global__ void wf_split_kernel(const unsigned long long* __restrict__ arg, const unsigned int* __restrict__ idx,
+                                long long n, unsigned int* __restrict__ lo, unsigned int* __restrict__ hi) {
+  long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; j < n; j += stride) {
+    const unsigned long long x = arg[idx[j]];
+    lo[j] = (unsigned int)x;
+    hi[j] = (unsigned int)(x >> 32) ^ 0x80000000u;
+  }
+}
+
+// MIN / MAX: the sorted values, their in-block prefix and suffix extremes and level 0 of the sparse table (one warp per
+// 32-row block; rows past n take the identity)
+struct WRmq {
+  const unsigned long long* arg;
+  const unsigned int* idx;
+  long long n;
+  long long* v;
+  long long* in_pre;
+  long long* in_suf;
+  long long* table;
+  long long n_blocks;
+};
+template <int K>
+__global__ void __launch_bounds__(WF_THREADS) wf_rmq_blocks_kernel(const __grid_constant__ WRmq p) {
+  const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned lane = threadIdx.x & 31;
+  const long long x = j < p.n ? (long long)p.arg[p.idx[j]] : AggOp<K>::identity();
+  long long up = x, down = x;
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long a = __shfl_up_sync(FULL, up, o), b = __shfl_down_sync(FULL, down, o);
+    if ((int)lane >= o) up = AggOp<K>::op(a, up);
+    if ((int)lane + o < 32) down = AggOp<K>::op(down, b);
+  }
+  if (j < p.n) {
+    p.v[j] = x;
+    p.in_pre[j] = up;
+    p.in_suf[j] = down;
+  }
+  if (lane == 0 && (j >> 5) < p.n_blocks) p.table[j >> 5] = down;
+}
+
+// level k of the sparse table from level k - 1 (a range past the last block is clipped to it)
+template <int K>
+__global__ void wf_rmq_level_kernel(long long* table, long long n_blocks, int k) {
+  const long long* prev = table + (long long)(k - 1) * n_blocks;
+  long long* cur = table + (long long)k * n_blocks;
+  const long long half = 1ll << (k - 1);
+  long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; b < n_blocks; b += stride) cur[b] = AggOp<K>::op(prev[b], prev[b + half < n_blocks ? b + half : n_blocks - 1]);
+}
+
 // out[c][o] = store[c][idx[j]] for the kept rows (keep null: every row, o = j), and the function column: fn[j], or
 // fn[at[j]] when `at` is given, with its validity byte from `valid` when that is given
 struct WGather {
@@ -606,6 +804,7 @@ class WindowFnOp final : public OpBase {
   uint64_t offset_ = 0;      // LAG / LEAD: k; NTH_VALUE: n - 1
   uint64_t dflt_ = 0;        // LAG / LEAD: the default's bits
   bool has_default_ = false;
+  ArroyoB200WindowFrame frame_{};  // units 0: the default frame (a default-equivalent frame is normalised to it)
   Layout layout_;
   bool typed_ = false;  // layout_ comes from a host or state batch (else: Int64 columns, no structs)
   int64_t late_wm_ = LLONG_MIN;
@@ -618,6 +817,7 @@ class WindowFnOp final : public OpBase {
   uint64_t stage_cap_ = 0;
   DevBuf flag_, off_, sums_, idx_[2], key_[2], cub_tmp_, bits_, tiles_, fnv_, keep_, off2_, agg_tiles_, at_;
   DevBuf seg_last_, valid_;  // value functions: each segment's last row at its first, each row's validity
+  DevBuf gfirst_, gcount_, pre_, rmq_, table_;  // explicit frames: see WFrame
   DevBuf out_[ARROYO_B200_MAX_COLS], out_fn_, out_valid_, out_bits_;
   ArroyoB200Stats st_{};
 
@@ -627,8 +827,11 @@ class WindowFnOp final : public OpBase {
   WCounters* counters() const { return counters_.as<WCounters>(); }
   bool ranking() const { return fn_ <= ARROYO_B200_FN_DENSE_RANK; }
   bool value_fn() const { return fn_ >= ARROYO_B200_FN_LAG && fn_ <= ARROYO_B200_FN_NTH_VALUE; }
-  // LAG / LEAD / NTH_VALUE may give NULL; `null_rows()`: with these arguments some row can be NULL
+  // LAG / LEAD / NTH_VALUE, and under an explicit frame every function but COUNT, may give NULL; `null_rows()`: with
+  // these arguments some row can be NULL
   bool nullable() const {
+    if (frame_.units != ARROYO_B200_FRAME_DEFAULT)
+      return !(fn_ == ARROYO_B200_FN_AGGREGATE && agg_kind_ == ARROYO_B200_AGG_COUNT_STAR);
     return fn_ == ARROYO_B200_FN_LAG || fn_ == ARROYO_B200_FN_LEAD || fn_ == ARROYO_B200_FN_NTH_VALUE;
   }
   bool null_rows() const { return nullable() && !has_default_; }
@@ -654,6 +857,9 @@ class WindowFnOp final : public OpBase {
   }
   void aggregate(const WRank& r, uint64_t n_tiles);
   void values(const WRank& r, uint64_t n_tiles);
+  void framed(const WRank& r, uint64_t n_tiles);
+  void check_frame(const ArroyoB200WindowFrame& f);
+  unsigned long long flip_of(int col, bool desc) const;
   Layout layout_of(const std::vector<InColumn>& cols, const std::vector<Nest>& nests, const ArrowSchema* s) const;
   void check_layout(const Layout& l, int bad_type_status) const;
   void adopt(const Layout& l);
@@ -753,6 +959,7 @@ WindowFnOp::WindowFnOp(const ArroyoB200OpConfig& c) {
     order_col_[k] = a.input_col;
     order_desc_[k] = a.kind == ARROYO_B200_ORDER_DESC;
   }
+  check_frame(c.frame);
   for (int f = 0; f < n_cols_; ++f) {
     layout_.names.push_back(f == ts_col_ ? "_timestamp" : "c" + std::to_string(f));
     layout_.formats.push_back(f == ts_col_ ? "tsn:" : "l");
@@ -763,6 +970,47 @@ WindowFnOp::WindowFnOp(const ArroyoB200OpConfig& c) {
   cap_ = 1u << 16;
   alloc_store(cur_, cap_);
   AB_CUDA(cudaStreamSynchronize(stream_));
+}
+
+// The frame clause: refusals as DataFusion's planner refuses them (INVALID_ARGUMENT), a start after the end, which
+// SQLite refuses and nothing here pins, UNSUPPORTED; a frame equal to the default is kept as units 0, so that it runs
+// the default frame's kernels and gives their bits.
+void WindowFnOp::check_frame(const ArroyoB200WindowFrame& f) {
+  AB_REQUIRE(f.units >= ARROYO_B200_FRAME_DEFAULT && f.units <= ARROYO_B200_FRAME_GROUPS, ARROYO_B200_INVALID_ARGUMENT,
+             "window function: frame.units must be DEFAULT (0), ROWS (1), RANGE (2) or GROUPS (3)");
+  if (f.units == ARROYO_B200_FRAME_DEFAULT) return;
+  const bool takes_frame = fn_ == ARROYO_B200_FN_AGGREGATE || fn_ == ARROYO_B200_FN_FIRST_VALUE ||
+                           fn_ == ARROYO_B200_FN_LAST_VALUE || fn_ == ARROYO_B200_FN_NTH_VALUE;
+  AB_REQUIRE(takes_frame, ARROYO_B200_INVALID_ARGUMENT,
+             std::string("window function: ") + fn_name() + " takes no frame (frame.units must be 0)");
+  auto bound_ok = [](int k) {
+    return k >= ARROYO_B200_BOUND_UNBOUNDED_PRECEDING && k <= ARROYO_B200_BOUND_UNBOUNDED_FOLLOWING;
+  };
+  AB_REQUIRE(bound_ok(f.start_kind) && bound_ok(f.end_kind), ARROYO_B200_INVALID_ARGUMENT,
+             "window function: frame.start_kind / end_kind must be ArroyoB200FrameBound codes (1 to 5)");
+  AB_REQUIRE(f.start_kind != ARROYO_B200_BOUND_UNBOUNDED_FOLLOWING, ARROYO_B200_INVALID_ARGUMENT,
+             "window function: a frame cannot start at UNBOUNDED FOLLOWING");
+  AB_REQUIRE(f.end_kind != ARROYO_B200_BOUND_UNBOUNDED_PRECEDING, ARROYO_B200_INVALID_ARGUMENT,
+             "window function: a frame cannot end at UNBOUNDED PRECEDING");
+  auto offset = [](int k) { return k == ARROYO_B200_BOUND_PRECEDING || k == ARROYO_B200_BOUND_FOLLOWING; };
+  AB_REQUIRE((!offset(f.start_kind) || f.start_offset >= 0) && (!offset(f.end_kind) || f.end_offset >= 0),
+             ARROYO_B200_INVALID_ARGUMENT, "window function: a frame offset must be >= 0");
+  AB_REQUIRE(f.units != ARROYO_B200_FRAME_RANGE || !(offset(f.start_kind) || offset(f.end_kind)) || n_order_ == 1,
+             ARROYO_B200_INVALID_ARGUMENT, "window function: a RANGE frame with an offset takes exactly one ORDER BY key");
+  AB_REQUIRE(f.units != ARROYO_B200_FRAME_GROUPS || n_order_ >= 1, ARROYO_B200_INVALID_ARGUMENT,
+             "window function: a GROUPS frame takes an ORDER BY");
+  const bool after = (f.start_kind == ARROYO_B200_BOUND_FOLLOWING && (f.end_kind == ARROYO_B200_BOUND_CURRENT_ROW ||
+                                                                     f.end_kind == ARROYO_B200_BOUND_PRECEDING)) ||
+                     (f.start_kind == ARROYO_B200_BOUND_CURRENT_ROW && f.end_kind == ARROYO_B200_BOUND_PRECEDING);
+  AB_REQUIRE(!after, ARROYO_B200_UNSUPPORTED,
+             "window function: a frame that starts after its end (n FOLLOWING AND CURRENT ROW | m PRECEDING, CURRENT "
+             "ROW AND m PRECEDING) is not supported");
+  const bool is_default =
+      n_order_ > 0 ? f.units == ARROYO_B200_FRAME_RANGE && f.start_kind == ARROYO_B200_BOUND_UNBOUNDED_PRECEDING &&
+                         f.end_kind == ARROYO_B200_BOUND_CURRENT_ROW
+                   : f.start_kind == ARROYO_B200_BOUND_UNBOUNDED_PRECEDING &&
+                         f.end_kind == ARROYO_B200_BOUND_UNBOUNDED_FOLLOWING;
+  if (!is_default) frame_ = f;
 }
 
 // The flat layout of an imported batch: names and formats per flat column, and its struct columns.
@@ -959,6 +1207,12 @@ void WindowFnOp::process_device_batch(uint32_t, uint32_t, const uint64_t* cols, 
   ingest((const unsigned long long* const*)cols, n_rows, late_wm_);
 }
 
+// What a sort key's 64 bits are XORed with to sort as unsigned: the sign bit for signed types, every bit for DESC.
+unsigned long long WindowFnOp::flip_of(int col, bool desc) const {
+  const unsigned long long f = layout_.formats[col] == "L" ? 0ull : 1ull << 63;
+  return desc ? ~f : f;
+}
+
 // Sorts the `e` store indices in idx_[0] and returns the buffer holding the sorted ones: stable LSD radix passes from
 // arrival order, the ORDER BY keys last to first, the partition key, then `_timestamp` (`by_ts_only`: that pass alone).
 unsigned int* WindowFnOp::sort_rows(uint64_t e, bool by_ts_only) {
@@ -971,11 +1225,6 @@ unsigned int* WindowFnOp::sort_rows(uint64_t e, bool by_ts_only) {
     int end_bit;
   };
   std::vector<Pass> passes;
-  const unsigned long long sign = 1ull << 63;
-  auto flip_of = [&](int col, bool desc) {
-    const unsigned long long f = layout_.formats[col] == "L" ? 0ull : sign;
-    return desc ? ~f : f;
-  };
   if (!by_ts_only) {
     for (int k = n_order_ - 1; k >= 0; --k) passes.push_back({order_col_[k], flip_of(order_col_[k], order_desc_[k]), 64});
     if (key_col_ >= 0) passes.push_back({key_col_, flip_of(key_col_, false), 64});
@@ -1064,7 +1313,10 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
   wf_carry_kernel<RankVal><<<1, 1024, 0, stream_>>>(r.tiles, (long long)n_tiles);
   AB_CUDA(cudaGetLastError());
   unsigned long long m = e, n_inst = 0;
-  if (agg) {
+  const bool frame = frame_.units != ARROYO_B200_FRAME_DEFAULT;
+  if (frame) {
+    framed(r, n_tiles);  // every row leaves
+  } else if (agg) {
     aggregate(r, n_tiles);  // every row leaves
   } else if (!rank) {
     values(r, n_tiles);  // every row leaves
@@ -1093,7 +1345,7 @@ void WindowFnOp::emit(int64_t w, BatchesPriv* out) {
     g.keep = rank ? keep_.as<unsigned int>() : nullptr;
     g.off = rank ? off2_.as<unsigned long long>() : nullptr;
     g.fn = fnv_.as<unsigned long long>();
-    g.at = agg ? at_.as<unsigned int>() : nullptr;
+    g.at = agg && !frame ? at_.as<unsigned int>() : nullptr;
     g.fn_out = out_fn_.as<unsigned long long>();
     if (null_rows()) {
       reserve(out_valid_, m);
@@ -1202,6 +1454,116 @@ void WindowFnOp::values(const WRank& r, uint64_t n_tiles) {
   wf_value_apply_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(p);
   AB_CUDA(cudaGetLastError());
   st_.kernel_launches += 4;  // with wf_rank_flags and the rank tiles' carry
+}
+
+// An aggregate or value function over the explicit frame (after wf_rank_flags and the rank tiles' carry): fnv_ gets
+// each row's value and, unless the function is COUNT, valid_ its validity.  at_ holds each peer group's last row,
+// seg_last_ each segment's, at their first rows.  The key buffers are free after the sort: key_[0] holds the RANGE
+// key, key_[1] the split values of SUM / AVG or the sorted values of MIN / MAX.
+void WindowFnOp::framed(const WRank& r, uint64_t n_tiles) {
+  const uint64_t n = (uint64_t)r.n;
+  reserve(at_, n * 4);
+  reserve(seg_last_, n * 4);
+  WFrame p{};
+  WValue& b = p.b;
+  b.arg = arg_col_ >= 0 ? cur_.col[arg_col_].as<unsigned long long>() : nullptr;
+  b.idx = r.idx;
+  b.bits = r.bits;
+  b.n = r.n;
+  b.rank_tiles = r.tiles;
+  b.peer_last = at_.as<unsigned int>();
+  b.seg_last = seg_last_.as<unsigned int>();
+  b.fn = fn_;
+  b.offset = offset_;
+  b.fv = fnv_.as<unsigned long long>();
+  if (null_rows()) {
+    reserve(valid_, n);
+    b.valid = valid_.as<unsigned char>();
+  }
+  p.units = frame_.units;
+  p.start_kind = frame_.start_kind;
+  p.end_kind = frame_.end_kind;
+  p.start_off = (unsigned long long)frame_.start_offset;
+  p.end_off = (unsigned long long)frame_.end_offset;
+  wf_bounds_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(b);
+  AB_CUDA(cudaGetLastError());
+  st_.kernel_launches += 4;  // with wf_rank_flags, the rank tiles' carry and the apply pass
+  if (frame_.units == ARROYO_B200_FRAME_GROUPS) {
+    reserve(gfirst_, n * 4);
+    reserve(gcount_, n * 4);
+    p.gfirst = gfirst_.as<unsigned int>();
+    p.gcount = gcount_.as<unsigned int>();
+    wf_groups_kernel<<<(unsigned)n_tiles, WF_TILE, 0, stream_>>>(p);
+    AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
+  }
+  auto offset = [](int k) { return k == ARROYO_B200_BOUND_PRECEDING || k == ARROYO_B200_BOUND_FOLLOWING; };
+  if (frame_.units == ARROYO_B200_FRAME_RANGE && (offset(frame_.start_kind) || offset(frame_.end_kind))) {
+    wf_key_kernel<<<grid_for(n), WF_THREADS, 0, stream_>>>(cur_.col[order_col_[0]].as<unsigned long long>(), r.idx,
+                                                           r.n, flip_of(order_col_[0], order_desc_[0]),
+                                                           key_[0].as<unsigned long long>());
+    AB_CUDA(cudaGetLastError());
+    ++st_.kernel_launches;
+    p.ukey = key_[0].as<unsigned long long>();
+  }
+  const int kind = fn_ == ARROYO_B200_FN_AGGREGATE ? agg_kind_ : 0;
+  if (kind == ARROYO_B200_AGG_SUM_I64 || kind == ARROYO_B200_AGG_AVG_I64) {
+    // two exact prefix sums of 32-bit parts, each below 2^63 over 2^31 rows
+    reserve(pre_, (n + 1) * 16);
+    unsigned long long* lo = pre_.as<unsigned long long>();
+    unsigned long long* hi = lo + n + 1;
+    unsigned int* parts = key_[1].as<unsigned int>();
+    wf_split_kernel<<<grid_for(n), WF_THREADS, 0, stream_>>>(b.arg, r.idx, r.n, parts, parts + n);
+    AB_CUDA(cudaGetLastError());
+    device_exclusive_scan(parts, (int64_t)n, lo, lo + n, sums_, stream_);
+    device_exclusive_scan(parts + n, (int64_t)n, hi, hi + n, sums_, stream_);
+    st_.kernel_launches += 7;
+    p.pre_lo = lo;
+    p.pre_hi = hi;
+  } else if (kind == ARROYO_B200_AGG_MIN_I64 || kind == ARROYO_B200_AGG_MAX_I64) {
+    WRmq q{};
+    q.arg = b.arg;
+    q.idx = r.idx;
+    q.n = r.n;
+    q.n_blocks = (long long)((n + 31) / 32);
+    int levels = 1;
+    while ((1ll << levels) <= q.n_blocks) ++levels;
+    reserve(rmq_, n * 16);
+    reserve(table_, (size_t)q.n_blocks * levels * 8);
+    q.v = key_[1].as<long long>();
+    q.in_pre = rmq_.as<long long>();
+    q.in_suf = q.in_pre + n;
+    q.table = table_.as<long long>();
+    const bool mn = kind == ARROYO_B200_AGG_MIN_I64;
+    const unsigned grid = (unsigned)((n + WF_THREADS - 1) / WF_THREADS);
+    if (mn) wf_rmq_blocks_kernel<ARROYO_B200_AGG_MIN_I64><<<grid, WF_THREADS, 0, stream_>>>(q);
+    else wf_rmq_blocks_kernel<ARROYO_B200_AGG_MAX_I64><<<grid, WF_THREADS, 0, stream_>>>(q);
+    AB_CUDA(cudaGetLastError());
+    for (int k = 1; k < levels; ++k) {
+      const int lg = grid_for((uint64_t)q.n_blocks);
+      if (mn) wf_rmq_level_kernel<ARROYO_B200_AGG_MIN_I64><<<lg, WF_THREADS, 0, stream_>>>(q.table, q.n_blocks, k);
+      else wf_rmq_level_kernel<ARROYO_B200_AGG_MAX_I64><<<lg, WF_THREADS, 0, stream_>>>(q.table, q.n_blocks, k);
+      AB_CUDA(cudaGetLastError());
+    }
+    st_.kernel_launches += (uint64_t)levels;
+    p.v = q.v;
+    p.in_pre = q.in_pre;
+    p.in_suf = q.in_suf;
+    p.table = q.table;
+    p.n_blocks = q.n_blocks;
+  }
+  const unsigned grid = (unsigned)n_tiles;
+  switch (fn_ == ARROYO_B200_FN_AGGREGATE ? agg_kind_ : fn_) {
+    case ARROYO_B200_AGG_COUNT_STAR: wf_frame_apply_kernel<ARROYO_B200_AGG_COUNT_STAR><<<grid, WF_TILE, 0, stream_>>>(p); break;
+    case ARROYO_B200_AGG_SUM_I64: wf_frame_apply_kernel<ARROYO_B200_AGG_SUM_I64><<<grid, WF_TILE, 0, stream_>>>(p); break;
+    case ARROYO_B200_AGG_AVG_I64: wf_frame_apply_kernel<ARROYO_B200_AGG_AVG_I64><<<grid, WF_TILE, 0, stream_>>>(p); break;
+    case ARROYO_B200_AGG_MIN_I64: wf_frame_apply_kernel<ARROYO_B200_AGG_MIN_I64><<<grid, WF_TILE, 0, stream_>>>(p); break;
+    case ARROYO_B200_AGG_MAX_I64: wf_frame_apply_kernel<ARROYO_B200_AGG_MAX_I64><<<grid, WF_TILE, 0, stream_>>>(p); break;
+    case ARROYO_B200_FN_FIRST_VALUE: wf_frame_apply_kernel<ARROYO_B200_FN_FIRST_VALUE><<<grid, WF_TILE, 0, stream_>>>(p); break;
+    case ARROYO_B200_FN_LAST_VALUE: wf_frame_apply_kernel<ARROYO_B200_FN_LAST_VALUE><<<grid, WF_TILE, 0, stream_>>>(p); break;
+    default: wf_frame_apply_kernel<ARROYO_B200_FN_NTH_VALUE><<<grid, WF_TILE, 0, stream_>>>(p); break;
+  }
+  AB_CUDA(cudaGetLastError());
 }
 
 // handle_checkpoint: table "input" gets the rows accepted since the previous checkpoint, one batch per instant in

@@ -7,7 +7,7 @@ import os
 
 from . import build as _build
 
-ABI_VERSION = 1
+ABI_VERSION = 2  # 2: OpConfig gained `frame` at its end
 MAX_AGGS = 8
 MAX_COLS = 16
 
@@ -19,6 +19,8 @@ FN_ROW_NUMBER, FN_RANK, FN_DENSE_RANK, FN_AGGREGATE = 1, 2, 3, 4
 FN_LAG, FN_LEAD, FN_FIRST_VALUE, FN_LAST_VALUE, FN_NTH_VALUE, FN_PERCENT_RANK, FN_CUME_DIST = 5, 6, 7, 8, 9, 10, 11
 ORDER_ASC, ORDER_DESC = 16, 17
 FN_ARGUMENT = 18
+FRAME_DEFAULT, FRAME_ROWS, FRAME_RANGE, FRAME_GROUPS = 0, 1, 2, 3
+BOUND_UNBOUNDED_PRECEDING, BOUND_PRECEDING, BOUND_CURRENT_ROW, BOUND_FOLLOWING, BOUND_UNBOUNDED_FOLLOWING = 1, 2, 3, 4, 5
 MAX_ORDER_KEYS = 4
 AGG_COUNT_STAR, AGG_SUM_I64, AGG_AVG_I64, AGG_MIN_I64, AGG_MAX_I64 = 1, 2, 3, 4, 5
 JOIN_INNER, JOIN_LEFT, JOIN_RIGHT, JOIN_FULL = 0, 1, 2, 3
@@ -58,6 +60,11 @@ class Agg(C.Structure):
     _fields_ = [("kind", C.c_int32), ("input_col", C.c_int32)]
 
 
+class WindowFrame(C.Structure):
+    _fields_ = [("units", C.c_int32), ("start_kind", C.c_int32), ("end_kind", C.c_int32), ("pad", C.c_int32),
+                ("start_offset", C.c_int64), ("end_offset", C.c_int64)]
+
+
 class OpConfig(C.Structure):
     _fields_ = [
         ("kind", C.c_int32), ("device", C.c_int32), ("stream", C.c_uint64),
@@ -71,6 +78,7 @@ class OpConfig(C.Structure):
         ("left_n_routing", C.c_int32), ("right_n_routing", C.c_int32),
         ("partial_count_col_plus1", C.c_int32), ("window_fn", C.c_int32),
         ("expected_keys", C.c_uint64), ("flags", C.c_uint32), ("reserved", C.c_uint32),
+        ("frame", WindowFrame),
     ]
 
 

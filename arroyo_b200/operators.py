@@ -437,6 +437,23 @@ def _flat_fields(schema: pa.Schema):
     return fields
 
 
+_FRAME_UNITS = {"rows": ffi.FRAME_ROWS, "range": ffi.FRAME_RANGE, "groups": ffi.FRAME_GROUPS}
+_FRAME_BOUNDS = {"unbounded_preceding": ffi.BOUND_UNBOUNDED_PRECEDING, "preceding": ffi.BOUND_PRECEDING,
+                 "current_row": ffi.BOUND_CURRENT_ROW, "following": ffi.BOUND_FOLLOWING,
+                 "unbounded_following": ffi.BOUND_UNBOUNDED_FOLLOWING}
+
+
+def _frame_bound(bound):
+    """A WindowFrame bound as (ArroyoB200FrameBound code, offset): a bare kind, or ("preceding" | "following", n).
+    The library checks the offset's sign; one outside Int64 is refused here, before ctypes would wrap it."""
+    kind, n = (bound, 0) if isinstance(bound, str) else bound
+    if kind not in _FRAME_BOUNDS or (kind in ("preceding", "following")) != (not isinstance(bound, str)):
+        raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, f"frame bound {bound!r}")
+    if not ffi.INT64_MIN <= int(n) <= ffi.INT64_MAX:
+        raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, f"frame offset {n} outside Int64")
+    return _FRAME_BOUNDS[kind], int(n)
+
+
 def _default_bits(value, arrow_type) -> int:
     """LAG / LEAD's default as the signed 64 bits of the argument's type: a Float64's IEEE bits, else the integer
     modulo 2^64."""
@@ -449,9 +466,11 @@ class WindowFunction(_WindowAggregate):
     """window_fn.rs: ROW_NUMBER / RANK / DENSE_RANK per instant (each upstream window stamps its rows with one
     `_timestamp`) and partition key, with the fused `WHERE fn <= top_n`, COUNT / SUM / AVG / MIN / MAX of
     `config.argument` over the default frame, LAG / LEAD / FIRST_VALUE / LAST_VALUE / NTH_VALUE of `config.argument`,
-    or PERCENT_RANK / CUME_DIST.  At watermark w every instant < w leaves in one batch: the input columns, struct
-    columns included, then the function column `config.name` (UInt64 for a rank, Float64 for avg, percent_rank and
-    cume_dist, the argument's type for a value function, else Int64; lag / lead / nth_value are nullable).  Columns
+    or PERCENT_RANK / CUME_DIST; the aggregates and FIRST_VALUE / LAST_VALUE / NTH_VALUE over `config.frame` when one is
+    given.  At watermark w every instant < w leaves in one batch: the input columns, struct columns included, then the
+    function column `config.name` (UInt64 for a rank, Float64 for avg, percent_rank and cume_dist, the argument's type
+    for a value function, else Int64; lag / lead / nth_value, and under an explicit frame every function but count,
+    are nullable).  Columns
     are named in the config by their flat names (`flat_names`).  Table "input" (retention 0) holds per instant the input
     rows since the previous checkpoint.  Device-resident input is flat; a schema given at construction declares the
     column types to the library, which device batches do not carry."""
@@ -507,6 +526,12 @@ class WindowFunction(_WindowAggregate):
             cfg.aggs[first + i].kind = ffi.ORDER_DESC if desc else ffi.ORDER_ASC
             cfg.aggs[first + i].input_col = flat.index(col)
         cfg.slide_ns = int(c.top_n)
+        if c.frame is not None:
+            if c.frame.units not in _FRAME_UNITS:
+                raise ffi.ArroyoB200Error(ffi.INVALID_ARGUMENT, f"frame units {c.frame.units!r}")
+            cfg.frame.units = _FRAME_UNITS[c.frame.units]
+            cfg.frame.start_kind, cfg.frame.start_offset = _frame_bound(c.frame.start)
+            cfg.frame.end_kind, cfg.frame.end_offset = _frame_bound(c.frame.end)
         self._create(cfg)
         self._names = list(names)
         if schema is not None:

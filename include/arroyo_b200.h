@@ -158,6 +158,39 @@ typedef enum ArroyoB200OpKind {
                                        *    flag on FN_FIRST_VALUE .. FN_CUME_DIST => INVALID_ARGUMENT (the ranking
                                        *    functions and the aggregates ignore flags, as before).  A nullable column
                                        *    carries an Arrow validity bitmap only when one of its rows is NULL;
+                                       *  - frame (ArroyoB200WindowFrame): units 0 (a zeroed struct) is the default frame
+                                       *    above.  ROWS / RANGE / GROUPS run the aggregates and FIRST_VALUE /
+                                       *    LAST_VALUE / NTH_VALUE over [lo, hi), sorted rows clipped to [s, e + 1)
+                                       *    (lo >= hi: an empty frame).  A start gives lo, an end hi:
+                                       *      ROWS    n PRECEDING j - n, CURRENT ROW j, n FOLLOWING j + n; an end one
+                                       *              past the row it names;
+                                       *      RANGE   CURRENT ROW: the row's first peer / one past its last peer; n
+                                       *              PRECEDING / FOLLOWING (exactly one ORDER BY key): the first row
+                                       *              whose key is within n before / after the row's, or one past the
+                                       *              last such row for an end.  "Before" is in sort order: under DESC
+                                       *              "n PRECEDING" reaches keys up to x + n.  Computed on the sort's
+                                       *              unsigned form of the key: a limit past the key type's range lies
+                                       *              past every row, so the frame runs to the segment's edge or is
+                                       *              empty (whether DataFusion errors on that overflow instead is not
+                                       *              pinned here);
+                                       *      GROUPS  the first row of the peer group n before / after the row's (an
+                                       *              end: one past that group's last row);
+                                       *      UNBOUNDED PRECEDING s, UNBOUNDED FOLLOWING e + 1.
+                                       *    ROWS and GROUPS offsets may be anything up to INT64_MAX.  COUNT gives
+                                       *    hi - lo; SUM the wrapping sum; AVG the exact sum converted to f64 once,
+                                       *    over hi - lo; MIN / MAX the extremes; FIRST_VALUE / LAST_VALUE /
+                                       *    NTH_VALUE x at lo / hi - 1 / lo + n - 1 (NULL unless < hi).  Every
+                                       *    function but COUNT is NULL on an empty frame, and its column is nullable.
+                                       *    A frame equal to the default (RANGE UNBOUNDED PRECEDING AND CURRENT ROW with
+                                       *    ORDER BY; UNBOUNDED PRECEDING AND UNBOUNDED FOLLOWING in any unit without
+                                       *    it) runs as units 0 and gives its bits.  INVALID_ARGUMENT: units outside 0
+                                       *    to 3, a frame on any other function, a bound code outside 1 to 5, a start at
+                                       *    UNBOUNDED FOLLOWING or an end at UNBOUNDED PRECEDING, a negative offset of
+                                       *    n PRECEDING / FOLLOWING, RANGE with an offset and not exactly one ORDER BY
+                                       *    key, GROUPS without ORDER BY.  UNSUPPORTED: a start after the end (n
+                                       *    FOLLOWING AND CURRENT ROW | m PRECEDING, CURRENT ROW AND m PRECEDING),
+                                       *    which SQLite refuses and nothing here pins.  Frames that are empty for
+                                       *    every row (2 FOLLOWING AND 1 FOLLOWING) are accepted;
                                        *  - slide_ns: N of a fused `WHERE fn <= N` (`fn = 1` is the same as `<= 1` for all
                                        *    three ranking functions); 0 = every row leaves; < 0, or not 0 for any other
                                        *    function => INVALID_ARGUMENT;
@@ -229,6 +262,33 @@ typedef struct ArroyoB200Agg {
   int32_t input_col; /* index into the input batch; ignored for COUNT  */
 } ArroyoB200Agg;
 
+/* WINDOW_FUNCTION: an explicit frame clause, `{ROWS | RANGE | GROUPS} BETWEEN start AND end` (DataFusion's
+ * WindowFrame).  units = ARROYO_B200_FRAME_DEFAULT (0, a zeroed struct) is DataFusion's default frame and the other
+ * fields are ignored.  Otherwise start_kind / end_kind are ArroyoB200FrameBound codes and start_offset / end_offset
+ * the n of `n PRECEDING` / `n FOLLOWING` (>= 0; ignored for the other bounds).  For RANGE over a Timestamp(ns) key
+ * the offsets are nanoseconds.  The kind-8 contract above says which frames run and which are refused. */
+typedef enum ArroyoB200FrameUnits {
+  ARROYO_B200_FRAME_DEFAULT = 0,
+  ARROYO_B200_FRAME_ROWS = 1,
+  ARROYO_B200_FRAME_RANGE = 2,
+  ARROYO_B200_FRAME_GROUPS = 3
+} ArroyoB200FrameUnits;
+typedef enum ArroyoB200FrameBound {
+  ARROYO_B200_BOUND_UNBOUNDED_PRECEDING = 1,
+  ARROYO_B200_BOUND_PRECEDING = 2,
+  ARROYO_B200_BOUND_CURRENT_ROW = 3,
+  ARROYO_B200_BOUND_FOLLOWING = 4,
+  ARROYO_B200_BOUND_UNBOUNDED_FOLLOWING = 5
+} ArroyoB200FrameBound;
+typedef struct ArroyoB200WindowFrame {
+  int32_t units;        /* ArroyoB200FrameUnits */
+  int32_t start_kind;   /* ArroyoB200FrameBound */
+  int32_t end_kind;     /* ArroyoB200FrameBound */
+  int32_t pad;          /* 0 */
+  int64_t start_offset;
+  int64_t end_offset;
+} ArroyoB200WindowFrame;
+
 /* Input batches are the operator's `in_schemas[i]` (ArroyoSchema, arroyo-rpc/src/df.rs):
  * [key cols (routing copies)..., payload cols..., _timestamp]; all supported columns are
  * 64-bit fixed width (int64 "l", uint64 "L", timestamp[ns] "tsn:", float64 "g" for payload). */
@@ -290,6 +350,12 @@ typedef struct ArroyoB200OpConfig {
   uint64_t expected_keys;   /* capacity hint for the key dictionary (0 = default)         */
   uint32_t flags;           /* ARROYO_B200_FLAG_*                                         */
   uint32_t reserved;        /* 0, or log2(rows per ingest launch) in [16, 26] (default 24)     */
+
+  /* ABI version 2 appended this field: the struct grew from 192 to 224 bytes, every earlier field keeping its
+   * offset.  op_create reads the whole struct, so a caller built against version 1's declaration must be rebuilt
+   * (arroyo_b200_abi_version tells the two apart); zero the field for today's behaviour. */
+  ArroyoB200WindowFrame frame; /* WINDOW_FUNCTION: the frame clause (zeroed: the default frame); every other kind
+                                * ignores it */
 } ArroyoB200OpConfig;
 
 #define ARROYO_B200_FLAG_PROFILE 1u       /* time kernels with CUDA events (op_stats)      */
@@ -358,7 +424,7 @@ typedef struct ArroyoB200Stats {
 } ArroyoB200Stats;
 
 /* ---- library ---- */
-/* ABI version of this header (checked by the bindings). */
+/* ABI version of this header (checked by the bindings): 2 since ArroyoB200OpConfig gained `frame`. */
 int32_t arroyo_b200_abi_version(void);
 /* Number of usable CUDA devices (0 on a box without a GPU). */
 int32_t arroyo_b200_device_count(void);

@@ -21,11 +21,24 @@ DESC, key DESC), with lag / lead's offset 1 and nth_value's n 2, and percent_ran
 
   wf_F_ms           F over the ordered window
 
+With --frame the same slides also take explicit frames, beside the default-frame SUM and MIN above (added when not
+asked for):
+
+  wf_sum_rows_ms    SUM(s) OVER (PARTITION BY window ORDER BY s DESC ROWS BETWEEN 100 PRECEDING AND 100 FOLLOWING)
+  wf_min_rows_ms    MIN(s) over the same frame
+  wf_sum_range_ms   SUM(s) OVER (... ORDER BY s DESC RANGE BETWEEN 1000 PRECEDING AND 1000 FOLLOWING)
+  wf_sum_range_ts_ms  SUM(s) OVER (... ORDER BY _timestamp RANGE BETWEEN 1 s PRECEDING AND CURRENT ROW), which
+                    holds the whole window, as every row of a window carries its one _timestamp
+  wf_sum_groups_ms  SUM(s) OVER (... ORDER BY s DESC GROUPS BETWEEN 5 PRECEDING AND 5 FOLLOWING)
+
+and --instant-rows N times every window function once more on one instant of N rows (s uniform in [-2^20, 2^20),
+one device batch, then the watermark past it): instant_W_ms.
+
 Each is timed with CUDA events on the operators' stream around the calls (every handle_watermark ends in a stream
 synchronise); the medians are reported, with the sorted rows per second of each window function.  Prints one JSON
 line with the card's name and power limit.
 
-    python tools/window_fn_rates.py [--scale S] [--slides K] [--function F [G ...]]
+    python tools/window_fn_rates.py [--scale S] [--slides K] [--function F [G ...]] [--frame] [--instant-rows N]
 
 --scale S divides the key count by 2^S (a quick rehearsal of the script)."""
 import argparse
@@ -64,6 +77,8 @@ def main():
     ap.add_argument("--function", nargs="+", default=["row_number"], choices=["row_number", *AGGREGATES, *ORDERED],
                     help="also time F(s) OVER (PARTITION BY window [ORDER BY s DESC]) for an aggregate, or F over "
                          "(PARTITION BY window ORDER BY s DESC, key DESC) for the other functions")
+    ap.add_argument("--frame", action="store_true", help="also time ROWS / RANGE / GROUPS frames")
+    ap.add_argument("--instant-rows", type=int, default=0, help="also time one instant of N rows")
     a = ap.parse_args()
     if not 0 <= a.scale <= 16 or a.slides < 1:
         ap.error("--scale must be in [0, 16] and --slides >= 1")
@@ -86,6 +101,8 @@ def main():
                           ("av", pa.float64()), (TS, ts_t)])
     cfgs = {what: config.WindowFunctionConfig("row_number", None, [("s", True), ("key", True)], "rn", top_n)
             for what, top_n in (("top1", 1), ("all", 0))}
+    if a.frame:
+        a.function += [f for f in ("sum", "min") if f not in a.function]
     for f in a.function:
         if f in AGGREGATES:
             for what, order_by in (("window", []), ("running", [("s", True)])):
@@ -94,6 +111,16 @@ def main():
             cfgs[f] = config.WindowFunctionConfig(f, None, [("s", True), ("key", True)], "f",
                                                   argument=None if f in ("percent_rank", "cume_dist") else "s",
                                                   offset=2 if f == "nth_value" else 1)
+    if a.frame:
+        s_desc = [("s", True)]
+        for what, f, order_by, frame in (
+                ("sum_rows", "sum", s_desc, ("rows", ("preceding", 100), ("following", 100))),
+                ("min_rows", "min", s_desc, ("rows", ("preceding", 100), ("following", 100))),
+                ("sum_range", "sum", s_desc, ("range", ("preceding", 1000), ("following", 1000))),
+                ("sum_range_ts", "sum", [(TS, False)], ("range", ("preceding", SEC), "current_row")),
+                ("sum_groups", "sum", s_desc, ("groups", ("preceding", 5), ("following", 5)))):
+            cfgs[what] = config.WindowFunctionConfig(f, None, order_by, "f", argument="s",
+                                                     frame=config.WindowFrame(*frame))
     fns = {what: native.WindowFunction(c, input_schema=w_schema, stream=stream.cuda_stream) for what, c in cfgs.items()}
     ctxs = {w: ab.OperatorContext(1) for w in fns}
     rng = np.random.default_rng(7)
@@ -135,9 +162,31 @@ def main():
             if step >= warm:
                 times["sliding_emit_ms"].append(t_s)
                 window_rows.append(n_rows)
+    if a.instant_rows:
+        n = a.instant_rows
+        cols = [torch.arange(n, dtype=torch.int64, device="cuda"), torch.zeros(n, dtype=torch.int64, device="cuda"),
+                torch.zeros(n, dtype=torch.int64, device="cuda"),
+                torch.from_numpy(rng.integers(-(1 << 20), 1 << 20, n).astype(np.int64)).cuda(),
+                torch.zeros(n, dtype=torch.int64, device="cuda"), torch.zeros(n, dtype=torch.int64, device="cuda")]
+        with torch.cuda.stream(stream):
+            for what, op in fns.items():
+                for rep in range(6):
+                    wm = T0 + (warm + a.slides + rep) * SEC
+                    cols[5].fill_(wm - 1)
+                    stream.synchronize()
+
+                    def call():
+                        op.process_device_batch([c.data_ptr() for c in cols], n)
+                        col = ab.Collector()
+                        ctxs[what].watermarks.set(0, wm)
+                        op.handle_watermark(wm, ctxs[what], col)
+                        return sum(b.num_rows for b in col.batches)
+                    _, t = timed(call)
+                    if rep >= 2:
+                        times.setdefault(f"instant_{what}_ms", []).append(t)
     med = {k: float(np.median(v)) for k, v in times.items()}
     rows = float(np.median(window_rows))
-    res = {**card(), "keys": keys, "slides": a.slides, "window_rows": int(rows),
+    res = {**card(), "keys": keys, "slides": a.slides, "window_rows": int(rows), "instant_rows": a.instant_rows,
            **{k: round(v, 3) for k, v in med.items()},
            **{f"wf_{w}_sorted_rows_per_s": round(rows / (med[f"wf_{w}_ms"] / 1e3)) for w in fns},
            **{f"rows_out_{w}": rows_out[w] for w in fns}}
