@@ -5,6 +5,7 @@
 #pragma once
 
 #include <algorithm>
+#include <deque>
 #include <string>
 #include <vector>
 
@@ -335,47 +336,77 @@ inline void batches_release(ArroyoB200Batches* b) {
 }
 
 // Host input batches the library has taken and holds until the stream has passed the copies that read them.  The
-// owner drains its stream before this is destroyed, which releases whatever is still held.
+// owner drains its streams before this is destroyed, which releases whatever is still held.
 class HeldInputs {
  public:
   HeldInputs() = default;
   HeldInputs(const HeldInputs&) = delete;
   HeldInputs& operator=(const HeldInputs&) = delete;
   ~HeldInputs() {
-    for (auto& h : held_) {
-      if (h.second.release) h.second.release(&h.second);
-      cudaEventDestroy(h.first);
+    for (auto& a : taken_)
+      if (a.release) a.release(&a);
+    for (auto& g : sealed_) {
+      for (auto& a : g.batches)
+        if (a.release) a.release(&a);
+      cudaEventDestroy(g.ev);
     }
+    for (cudaEvent_t e : pool_) cudaEventDestroy(e);
   }
 
-  // Takes `batch` (its `release` is set to NULL) until `s` has passed the work enqueued on it so far.
-  void hold(ArrowArray* batch, cudaStream_t s) {
-    cudaEvent_t ev;
-    AB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    AB_CUDA(cudaEventRecord(ev, s));
-    held_.emplace_back(ev, *batch);
+  // Takes `batch` (its `release` is set to NULL).  It is held from the next seal() on.
+  void take(ArrowArray* batch) {
+    taken_.push_back(*batch);
     batch->release = nullptr;
   }
+  size_t n_unsealed() const { return taken_.size(); }
 
-  // Releases, in the order they were taken, the batches whose copies have completed; with `wait`, all of them.
+  // Holds every batch taken since the last seal until `s` has passed the work enqueued on it so far: one event for
+  // all of them, taken from a pool.
+  void seal(cudaStream_t s) {
+    if (taken_.empty()) return;
+    if (pool_.empty()) {
+      cudaEvent_t e;
+      AB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+      pool_.push_back(e);
+    }
+    AB_CUDA(cudaEventRecord(pool_.back(), s));
+    sealed_.push_back({pool_.back(), std::move(taken_)});
+    pool_.pop_back();
+    taken_.clear();
+  }
+
+  // Takes `batch` until `s` has passed the work enqueued on it so far.
+  void hold(ArrowArray* batch, cudaStream_t s) {
+    take(batch);
+    seal(s);
+  }
+
+  // Releases, in the order they were sealed, the batches whose copies have completed; with `wait`, every sealed one.
   void release(bool wait) {
-    while (!held_.empty()) {
-      auto& h = held_.front();
+    while (!sealed_.empty()) {
+      Sealed& g = sealed_.front();
       if (wait) {
-        AB_CUDA(cudaEventSynchronize(h.first));
+        AB_CUDA(cudaEventSynchronize(g.ev));
       } else {
-        const cudaError_t e = cudaEventQuery(h.first);
+        const cudaError_t e = cudaEventQuery(g.ev);
         if (e == cudaErrorNotReady) break;
         AB_CUDA(e);
       }
-      if (h.second.release) h.second.release(&h.second);
-      cudaEventDestroy(h.first);
-      held_.erase(held_.begin());
+      for (auto& a : g.batches)
+        if (a.release) a.release(&a);
+      pool_.push_back(g.ev);
+      sealed_.pop_front();
     }
   }
 
  private:
-  std::vector<std::pair<cudaEvent_t, ArrowArray>> held_;
+  struct Sealed {
+    cudaEvent_t ev;
+    std::vector<ArrowArray> batches;
+  };
+  std::vector<ArrowArray> taken_;  // taken since the last seal
+  std::deque<Sealed> sealed_;
+  std::vector<cudaEvent_t> pool_;  // recorded events whose batches have been released
 };
 
 }  // namespace ab

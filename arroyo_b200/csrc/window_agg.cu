@@ -694,12 +694,6 @@ struct LaunchRec {
   int chunk = -1;  // staging chunk read by this launch (-1: none)
 };
 
-constexpr size_t RELEASE_GROUP = 16;
-struct PendingRelease {
-  cudaEvent_t ev;
-  std::vector<ArrowArray> arrs;  // moved-in copies; released when ev completes
-};
-
 class WindowAggOp final : public OpBase {
  public:
   explicit WindowAggOp(const ArroyoB200OpConfig& c);
@@ -757,6 +751,9 @@ class WindowAggOp final : public OpBase {
   int part_flip_ = 0;
   bool two_pass_attr_set_ = false;
   bool two_pass_enabled_ = true;
+  // smaller launches take the one-pass kernel (the per-bucket set-up does not pay for them) unless
+  // ARROYO_B200_FLAG_TWO_PASS_ALWAYS
+  static constexpr uint64_t TWO_PASS_MIN_ROWS = 1ull << 19;
   uint64_t part_overflow_seen_ = 0;
   mutable int two_pass_pause_ = 0;  // launches left on the one-pass kernel after a skewed launch
   bool two_pass_eligible(uint64_t rows) const;
@@ -773,9 +770,10 @@ class WindowAggOp final : public OpBase {
   bool batch_copy_ok_ = true;
   void queue_copy(void* dst, const void* src, size_t bytes);
   void flush_copies();
-  std::vector<ArrowArray> open_release_;  // staged inputs whose copies have no release event yet
-  std::vector<cudaEvent_t> ev_pool_;
-  void seal_release();
+  // host batches whose copies to the chunks may still run, sealed behind the copies on copy_stream_ every
+  // RELEASE_GROUP batches and at every launch: one event per group instead of one per batch
+  static constexpr size_t RELEASE_GROUP = 16;
+  HeldInputs inputs_;
 
   // ring
   uint32_t ring_ = 16;
@@ -823,8 +821,6 @@ class WindowAggOp final : public OpBase {
   PinnedBuf h_book_[NLAUNCH];
   int next_launch_ = 0;
   std::deque<int> in_flight_;
-  std::deque<PendingRelease> releases_;
-  std::vector<ArrowArray> zero_copy_inputs_;  // pinned input batches read in place by the next launch
 
   // deferred rows (two sets: one being filled, one being re-ingested)
   uint64_t defer_cap_ = 0;
@@ -883,7 +879,6 @@ class WindowAggOp final : public OpBase {
   void absorb(int li);
   void sync_all();
   void drain_deferred();
-  void poll_releases(bool wait);
   void rotate_chunk();
   void touch(int64_t bin);
   OutSet* out_set(size_t i, uint64_t cap);
@@ -958,10 +953,7 @@ WindowAggOp::WindowAggOp(const ArroyoB200OpConfig& c) {
   dict_.init(stream_, num_sms_, plan_.keyed, (unsigned int*)((char*)book_.p + offsetof(Counters, n_keys)),
              &st_.kernel_launches);
   dict_.alloc(plan_.keyed ? bd_buckets_for(want) : 1);
-  {
-    const char* e = getenv("ARROYO_B200_NO_TWO_PASS");
-    two_pass_enabled_ = !(e && atoi(e) != 0) && !(c.flags & ARROYO_B200_FLAG_NO_TWO_PASS);
-  }
+  two_pass_enabled_ = !(c.flags & ARROYO_B200_FLAG_NO_TWO_PASS);
 
   h_pane_bins_.assign(MAX_RING, FREE_BIN);
   h_pane_ptrs_.assign(MAX_RING, nullptr);
@@ -1028,20 +1020,11 @@ void WindowAggOp::preallocate() {
 WindowAggOp::~WindowAggOp() {
   cudaSetDevice(device_);
   if (counts_done_) cudaEventDestroy(counts_done_);
-  // nothing may still be reading the input batches or writing output buffers when they are handed back
+  // nothing may still be reading the input batches or writing output buffers when the members' destructors hand
+  // them back
   if (copy_stream_) cudaStreamSynchronize(copy_stream_);
   if (out_stream_) cudaStreamSynchronize(out_stream_);
   cudaStreamSynchronize(stream_);
-  for (auto& r : releases_) {
-    for (auto& a : r.arrs)
-      if (a.release) a.release(&a);
-    cudaEventDestroy(r.ev);
-  }
-  for (auto& a : zero_copy_inputs_)
-    if (a.release) a.release(&a);
-  for (auto& a : open_release_)
-    if (a.release) a.release(&a);
-  for (auto e : ev_pool_) cudaEventDestroy(e);
   for (int i = 0; i < NCHUNK; ++i)
     if (chunk_free_[i]) cudaEventDestroy(chunk_free_[i]);
   if (copy_stream_) {
@@ -1334,41 +1317,6 @@ void WindowAggOp::flush_copies() {
   copy_size_.clear();
 }
 
-// Input batches are handed back in groups: one CUDA event per RELEASE_GROUP batches (or per launch / flush)
-// instead of one per batch, and the events are recycled.
-void WindowAggOp::seal_release() {
-  flush_copies();
-  if (open_release_.empty()) return;
-  PendingRelease r;
-  if (!ev_pool_.empty()) {
-    r.ev = ev_pool_.back();
-    ev_pool_.pop_back();
-  } else {
-    AB_CUDA(cudaEventCreateWithFlags(&r.ev, cudaEventDisableTiming));
-  }
-  AB_CUDA(cudaEventRecord(r.ev, copy_stream_));
-  r.arrs.swap(open_release_);
-  releases_.push_back(std::move(r));
-}
-
-void WindowAggOp::poll_releases(bool wait) {
-  if (wait) seal_release();
-  while (!releases_.empty()) {
-    PendingRelease& r = releases_.front();
-    if (wait) {
-      AB_CUDA(cudaEventSynchronize(r.ev));
-    } else {
-      cudaError_t e = cudaEventQuery(r.ev);
-      if (e == cudaErrorNotReady) break;
-      AB_CUDA(e);
-    }
-    for (auto& a : r.arrs)
-      if (a.release) a.release(&a);
-    ev_pool_.push_back(r.ev);
-    releases_.pop_front();
-  }
-}
-
 void WindowAggOp::add_segment(const long long* key, const long long* ts, const long long* const* vals, int64_t n) {
   if (n <= 0) return;
   if (!segs_.empty()) {
@@ -1406,7 +1354,7 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
   AB_REQUIRE((int)cols.size() == cfg.n_cols, ARROYO_B200_INVALID_ARGUMENT, "batch has the wrong number of columns");
   require_aggregate_input_types(cols, plan_.keyed ? plan_.key_col : -1, plan_.val_cols, plan_.n_vals);
   if (plan_.keyed) key_format_ = cols[plan_.key_col].format;
-  poll_releases(false);
+  inputs_.release(false);
   st_.rows_in += (uint64_t)n;
   if (n > 0 && panes_.empty() && max_bin_seen_ == LLONG_MIN) {
     // residency hint only (no semantics): make the first row's pane resident so a cold start does
@@ -1416,43 +1364,6 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
       ensure_pane(b0);
       max_bin_seen_ = b0;
       lookahead();
-    }
-  }
-  // ARROYO_B200_FLAG_ZERO_COPY: pinned (page-locked, device-mapped) Arrow buffers are read in place by the
-  // ingest kernel over PCIe: no staging memory.  SM loads over PCIe move less than the copy engines do, so this
-  // is slower than DMA staging end to end, hence opt-in.
-  if (n > 0 && (cfg.flags & ARROYO_B200_FLAG_ZERO_COPY)) {
-    bool pinned = true;
-    const uint64_t* devp[ARROYO_B200_MAX_COLS] = {nullptr};
-    auto probe = [&](int c) {
-      cudaPointerAttributes at{};
-      if (cudaPointerGetAttributes(&at, cols[c].data) != cudaSuccess) {
-        cudaGetLastError();
-        pinned = false;
-        return;
-      }
-      if (at.type != cudaMemoryTypeHost || at.devicePointer == nullptr) pinned = false;
-      else devp[c] = (const uint64_t*)at.devicePointer;
-    };
-    if (plan_.keyed) probe(plan_.key_col);
-    probe(plan_.ts_col);
-    for (int v = 0; v < plan_.n_vals; ++v) probe(plan_.val_cols[v]);
-    if (pinned) {
-      int64_t done = 0;
-      while (done < n) {
-        int64_t take = std::min<int64_t>(n - done, launch_rows_ - pending_rows_);
-        const long long* vals[MAX_VALS];
-        for (int v = 0; v < plan_.n_vals; ++v) vals[v] = (const long long*)devp[plan_.val_cols[v]] + done;
-        add_segment(plan_.keyed ? (const long long*)devp[plan_.key_col] + done : nullptr, (const long long*)devp[plan_.ts_col] + done,
-                    vals, take);
-        done += take;
-        if (done < n && pending_rows_ >= launch_rows_) launch_pending();
-      }
-      st_.h2d_bytes += (uint64_t)n * 8 * (uint64_t)((plan_.keyed ? 1 : 0) + 1 + plan_.n_vals);
-      zero_copy_inputs_.push_back(*batch);
-      batch->release = nullptr;
-      if (pending_rows_ >= launch_rows_) launch_pending();
-      return;
     }
   }
   const int n_used = 2 + plan_.n_vals;
@@ -1484,9 +1395,11 @@ void WindowAggOp::process_batch(uint32_t, uint32_t, ArrowArray* batch, const Arr
     done += take;
   }
   // ownership of the input moves to the library; released once the copies have completed
-  open_release_.push_back(*batch);
-  batch->release = nullptr;
-  if (open_release_.size() >= RELEASE_GROUP) seal_release();
+  inputs_.take(batch);
+  if (inputs_.n_unsealed() >= RELEASE_GROUP) {
+    flush_copies();  // the event must follow the copies that read the batches
+    inputs_.seal(copy_stream_);
+  }
   if (cur_rows_ == chunk_rows_) {
     launch_pending();
     rotate_chunk();
@@ -1522,11 +1435,7 @@ bool WindowAggOp::two_pass_eligible(uint64_t rows) const {
     --two_pass_pause_;
     return false;
   }
-  static const uint64_t min_rows = [] {
-    const char* e = getenv("ARROYO_B200_TWO_PASS_MIN_ROWS");
-    return e ? strtoull(e, nullptr, 10) : (1ull << 19);
-  }();
-  return rows >= min_rows || (cfg.flags & ARROYO_B200_FLAG_TWO_PASS_ALWAYS);
+  return rows >= TWO_PASS_MIN_ROWS || (cfg.flags & ARROYO_B200_FLAG_TWO_PASS_ALWAYS);
 }
 
 void WindowAggOp::launch_two_pass(IngestParams& p, uint64_t rows, long long tiles) {
@@ -1721,7 +1630,8 @@ void WindowAggOp::launch_segments(const std::vector<Segment>& segs_in, int chunk
 }
 
 void WindowAggOp::launch_pending() {
-  seal_release();
+  flush_copies();
+  inputs_.seal(copy_stream_);
   if (segs_.empty()) return;
   std::vector<Segment> segs;
   segs.swap(segs_);
@@ -1734,19 +1644,6 @@ void WindowAggOp::launch_pending() {
     AB_CUDA(cudaStreamWaitEvent(stream_, copied_, 0));
   }
   launch_segments(segs, chunk);
-  if (!zero_copy_inputs_.empty()) {
-    // the pinned input batches these segments point into may be released once this kernel has run
-    PendingRelease r;
-    if (!ev_pool_.empty()) {
-      r.ev = ev_pool_.back();
-      ev_pool_.pop_back();
-    } else {
-      AB_CUDA(cudaEventCreateWithFlags(&r.ev, cudaEventDisableTiming));
-    }
-    AB_CUDA(cudaEventRecord(r.ev, stream_));
-    r.arrs.swap(zero_copy_inputs_);
-    releases_.push_back(std::move(r));
-  }
 }
 
 void WindowAggOp::touch(int64_t bin) {
@@ -1874,9 +1771,9 @@ void WindowAggOp::drain_deferred() {
 void WindowAggOp::flush() {
   set_device();
   resolve_deferred();
-  launch_pending();
+  launch_pending();  // seals every batch taken so far
   sync_all();
-  poll_releases(true);
+  inputs_.release(true);
 }
 
 void WindowAggOp::submit() {
@@ -2191,7 +2088,7 @@ void WindowAggOp::handle_watermark(int64_t wm, BatchesPriv* out_host, std::vecto
   wait_outputs();
   launch_pending();
   sync_all();
-  poll_releases(false);
+  inputs_.release(false);
   std::vector<PlanStep> steps;
   if (sliding_) sliding_planner_->watermark(wm, steps);
   else tumbling_->watermark(wm, steps);

@@ -365,8 +365,9 @@ typedef struct ArroyoB200OpConfig {
 #define ARROYO_B200_FLAG_AVG_F64 8u       /* AVG(Int64) with its own f64 accumulator from the start  */
                                           /* (default: exact integer sum, promoted on demand)        */
 #define ARROYO_B200_FLAG_COMBINE 4u       /* (default behaviour; kept for ABI stability)   */
-#define ARROYO_B200_FLAG_ZERO_COPY 32u    /* read pinned host batches in place over PCIe  */
-                                          /* instead of staging them with the copy engine */
+#define ARROYO_B200_FLAG_ZERO_COPY 32u    /* accepted and ignored (pinned host batches were read in   */
+                                          /* place over PCIe, which was slower than staging them      */
+                                          /* with the copy engine; every host batch is staged now)    */
 #define ARROYO_B200_FLAG_NO_COMBINE 16u   /* do not warp-combine equal keys before the     */
                                           /* atomics (measurement knob)                    */
 #define ARROYO_B200_FLAG_NO_DIRECT 64u    /* accepted and ignored (round 1 mapped dense key ranges    */

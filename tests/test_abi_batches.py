@@ -161,6 +161,30 @@ def test_a_refused_on_start_leaves_the_state_batches_to_the_caller(kind, how):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("flags", [0, ffi.FLAG_ZERO_COPY], ids=["staged", "zero_copy_flag"])
+def test_window_aggregate_releases_every_host_batch_by_flush(flags):
+    """The tumbling / sliding aggregate holds the host batches it takes until their copies have run, in groups of 16,
+    and flush hands every one of them back: the Arrow pool's bytes return to their baseline.  40 batches leave two
+    sealed groups and 8 batches that only flush seals.  FLAG_ZERO_COPY is accepted and changes nothing."""
+    rng = np.random.default_rng(6)
+    op = native.SlidingAggregatingWindowFunc(
+        O.WindowAggConfig(width=4 * S, slide=S, key_names=["key"], aggs=AGGS, window_index=1),
+        input_schema=SCHEMA, flags=flags)
+    ctx, out = ab.OperatorContext(1), ab.Collector()
+    base = pa.total_allocated_bytes()
+    for i in range(40):
+        b = _batch(rng, i * S // 8)
+        b = b.take(pa.array(np.arange(b.num_rows)))  # buffers from the Arrow pool, not wrapped numpy memory
+        op.process_batch(b, ctx, out)
+    del b
+    assert pa.total_allocated_bytes() > base  # the batches taken since the last sealed group are still held
+    op.flush()
+    assert pa.total_allocated_bytes() == base
+    assert op.stats()["rows_in"] == 40 * 1000
+    op.close()
+
+
+@pytest.mark.gpu
 def test_null_out_is_refused_except_by_on_close():
     op = _new("updating")
     for name, call in _entry_points(op._lib).items():

@@ -482,9 +482,9 @@ def test_avg_only_and_avg_with_min_max(G):
         assert_same(want, got, float_cols=("avg",))
 
 
-def test_pinned_host_batches_are_read_in_place(G):
-    """FLAG_ZERO_COPY: Arrow buffers in page-locked memory are read in place (no staging memcpy); results
-    and the release of every input batch are the same as for staged buffers."""
+def test_zero_copy_flag_is_accepted_with_the_same_results(G):
+    """FLAG_ZERO_COPY is accepted and ignored: Arrow buffers in page-locked memory are staged like any other host
+    batch, and the results are the oracle's."""
     import pyarrow as pa
     import torch
     import arroyo_b200 as ab
