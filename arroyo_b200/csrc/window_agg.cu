@@ -306,10 +306,16 @@ __device__ __forceinline__ unsigned long long group_reduce(int kind, unsigned pe
 // keys (Nexmark: 75 % of the bids on the hot bidder) would otherwise serialise tens of millions of REDs on
 // one L2 address; unkeyed aggregates hit a single address by construction.  The neighbour test keeps the
 // common case (all ids distinct) at two shuffles and a vote.
+//
+// The group key: a fast lane's is (id << 32) | low word of its pane number, a non-fast lane's is (~0u << 32) | lane.
+// Fast ids are below ID_OVERFLOW = 0xFFFFFFFE, so no fast key has the non-fast high word, and non-fast lanes never
+// group with anything.  A fast lane's pane is resident, resident panes hold distinct ring slots q mod R, and R divides
+// 2^32: the low word names the pane exactly.
 template <int NV, int SIG>
 __device__ __forceinline__ void combine_accumulate(const IngestParams& p, const PaneCache& pc, bool fast, uint32_t id,
                                                    const Vals& v, int lane) {
-  const unsigned long long gkey = fast ? ((unsigned long long)id | (pc.q << 32)) : (0xFFFFFFFF00000000ull | (unsigned)lane);
+  const unsigned long long gkey =
+      fast ? (((unsigned long long)id << 32) | (uint32_t)pc.q) : (0xFFFFFFFF00000000ull | (unsigned)lane);
   const unsigned long long nb = __shfl_xor_sync(0xffffffffu, gkey, 1);
   if (!__any_sync(0xffffffffu, fast && nb == gkey)) {
     if (fast) accumulate<NV, SIG>(p, v, pc.ptr, id);

@@ -322,9 +322,9 @@ def device_rows(wins, names):
     return rows
 
 
-def run_gpu(st, kind, cfg, entry, expected_keys=0):
-    """The CUDA operator on the same events.  Returns (one list of output rows per watermark, rows_in, rows_late,
-    n_keys of the last operator).
+def run_gpu(st, kind, cfg, entry, expected_keys=0, flags=0):
+    """The CUDA operator on the same events, with operator flags `flags` added to those of `kind` and `entry`.  Returns
+    (one list of output rows per watermark, rows_in, rows_late, n_keys of the last operator).
     `poll_host` feeds device batches and alternates the watermarks between the host call (even ones) and the device
     begin / poll pair (odd ones), so host emissions and checkpoints follow device emissions of any size."""
     import torch
@@ -333,7 +333,7 @@ def run_gpu(st, kind, cfg, entry, expected_keys=0):
     from arroyo_b200 import ffi, operators as native
     from arroyo_b200.context import clamp_watermark
     from tests.gpu_ops import from_arrow, to_arrow
-    flags = {"running": 0, "remerge": ffi.FLAG_REMERGE_ONLY, "tumbling": 0}[kind]
+    flags |= {"running": 0, "remerge": ffi.FLAG_REMERGE_ONLY, "tumbling": 0}[kind]
     flags |= {"two_pass": ffi.FLAG_TWO_PASS_ALWAYS, "one_pass": ffi.FLAG_NO_TWO_PASS}.get(entry, 0)
     cls = native.TumblingAggregatingWindowFunc if kind == "tumbling" else native.SlidingAggregatingWindowFunc
     first = next(ev[1] for ev in st.events if ev[0] == "batch")
